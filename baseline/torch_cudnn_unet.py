@@ -1,11 +1,11 @@
 """LIBRARY BASELINE — not part of the product path (nothing under open-solution-mapping-challenge_b200/ imports it).
 
-"The baseline to beat on the same box" (BASELINE.md 3.4, SURVEY.md 2.3): the reference's network
-(/root/reference/src/unet_models.py:338-403: torchvision ResNet encoder, DecoderBlockV2 with ConvTranspose2d(4, 2, 1),
-ConvRelu, 1x1 classifier) and train step (/root/reference/src/steps/pytorch/models.py:76-113 with
-PyTorchUNetWeighted's loss, /root/reference/src/models.py:310-454) written with STOCK PyTorch modules and run the way a
+"The baseline to beat on the same box" (SURVEY.md 2.3): the reference's network
+(src/unet_models.py:338-403: torchvision ResNet encoder, DecoderBlockV2 with ConvTranspose2d(4, 2, 1),
+ConvRelu, 1x1 classifier) and train step (src/steps/pytorch/models.py:76-113 with
+PyTorchUNetWeighted's loss, src/models.py:310-454) written with STOCK PyTorch modules and run the way a
 PyTorch user would run it on this GPU today: cuDNN / cuBLAS kernels, channels_last, bf16 autocast, torch.optim.Adam
-(fused).  /root/reference does not exist on the GPU box and its torch-0.3 idioms (Variable, reduce=False) add nothing
+(fused).  The reference itself is not imported: its torch-0.3 idioms (Variable, reduce=False) add nothing
 but deprecation shims, hence the restatement; the module tree and state_dict keys are the reference's."""
 import torch
 import torch.nn.functional as F

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200 hot path (contract in the task statement, section 4).
+"""bench.py — headline benchmark of the H100 hot path.
 
   python bench.py --gpus N --steps K --warmup W          our arm: ResNet101-UNet train step, batch 32/GPU, 300x300
                                                           tiles replicate-padded to the 320x320 net input
@@ -11,7 +11,12 @@
                                                           batch 64, host images in -> host label maps out
 
 One JSON line on stdout (rank 0).  `value` = tiles/s with inputs resident in HBM; `e2e` = the same metric through the
-reference-facing API (PyTorchUNetWeighted._fit_loop on pinned HOST batches, loss read back every step)."""
+reference-facing API (PyTorchUNetWeighted._fit_loop on pinned HOST batches, loss read back every step).
+
+  --dump-outputs DIR   (train workload) after the timed steps, write what they computed as DIR/<name>.npy (float32 /
+                       float64): the last step's loss and a fixed, seeded sample of the trained fp32 parameters.  Inputs
+                       and initial weights are seeded, so two builds run with the same arguments compare output for
+                       output."""
 import argparse
 import json
 import os
@@ -28,7 +33,7 @@ FLOP_PER_TILE = {(101, 320): 205.71e9, (101, 256): 131.7e9, (34, 256): 79.54e9, 
 
 
 def unet_config(encoder, lr=5e-4):
-    """the `config.unet` dict of /root/reference/src/pipeline_config.py:61-120 (values from neptune.yaml)"""
+    """the `config.unet` dict of the reference's src/pipeline_config.py:61-120 (values from neptune.yaml)"""
     return {
         'architecture_config': {
             'model_params': {'n_filters': 16, 'conv_kernel': 3, 'pool_kernel': 3, 'pool_stride': 2, 'repeat_blocks': 4,
@@ -51,7 +56,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d.get("bf16_tflops_sustained", d.get("bf16_tflops")), d.get("hbm_gbs"), "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, "data sheet (H100 SXM, dense BF16 / HBM3, at 700 W)"
 
 
 class ClockSampler:
@@ -376,7 +381,7 @@ def infer_line(args, dev, rank, world):
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": round(ms_dev, 4), "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None, "dtype": "bf16 (network) / f32, u8, i32 (post-processing)", "data": "synthetic",
         "config": {"workload": infer_workload_name(args), "global_batch": tiles, "parallelism": "dp%d replicas" % world,
-                   "l2": "the batch's maps (92 MB of probabilities + labels, GBs of activations) exceed the 126 MB L2"},
+                   "l2": "the batch's maps (92 MB of probabilities + labels, GBs of activations) exceed the 50 MB L2"},
         "e2e": {"value": round(tiles / (ms_e2e * 1e-3), 2), "unit": "tiles/s", "ms_per_step": round(ms_e2e, 4),
                 "h2d_bytes_per_step": int(Xh.numel() * 4), "d2h_bytes_per_step": d2h,
                 "api": "PyTorchUNet net forward on pinned host images -> MaskPostprocessor + dense_crf_batch + "
@@ -393,7 +398,7 @@ def infer_line(args, dev, rank, world):
                      "frac": round(b * POST_BYTES_PER_IMAGE / (chain_ms * 1e-3) / 1e9 / peak_hbm, 4) if chain_ms else None,
                      "traffic": None, "peak_source": peak_src,
                      "what": "reference post-processing chain of one batch: 1.44 MB/image algorithmic (SURVEY.md 8d) / its "
-                             "device time; per-kernel DRAM bytes and durations: profiles/r02_postproc_ncu.md"},
+                             "device time"},
     }
     plan = net.module.plan(b, s, s, False) if hasattr(net, "module") else net.plan(b, s, s, False)
     line["gpu_launches"] = (plan.launches_fwd + 40) * args.steps
@@ -487,6 +492,23 @@ def emit(line):
         os.write(_REAL_STDOUT, data)
 
 
+DUMP_PARAM_SAMPLE = 1 << 20   # parameters written by --dump-outputs (4 MB of float32)
+
+
+def dump_train_outputs(out_dir, loss, p32):
+    """the timed path's results: the loss of its last step and the fp32 master parameters it trained, sampled at
+    seeded positions (the same positions for every run of the same network)"""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().double().cpu().numpy().reshape(-1))
+    n = p32.numel()
+    g = torch.Generator().manual_seed(1234)
+    idx = torch.randperm(n, generator=g)[:DUMP_PARAM_SAMPLE].sort().values if n > DUMP_PARAM_SAMPLE else torch.arange(n)
+    np.save(os.path.join(out_dir, "params_sample.npy"), p32.detach().reshape(-1)[idx.to(p32.device)].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "params_sample_index.npy"), idx.double().numpy())
+
+
 def main():
     global _REAL_STDOUT
     sys.stdout.flush()
@@ -504,7 +526,11 @@ def main():
     ap.add_argument("--size", type=int, default=320)
     ap.add_argument("--no-breakdown", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="train workload: write the last timed step's loss and a seeded parameter sample as DIR/*.npy")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "train" or args.impl != "ours"):
+        raise SystemExit("--dump-outputs writes the outputs of the train workload of impl ours")
     if args.batch is None:
         args.batch = 64 if args.workload == "infer" else 32
     args.warmup = max(args.warmup, 3) if args.impl != "reference" else args.warmup
@@ -613,13 +639,15 @@ def main():
     ms_dev = timed(step_dev, args.steps)
     clocks = sampler.stop() if sampler else None
     loss_dev = float(last["loss"])
+    if args.dump_outputs and rank == 0:
+        dump_train_outputs(args.dump_outputs, last["loss"], model._net()._p32)
     note("device arm timed: %.3f ms/step" % ms_dev)
 
     # ---- end-to-end arm: pinned host batches in, loss read back EVERY step.  One step of pipelining: the D2H copy of
     # step i's loss is enqueued (into pinned memory, followed by an event) right behind step i, and the host consumes it
     # after it has enqueued step i+1 -- so the H2D copy of the next batch and the host-side launch work overlap compute.
     # (A plain loss.cpu() of the previous step would be stream-ordered behind the step just enqueued and stall the host
-    # for a whole step: tools/dbg_e2e.py.)
+    # for a whole step.)
     loss_host = [torch.zeros(1, dtype=torch.float32).pin_memory() for _ in range(2)]
     loss_ev = [torch.cuda.Event() for _ in range(2)]
     prev = {"i": 0, "pending": False}
@@ -686,7 +714,7 @@ def main():
                    "grad_allreduce": ("in-graph, per arena segment, overlapped with the backward pass" if fused.inline_allreduce
                                       else "one call after the backward graph") if world > 1 else None,
                    "replicas_in_sync": in_sync,
-                   "l2": "per-step working set (activations + gradients, GBs) far exceeds the 126 MB L2; no flush needed",
+                   "l2": "per-step working set (activations + gradients, GBs) far exceeds the 50 MB L2; no flush needed",
                    "loss_last_step": loss_dev},
         "e2e": {"value": round(e2e, 2), "unit": "tiles/s", "ms_per_step": round(ms_e2e, 4),
                 "h2d_bytes_per_step": int(Xh.numel() * 4 + Th.numel() * 4), "d2h_bytes_per_step": 4,
@@ -696,21 +724,9 @@ def main():
         "clocks": clocks,
         "roofline": {"bound": "tensor", "achieved": round(achieved, 1), "peak": peak_tf, "unit": "TFLOP/s",
                      "frac": round(achieved / peak_tf, 4), "traffic": None, "peak_source": peak_src,
-                     "what": "conv/convT fwd+dgrad+wgrad tcgen05 GEMM family: algorithmic conv FLOPs of the step "
+                     "what": "conv/convT fwd+dgrad+wgrad wgmma GEMM family: algorithmic conv FLOPs of the step "
                              "(%.2f GFLOP/tile) / whole-step time per GPU" % (fpt / 1e9)},
     }
-    # DRAM traffic of the GEMM family over one step, from the committed ncu capture of this same workload (a number
-    # taken under the profiler is evidence, not a bench value): compare with the family's algorithmic bytes
-    tj = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "r02_gemm_traffic.json")
-    if not os.path.exists(tj):
-        tj = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "r01c_gemm_traffic.json")
-    if (args.encoder, args.batch, args.size) == (101, 32, 320) and os.path.exists(tj):
-        with open(tj) as f:
-            tr = json.load(f)
-        line["roofline"]["traffic"] = int(tr["dram_bytes"])
-        line["roofline"]["traffic_unit"] = "DRAM bytes per step per GPU, summed over the family's %d launches " \
-                                           "(ncu dram__bytes_read.sum + dram__bytes_write.sum, cold-cache replay)" % tr["launches"]
-        line["roofline"]["traffic_source"] = "profiles/" + os.path.basename(tj)
     if not args.no_breakdown:
         bd, total = breakdown(fused)
         note("breakdown done")
@@ -724,7 +740,7 @@ def main():
         line["roofline"]["gemm_family_algorithmic_bytes"] = int(sum((v["algo_gbs"] or 0) * v["ms"] * 1e6 for v in gemm))
     if not args.no_library_baseline and world == 1:
         # the stock-PyTorch (cuDNN) train step of the same net on the same GPU, measured right here: the library
-        # baseline this framework has to beat (BASELINE.md 3.4)
+        # baseline this framework has to beat
         del Xh, Th
         lb = library_baseline(args, dev, Xd, Td, steps=min(args.steps, 10), warmup=3)
         line["library_baseline"] = lb

@@ -1,8 +1,8 @@
-/* mcb200.h — C ABI of libmcb200.so: the B200 (sm_100a) hot path of neptune-ai/open-solution-mapping-challenge.
+/* mcb200.h — C ABI of libmcb200.so: the H100 (sm_90a) hot path of neptune-ai/open-solution-mapping-challenge.
  *
  * The reference is 100 % Python; every FLOP of its hot path runs inside torch 0.3.1 / cuDNN / scipy / skimage /
  * pydensecrf calls.  This header is what a Python host binds (ctypes, see INTEGRATION.md) in place of those library
- * calls.  Each entry point cites the reference call site it replaces as  file:line  under /root/reference.
+ * calls.  Each entry point cites the reference call site it replaces as  file:line  of the reference repository.
  *
  * Conventions
  *   - every function returns 0 on success, a negative MCB_ERR_* code on failure; mcb_last_error() returns a
@@ -35,7 +35,7 @@ int mcb_version(void);
 int mcb_zero_bytes(void* p, size_t bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
- * Convolutions as tcgen05 implicit GEMMs (TMA-fed, TMEM accumulators).
+ * Convolutions as wgmma implicit GEMMs (TMA-fed, register accumulators).
  * Replaces nn.Conv2d / nn.ConvTranspose2d forward + autograd backward at
  *   src/unet_models.py:21-34 (conv3x3, ConvRelu), :125-150 (DecoderBlockV2), :360-383 (encoder stages, final),
  *   torchvision/models/resnet.py BasicBlock / Bottleneck (used at src/unet_models.py:344-352).

@@ -1,5 +1,5 @@
-"""B200-native hot path of neptune-ai/open-solution-mapping-challenge: ResNet-encoder U-Net forward/backward, the
-weighted-CE + Dice loss and the per-pixel mask post-processing, as hand-written sm_100a CUDA behind a C ABI
+"""H100-native hot path of neptune-ai/open-solution-mapping-challenge: ResNet-encoder U-Net forward/backward, the
+weighted-CE + Dice loss and the per-pixel mask post-processing, as hand-written sm_90a CUDA behind a C ABI
 (libmcb200.so, include/mcb200.h).  The Python modules mirror the reference's plugin surface:
 
     mcb200.unet_models.UNetResNet          <- src/unet_models.py:315-403

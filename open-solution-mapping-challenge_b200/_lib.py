@@ -7,7 +7,7 @@ LIB_PATH = os.path.join(_HERE, "libmcb200.so")
 
 if not os.path.exists(LIB_PATH):
     raise ImportError(
-        "libmcb200.so not built: run `python __graft_entry__.py` (nvcc, sm_100a). There is no CPU fallback.")
+        "libmcb200.so not built: run `python __graft_entry__.py` (nvcc, sm_90a). There is no CPU fallback.")
 
 lib = C.CDLL(LIB_PATH)
 lib.mcb_last_error.restype = C.c_char_p

@@ -1,10 +1,11 @@
 // conv_gemm.cu — host side of the convolution family: decomposes each conv / transposed conv / gradient into
-// taps + phases, picks pixel tiles, encodes the TMA tensor maps and launches the tcgen05 kernels of conv_gemm.cuh.
+// taps + phases, picks pixel tiles, encodes the TMA tensor maps and launches the wgmma kernels of conv_gemm.cuh.
 // Exposed through the C ABI declared in include/mcb200.h.
 #include "host_common.h"
 #include "conv_gemm.cuh"
 #include "../../include/mcb200.h"
 #include <algorithm>
+#include <mutex>
 #include <stdlib.h>
 
 namespace mcb {
@@ -71,8 +72,9 @@ static int launch_conv(int BN, int BK, bool b_mn, ConvGemmParams& p, int m_tiles
   const int stage = halo ? b_bytes : a_bytes + b_bytes;
   const int out_bufs = BN <= 64 ? 4 : (BN == 128 ? 2 : 1);
   const int out_bytes = out_bufs * 128 * BN * 2;
-  const int stat_bytes = 16 * 1024;  // two halves x 8 KB reduction scratch
-  const int fixed = out_bytes + stat_bytes + 1024 /*align*/ + 1536 /*barriers, row tables*/ + (halo ? 2 * a_bytes : 0);
+  const int aux_bytes = p.aux_mode != 0 ? 2 * 128 * (BN >= 64 ? 64 : 32) * 2 : 0;  // one aux chunk per MMA warpgroup
+  const int fixed = out_bytes + aux_bytes + kStatBytes + 1024 /*align*/ + 1536 /*barriers, row table*/ +
+                    (halo ? 2 * a_bytes : 0);
   const int budget = std::min(env_int("MCB_SMEM_BUDGET_KB", 227) * 1024, 232448);
   int stages = std::max(2, std::min(env_int("MCB_MAX_STAGES", halo ? 9 : 6), (budget - fixed) / stage));
   if (p.b_resident) {
@@ -85,23 +87,45 @@ static int launch_conv(int BN, int BK, bool b_mn, ConvGemmParams& p, int m_tiles
   const size_t smem = (size_t)stages * stage + fixed;
   const long total = (long)m_tiles * n_tiles * phases;
   dim3 grid((unsigned)std::min<long>(total, num_sms()), 1, 1);
+  const int nch = n_tiles * BN;  // N extent of this launch, channels p.n_off ..
+  const bool red = p.stats != nullptr || p.aux_mode == 2 || (p.aux_mode == 1 && p.bn_dbeta != nullptr);
+  p.red_stride = 2 * nch;
+  if (red && (long)grid.x * p.red_stride > kConvRedCap)
+    return fail(MCB_ERR_UNSUPPORTED, "conv: reduction rows %u x %d exceed the workspace", grid.x, p.red_stride);
+  int r;
   if (halo) {
-    if (BK == 64) return b_mn ? launch_conv_bn<64, true, true>(BN, p, grid, smem, st) : launch_conv_bn<64, false, true>(BN, p, grid, smem, st);
-    return b_mn ? launch_conv_bn<32, true, true>(BN, p, grid, smem, st) : launch_conv_bn<32, false, true>(BN, p, grid, smem, st);
+    if (BK == 64) r = b_mn ? launch_conv_bn<64, true, true>(BN, p, grid, smem, st) : launch_conv_bn<64, false, true>(BN, p, grid, smem, st);
+    else r = b_mn ? launch_conv_bn<32, true, true>(BN, p, grid, smem, st) : launch_conv_bn<32, false, true>(BN, p, grid, smem, st);
+  } else {
+    if (BK == 64) r = b_mn ? launch_conv_bn<64, true, false>(BN, p, grid, smem, st) : launch_conv_bn<64, false, false>(BN, p, grid, smem, st);
+    else r = b_mn ? launch_conv_bn<32, true, false>(BN, p, grid, smem, st) : launch_conv_bn<32, false, false>(BN, p, grid, smem, st);
   }
-  if (BK == 64) return b_mn ? launch_conv_bn<64, true, false>(BN, p, grid, smem, st) : launch_conv_bn<64, false, false>(BN, p, grid, smem, st);
-  return b_mn ? launch_conv_bn<32, true, false>(BN, p, grid, smem, st) : launch_conv_bn<32, false, false>(BN, p, grid, smem, st);
+  if (r || !red) return r;
+  // per-channel sums of the CTAs' rows, in CTA order (detsum.cuh)
+  const int rows = (int)grid.x;
+  if (p.aux_mode == 0) {
+    launch_pdl(conv_red_finish_kernel, det_finish_grid(2L * nch), kDetFinishThreads, 0, st, 0L, rows,
+               (long)p.red_stride, 2L * nch, (long)nch, p.stats + p.n_off, (long)p.stats_c);
+  } else {
+    launch_pdl(conv_red_finish_kernel, det_finish_grid(nch), kDetFinishThreads, 0, st, 0L, rows, (long)p.red_stride,
+               (long)nch, (long)nch, p.bn_dbeta + p.n_off, 0L);
+    if (p.aux_mode == 2)
+      launch_pdl(conv_red_finish_kernel, det_finish_grid(nch), kDetFinishThreads, 0, st, (long)nch, rows,
+                 (long)p.red_stride, (long)nch, (long)nch, p.bn_dgamma + p.n_off, 0L);
+  }
+  MCB_LAUNCH_CHECK();
+  return MCB_OK;
 }
 
 // haloed 3x3 path: worth it when 8x16 single-image tiles cover the image without much waste
-// k_channels = channels per tap of the GEMM-K dimension.  Sweep (gpurun r1, tools/sweep_gemm.py): the haloed tile wins
-// ~9% where the nine per-tap fetches made the kernel L2-bound (>= 128 channels on large images whose extent the 8x16
-// tile divides), and loses on thin layers (the per-tile issue cost dominates) and on ragged small images.
-// MCB_HALO: 0 never, 1 whenever the tile covers >= 80% (old behaviour), 2 (default) the measured-win rule.
+// k_channels = channels per tap of the GEMM-K dimension.  The haloed tile saves the nine per-tap fetches where they make
+// the kernel L2-bound (>= 128 channels on large images whose extent the 8x16 tile divides); on thin layers the
+// per-tile issue cost dominates and ragged small images waste rows.
+// MCB_HALO: 0 never, 1 whenever the tile covers >= 80%, 2 (default) the rule above.
 static bool use_halo(int ksize, int stride, int W, int H, int k_channels) {
   const int mode = env_int("MCB_HALO", 2);
   if (ksize != 3 || stride != 1 || mode == 0) return false;
-  // experimental (MCB_BRES=1, not yet run on hardware): one-chunk layers (32 / 64 channels) take the haloed tile with
+  // experimental (MCB_BRES=1, off by default): one-chunk layers (32 / 64 channels) take the haloed tile with
   // RESIDENT weights -- one TMA load and 18 / 36 back-to-back MMAs per tile instead of 18 loads and 9 barrier waits
   if (env_int("MCB_BRES", 0) == 1 && k_channels <= 64 && W % 8 == 0 && H % 16 == 0) return true;
   if (mode == 2) return k_channels >= env_int("MCB_HALO_MINC", 128) && W % 8 == 0 && H % 16 == 0 && W >= 80;
@@ -116,9 +140,8 @@ static int pick_bn(int n_total, long m_tiles, int phases) {
   }
   // keep the machine filled when the pixel dimension is small
   const long sms = num_sms();
-  // (fat tiles beat many thin ones: go below 128 only when even 128-wide tiles leave most SMs idle)
-  // (measured, gpurun r2 sweep: at 100 pixel tiles -- layer3's 20x20 maps -- ONE round of 256-wide tiles beats two
-  // rounds of 128-wide ones by 7-15 %; at 25 pixel tiles the 128-wide split wins 25 %: switch below ~0.6 of a wave)
+  // (fat tiles beat many thin ones: go below 128 only when even 128-wide tiles leave most SMs idle; one round of
+  // 256-wide tiles beats two rounds of 128-wide ones until the tile count falls below ~0.6 of a wave)
   if (bn > 128 && m_tiles * phases * (n_total / bn) * 10 < sms * env_int("MCB_BN256_MIN_WAVE_X10", 6)) bn = 128;
   if (bn > 64 && n_total % 64 == 0 && m_tiles * phases * (n_total / bn) < sms / 3) bn = 64;
   int forced = env_int("MCB_FORCE_BN", 0);
@@ -453,6 +476,26 @@ static int launch_wgrad_inst(const WgradParams& p, dim3 grid, size_t smem, cudaS
   return MCB_OK;
 }
 
+// Region of g_wgrad_red for launches on stream st.  Launches of one stream are serialised; launches of different
+// streams may overlap, so each stream keeps its own region (the kWgradRegions most recently used streams do; a step
+// uses two streams at a time).
+static long wgrad_region_offset(cudaStream_t st) {
+  static std::mutex mu;
+  static cudaStream_t owner[kWgradRegions];
+  static unsigned long last_use[kWgradRegions];
+  static unsigned long clock = 0;
+  std::lock_guard<std::mutex> lock(mu);
+  ++clock;
+  int r = 0;
+  for (int i = 0; i < kWgradRegions; ++i) {
+    if (last_use[i] != 0 && owner[i] == st) { r = i; break; }
+    if (last_use[i] < last_use[r]) r = i;   // otherwise: the least recently used region
+  }
+  owner[r] = st;
+  last_use[r] = clock;
+  return (long)r * kWgradRegionCap;
+}
+
 static int launch_wgrad(WgradParams& p, int cin_src, cudaStream_t st) {
   int BN = 32;
   for (int cand : {256, 128, 64, 32})
@@ -462,18 +505,15 @@ static int launch_wgrad(WgradParams& p, int cin_src, cudaStream_t st) {
   // split-K over the pixel tiles so the grid covers the machine a few times
   // Every split adds a full fp32 output tile with red.add (atomic traffic = splits x |dW|), while the operand
   // streams are L2/HBM-bound and want every SM busy.  So: exactly ONE resident wave of CTAs (never a ragged second
-  // wave) and at least `min_kb` K blocks per CTA (sweep: tools/sweep_gemm.py, gpurun_out/sweep1.log).
+  // wave; the 384-thread CTA takes the whole register file, one CTA per SM) and at least `min_kb` K blocks per CTA.
   const long base = (long)m_tiles * n_tiles * p.ntaps;
-  const int b_cw0 = BN >= 64 ? 64 : 32;
-  const int stage0 = 2 * 64 * 128 + (BN / b_cw0) * 64 * b_cw0 * 2;
-  const int ctas_per_sm = std::max(1, std::min(2, (227 * 1024) / (2 * stage0 + 2048)));
-  const long cap = (long)num_sms() * ctas_per_sm * env_int("MCB_WGRAD_WAVES_X10", 10) / 10;
+  const long cap = (long)num_sms() * env_int("MCB_WGRAD_WAVES_X10", 10) / 10;
   int splits = (int)std::max(1L, std::min((long)p.tiles_total, cap / std::max(1L, base)));
   const int min_kb = env_int("MCB_WGRAD_MIN_KB", 6);
   splits = std::max(1, std::min(splits, std::max(1, p.tiles_total / min_kb)));
   // short reductions (deep layers: few pixel tiles, many weights) are bound by the fp32 red.add epilogues, not by the
-  // operand streams: aim for `kb_target` K blocks per CTA, but keep at least 0.4 of a wave busy (tuned on the full
-  // step, where these GEMMs share the SMs with the BatchNorm-backward kernels: profiles/r01c_env_sweeps.log)
+  // operand streams: aim for `kb_target` K blocks per CTA, but keep at least 0.4 of a wave busy (on the full step
+  // these GEMMs share the SMs with the BatchNorm-backward kernels)
   const int kb_target = env_int("MCB_WGRAD_KB_TARGET", 64);
   if (kb_target > 0) {
     const long lo_cap = cap * env_int("MCB_WGRAD_MIN_WAVE_X10", 4) / 10;
@@ -483,20 +523,33 @@ static int launch_wgrad(WgradParams& p, int cin_src, cudaStream_t st) {
   }
   int forced = env_int("MCB_WGRAD_SPLITS", 0);
   if (forced > 0) splits = std::min(forced, p.tiles_total);
+  // several splits store their partial products in split-ordered rows of the workspace (summed deterministically below)
+  p.cin_src = cin_src;
+  p.slice = (long)p.ntaps * p.cout * cin_src;
+  if (splits > 1) splits = (int)std::max(1L, std::min((long)splits, kWgradRegionCap / p.slice));
+  p.ws_off = splits > 1 ? wgrad_region_offset(st) : 0;
   p.splits = splits;
   const int b_cw = BN >= 64 ? 64 : 32;
   const int stage = 2 * 64 * 128 + (BN / b_cw) * 64 * b_cw * 2;
-  const int budget = env_int("MCB_SMEM_BUDGET_KB", 110) * 1024;
+  const int budget = env_int("MCB_SMEM_BUDGET_KB", 227) * 1024;
   const int per = (p.tiles_total + splits - 1) / splits;
   p.stages = std::max(2, std::min(std::min(per, 8), budget / stage));
   const size_t smem = (size_t)p.stages * stage + 1024 + 512;
   dim3 grid(n_tiles, m_tiles, p.ntaps * splits);
+  int r;
   switch (BN) {
-    case 256: return launch_wgrad_inst<256>(p, grid, smem, st);
-    case 128: return launch_wgrad_inst<128>(p, grid, smem, st);
-    case 64: return launch_wgrad_inst<64>(p, grid, smem, st);
-    default: return launch_wgrad_inst<32>(p, grid, smem, st);
+    case 256: r = launch_wgrad_inst<256>(p, grid, smem, st); break;
+    case 128: r = launch_wgrad_inst<128>(p, grid, smem, st); break;
+    case 64: r = launch_wgrad_inst<64>(p, grid, smem, st); break;
+    default: r = launch_wgrad_inst<32>(p, grid, smem, st); break;
   }
+  if (r || splits == 1) return r;
+  // the splits that own pixel tiles, summed in split order into dW[tap][cout][ci_off + ci] (detsum.cuh)
+  const int rows = (p.tiles_total + per - 1) / per;
+  launch_pdl(wgrad_red_finish_kernel, det_finish_grid(p.slice), kDetFinishThreads, 0, st, p.ws_off, rows, p.slice, p.slice,
+             (long)cin_src, p.dw + p.ci_off, (long)p.cin_total);
+  MCB_LAUNCH_CHECK();
+  return MCB_OK;
 }
 
 static int wgrad_common_setup(WgradParams& p, int Wv, int Hv, int N, int cout, int cin_src) {

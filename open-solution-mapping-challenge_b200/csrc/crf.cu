@@ -14,8 +14,8 @@
 // iteration), so the tap body is cut to the bone:
 //   * every thread owns FOUR vertically adjacent outputs and walks the 16 source rows they share, so each staged
 //     pixel is loaded once for up to four taps; lanes run along x (conflict-free 16-byte shared-memory loads);
-//   * the four outputs are processed as two PAIRS in packed fp32x2 instructions (FADD2 / FFMA2): colour difference,
-//     squared distance and both class accumulations cost 8 packed instructions + 2 MUFU.EX2 per pair of taps;
+//   * the four outputs are processed as two PAIRS (f2 helpers below): colour difference, squared distance and both
+//     class accumulations cost 16 FADD / FFMA + 2 MUFU.EX2 per pair of taps;
 //   * colours are pre-scaled by sqrt(log2(e) / (2 srgb^2)) and the horizontal spatial weight enters as an addend of the
 //     exponent, so one ex2 yields the complete horizontal x colour weight; the vertical weight multiplies the row sum;
 //   * out-of-image pixels are staged with a far-away colour (weight underflows to exactly 0) -- no per-tap branch;
@@ -34,8 +34,7 @@ constexpr int CRF_T = 32;                 // outputs per CTA edge
 constexpr int CRF_S = CRF_T + 2 * CRF_R;  // staged tile edge (44)
 constexpr int CRF_ROWS = 4;               // outputs per thread (vertical)
 constexpr int CRF_THREADS = CRF_T * (CRF_T / CRF_ROWS);   // 256
-// 73 KB per CTA -> three CTAs per SM (the first version kept Q*n_b duplicated as float4: 104 KB, two CTAs, 24 % warp
-// occupancy in the ncu capture profiles/r02_ncu_full_summary.md)
+// 73 KB per CTA -> three CTAs per SM within the 227 KB of shared memory an SM offers
 constexpr size_t CRF_SMEM = (size_t)CRF_S * CRF_S * (sizeof(float4) + sizeof(float2) + sizeof(float2)) +
                             (size_t)CRF_S * CRF_T * sizeof(float2);
 
@@ -54,13 +53,14 @@ __global__ void crf_rgb_kernel(const float* __restrict__ img, uint8_t* __restric
   }
 }
 
-// packed fp32x2 helpers (sm_100: FADD2 / FFMA2)
-typedef unsigned long long f2;
-__device__ __forceinline__ f2 pk(float a, float b) { f2 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk(f2 v, float& a, float& b) { asm("mov.b64 {%0,%1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { f2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
-__device__ __forceinline__ f2 sub2(f2 a, f2 b) { f2 r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f2 add2(f2 a, f2 b) { f2 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
+// fp32 pairs: sm_90 has no packed fp32x2 arithmetic, so each helper is two scalar FADD / FFMA with the same
+// round-to-nearest results the packed form gives
+typedef float2 f2;
+__device__ __forceinline__ f2 pk(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void upk(f2 v, float& a, float& b) { a = v.x; b = v.y; }
+__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ f2 sub2(f2 a, f2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ f2 add2(f2 a, f2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float ex2_approx(float x) { float r; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 
 // MODE 0: norms (writes n_g, n_b).  MODE 1: one mean-field iteration.
@@ -144,15 +144,15 @@ __global__ void __launch_bounds__(CRF_THREADS) crf_kernel(const float* __restric
   f2 ex[CRF_D];
 #pragma unroll
   for (int d = 0; d < CRF_D; ++d) ex[d] = pk(c_e1b[d], c_e1b[d]);
-  f2 acc0[2] = {0ull, 0ull}, acc1[2] = {0ull, 0ull};   // MODE 1: class-0 / class-1 messages; MODE 0: acc0 = weight sums
+  f2 acc0[2] = {pk(0.f, 0.f), pk(0.f, 0.f)}, acc1[2] = {pk(0.f, 0.f), pk(0.f, 0.f)};   // MODE 1: class-0 / class-1 messages; MODE 0: acc0 = weight sums
 #pragma unroll 1
   for (int s = 0; s < CRF_D + CRF_ROWS - 1; ++s) {
-    f2 r0[2] = {0ull, 0ull}, r1[2] = {0ull, 0ull};
+    f2 r0[2] = {pk(0.f, 0.f), pk(0.f, 0.f)}, r1[2] = {pk(0.f, 0.f), pk(0.f, 0.f)};
 #pragma unroll
     for (int d = 0; d < CRF_D; ++d) {
       const float4 o = s_rgb[ry + s][lane + d];
       const f2 orr = pk(o.x, o.x), og = pk(o.y, o.y), ob = pk(o.z, o.z);
-      f2 q0p = 0ull, q1p = 0ull;   // (q0, q0), (q1, q1): the register moves ride on the otherwise idle ALU pipe
+      f2 q0p = pk(0.f, 0.f), q1p = pk(0.f, 0.f);   // (q0, q0), (q1, q1)
       if (MODE == 1) {
         const float2 q = s_qb[ry + s][lane + d];
         q0p = pk(q.x, q.x);

@@ -3,6 +3,7 @@
 // All NHWC bf16 kernels move 16 bytes (8 channels) per thread per access; grids are sized in multiples of the SM count.
 #include "host_common.h"
 #include "../../include/mcb200.h"
+#include "detsum.cuh"
 #include <algorithm>
 #include <math.h>
 
@@ -316,6 +317,13 @@ __global__ void __launch_bounds__(256) bn_train_apply_kernel(const uint4* __rest
   }
 }
 
+// per-block partial rows of channel_reduce_kernel ([out0 | out1] over C channels) and final_conv_bwd_kernel ([dW | db]),
+// summed in block order by the finishing kernels (detsum.cuh)
+constexpr long kChannelRedCap = 1024L * 2 * 2048;
+constexpr long kFinalRedCap = 1024L * 66;
+MCB_DET_WORKSPACE(float, g_channel_red, kChannelRedCap, channel_red_finish_kernel)
+MCB_DET_WORKSPACE(float, g_final_red, kFinalRedCap, final_red_finish_kernel)
+
 // Per-channel reductions over NHWC: block = 256 threads = (256 / C8) pixel lanes x C8 channel groups (C8 = C/8 <= 256).
 // MODE 0: sum(x)                                  -> out0                 (bias gradient)
 // MODE 1: g = dy * (y > 0); sum(g), sum(g * xhat) -> out0 (dbeta), out1 (dgamma)   xhat = (z - mean) * invstd
@@ -390,7 +398,8 @@ __global__ void channel_reduce_kernel(const uint4* __restrict__ a, const uint4* 
     if (MODE == 1) r1[threadIdx.x * 8 + j] = s1[j];
   }
   __syncthreads();
-  // threads 0 .. C8*8-1 each own one channel and sum over the pixel lanes
+  // threads 0 .. C8*8-1 each own one channel and sum over the pixel lanes into this block's row
+  float* row = g_channel_red + (size_t)blockIdx.x * 2 * (C8 * 8);
   for (int ch = threadIdx.x; ch < C8 * 8; ch += blockDim.x) {
     const int g = ch / 8, j = ch % 8;
     float t0 = 0.f, t1 = 0.f;
@@ -398,8 +407,8 @@ __global__ void channel_reduce_kernel(const uint4* __restrict__ a, const uint4* 
       t0 += r0[(l * C8 + g) * 8 + j];
       if (MODE == 1) t1 += r1[(l * C8 + g) * 8 + j];
     }
-    atomicAdd(out0 + ch, t0);
-    if (MODE == 1) atomicAdd(out1 + ch, t1);
+    row[ch] = t0;
+    if (MODE == 1) row[C8 * 8 + ch] = t1;
   }
 }
 
@@ -562,11 +571,10 @@ __global__ void final_conv_bwd_kernel(const uint4* __restrict__ x, const float* 
                                       float* __restrict__ dw, float* __restrict__ db, long pixels_per_img,
                                       long pixels, int C, int K) {
   mcb::pdl_prologue();
-  extern __shared__ float sm[];  // K*C weights, then K*C + K block accumulators
+  extern __shared__ float sm[];  // K*C weights, then per warp K*C + K accumulators
   float* sw = sm;
   float* sacc = sm + K * C;
   for (int i = threadIdx.x; i < K * C; i += blockDim.x) sw[i] = w[i];
-  for (int i = threadIdx.x; i < K * C + K; i += blockDim.x) sacc[i] = 0.f;
   __syncthreads();
   const int C8 = C / 8;
   float lw[2][32];  // per-thread partial dW (K <= 2, C <= 32)
@@ -597,7 +605,8 @@ __global__ void final_conv_bwd_kernel(const uint4* __restrict__ x, const float* 
       dx[p * C8 + g] = pack8(o);
     }
   }
-  // warp reduce then block accumulate in shared memory
+  // warp reduce into per-warp slots, then the warps in order into this block's row [dW | db]
+  const int n_acc = K * C + K, wid = threadIdx.x >> 5;
 #pragma unroll
   for (int k = 0; k < 2; ++k) {
 #pragma unroll
@@ -605,17 +614,18 @@ __global__ void final_conv_bwd_kernel(const uint4* __restrict__ x, const float* 
       float v = lw[k][c];
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if ((threadIdx.x & 31) == 0) atomicAdd(&sacc[k * C + c], v);
+      if ((threadIdx.x & 31) == 0) sacc[wid * n_acc + k * C + c] = v;
     }
     float v = lb[k];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) atomicAdd(&sacc[K * C + k], v);
+    if ((threadIdx.x & 31) == 0) sacc[wid * n_acc + K * C + k] = v;
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < K * C + K; i += blockDim.x) {
-    if (i < K * C) atomicAdd(dw + i, sacc[i]);
-    else atomicAdd(db + (i - K * C), sacc[i]);
+  for (int i = threadIdx.x; i < n_acc; i += blockDim.x) {
+    float t = 0.f;
+    for (int w8 = 0; w8 < (int)(blockDim.x >> 5); ++w8) t += sacc[w8 * n_acc + i];
+    g_final_red[(size_t)blockIdx.x * n_acc + i] = t;
   }
 }
 
@@ -780,8 +790,11 @@ extern "C" int mcb_channel_sum(const void* x, float* out, long pixels, int c, vo
   if (int r = reduce_cfg(c, &threads, &c8)) return r;
   const int lanes = threads / c8;
   const int grid = (int)std::max(1L, std::min((pixels + lanes * 4 - 1) / (lanes * 4), (long)num_sms() * 4));
+  MCB_REQUIRE((long)grid * 2 * c <= kChannelRedCap, "channel_sum: %d blocks x %d channels exceed the workspace", grid, c);
   launch_pdl(channel_reduce_kernel<0>, grid, threads, (size_t)threads * 8 * 2 * sizeof(float), ST, 
       (const uint4*)x, nullptr, nullptr, nullptr, nullptr, out, nullptr, pixels, c8);
+  launch_pdl(channel_red_finish_kernel, det_finish_grid(c), kDetFinishThreads, 0, ST, 0L, grid, 2L * c, (long)c,
+             (long)c, out, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -792,8 +805,13 @@ extern "C" int mcb_bn_bwd_reduce(const void* dy, const void* y_mask, const void*
   if (int r = reduce_cfg(c, &threads, &c8)) return r;
   const int lanes = threads / c8;
   const int grid = (int)std::max(1L, std::min((pixels + lanes * 4 - 1) / (lanes * 4), (long)num_sms() * 4));
+  MCB_REQUIRE((long)grid * 2 * c <= kChannelRedCap, "bn_bwd_reduce: %d blocks x %d channels exceed the workspace", grid, c);
   launch_pdl(channel_reduce_kernel<1>, grid, threads, (size_t)threads * 8 * 2 * sizeof(float), ST, 
       (const uint4*)dy, (const uint4*)y_mask, (const uint4*)z, mean, invstd, dbeta, dgamma, pixels, c8);
+  launch_pdl(channel_red_finish_kernel, det_finish_grid(c), kDetFinishThreads, 0, ST, 0L, grid, 2L * c, (long)c,
+             (long)c, dbeta, 0L);
+  launch_pdl(channel_red_finish_kernel, det_finish_grid(c), kDetFinishThreads, 0, ST, (long)c, grid, 2L * c, (long)c,
+             (long)c, dgamma, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -863,8 +881,14 @@ extern "C" int mcb_final_conv_bwd(const void* x, const float* w, const float* dl
   MCB_REQUIRE(x && w && dlogits && dx && dw && db, "final_conv_bwd: null pointer");
   MCB_REQUIRE(c == 32 && k == 2, "final_conv_bwd: only the reference's 32 -> 2 classifier is built");
   const long ppi = (long)h * wd, pixels = ppi * n;
-  launch_pdl(final_conv_bwd_kernel, grid_for(pixels, 128, 4), 128, (size_t)(2 * k * c + k) * sizeof(float), ST, 
+  const int grid = grid_for(pixels, 128, 4), n_acc = k * c + k;
+  MCB_REQUIRE((long)grid * n_acc <= kFinalRedCap, "final_conv_bwd: %d blocks exceed the workspace", grid);
+  launch_pdl(final_conv_bwd_kernel, grid, 128, (size_t)(k * c + 4 * n_acc) * sizeof(float), ST, 
       (const uint4*)x, w, dlogits, (uint4*)dx, dw, db, ppi, pixels, c, k);
+  launch_pdl(final_red_finish_kernel, det_finish_grid(k * c), kDetFinishThreads, 0, ST, 0L, grid, (long)n_acc,
+             (long)(k * c), (long)(k * c), dw, 0L);
+  launch_pdl(final_red_finish_kernel, det_finish_grid(k), kDetFinishThreads, 0, ST, (long)(k * c), grid, (long)n_acc,
+             (long)k, (long)k, db, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }

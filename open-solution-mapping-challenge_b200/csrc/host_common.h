@@ -47,10 +47,10 @@ int num_sms();
 
 // ---- programmatic dependent launch (PDL) -------------------------------------------------------------------------
 // Every kernel of the train step is launched with programmatic stream serialization: the next kernel of the stream may
-// be scheduled (and run its prologue: barrier init, TMEM allocation, descriptor prefetch) while this one drains, and
+// be scheduled (and run its prologue: barrier init, descriptor prefetch) while this one drains, and
 // blocks in griddepcontrol.wait until its predecessors have completed and flushed memory.  Each kernel executes
 // pdl_prologue() before its first global-memory access.  Opt-in with MCB_PDL=1: inside the CUDA-graph replay of the
-// train step it measured 17.39 vs 17.19 ms/step (gpurun r1), so the default launches without the attribute.
+// train step it has not paid off, so the default launches without the attribute.
 bool pdl_enabled();
 
 template <typename... KArgs, typename... Args>

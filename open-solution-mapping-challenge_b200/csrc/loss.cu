@@ -6,6 +6,7 @@
 // (and cross-GPU: all-reduce them between the phases) coupling; phase 2 writes the loss and d(loss)/d(logits).
 #include "host_common.h"
 #include "../../include/mcb200.h"
+#include "detsum.cuh"
 #include <algorithm>
 
 namespace mcb {
@@ -24,6 +25,10 @@ __device__ __forceinline__ float pixel_weight(const LossCfg& cfg, float d, float
   if (s_ == 1.f) ws = 1.f;
   return wd * ws;
 }
+
+// per-block rows of the four loss sums, added in block order by loss_red_finish_kernel (detsum.cuh)
+constexpr long kLossRedCap = 2048L * 4;
+MCB_DET_WORKSPACE(double, g_loss_red, kLossRedCap, loss_red_finish_kernel)
 
 __global__ void loss_partials_kernel(const float* __restrict__ logits, const float* __restrict__ target, LossCfg cfg,
                                      double* __restrict__ sums, long ppi, long pixels, int tch) {
@@ -58,7 +63,7 @@ __global__ void loss_partials_kernel(const float* __restrict__ logits, const flo
   if (threadIdx.x < 4) {
     double t = 0.0;
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += (double)red[threadIdx.x][w];
-    atomicAdd(sums + threadIdx.x, t);
+    g_loss_red[(size_t)blockIdx.x * 4 + threadIdx.x] = t;
   }
 }
 
@@ -140,8 +145,12 @@ extern "C" int mcb_loss_partials(const mcb_loss_args* a, double* sums, void* str
   MCB_REQUIRE(a && a->logits && a->target && sums, "loss_partials: null pointer");
   MCB_REQUIRE(a->mode == 0 || a->mode == 1, "loss: mode %d", a->mode);
   const long ppi = (long)a->h * a->w, pixels = ppi * a->n;
-  launch_pdl(loss_partials_kernel, loss_grid(pixels), 256, 0, static_cast<cudaStream_t>(stream), 
+  const int grid = loss_grid(pixels);
+  MCB_REQUIRE((long)grid * 4 <= kLossRedCap, "loss_partials: %d blocks exceed the workspace", grid);
+  launch_pdl(loss_partials_kernel, grid, 256, 0, static_cast<cudaStream_t>(stream), 
       a->logits, a->target, make_cfg(a), sums, ppi, pixels, a->mode == 0 ? 3 : 1);
+  launch_pdl(loss_red_finish_kernel, det_finish_grid(4), kDetFinishThreads, 0, static_cast<cudaStream_t>(stream), 0L,
+             grid, 4L, 4L, 4L, sums, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }

@@ -13,8 +13,7 @@
 // The partial sums are complete when the kernel starts (stream order behind their producer).  Reuse across steps is
 // safe because a peer can push the next step's values of an exchange only after the gradient all-reduce of this step,
 // which every rank joins after its last exchange.  The step stamp lives in device memory (bumped by a tiny kernel at
-// the start of every forward), so the launches replay unchanged inside CUDA graphs.  (History, gpurun r2 at N=2: pull
-// model with flag handshake 14 us per exchange; push + fence + flag 8 us; stamped pairs -> see DESIGN.md section 5.)
+// the start of every forward), so the launches replay unchanged inside CUDA graphs.
 #include "host_common.h"
 #include "sync.cuh"
 #include "../../include/mcb200.h"

@@ -3,8 +3,8 @@ NHWC bf16 buffers, replayable as CUDA graphs.
 
 Data flow per conv+BN unit in training:  z = conv(a_prev) [+ per-channel sum / sumsq in the GEMM epilogue]
 -> bn_finalize (batch statistics, running-stat update) -> a = relu(z*scale + shift [+ residual]) in one pass.
-Backward mirrors torch autograd of /root/reference/src/unet_models.py:385-403: per unit a reduction
-(dbeta, dgamma with the ReLU mask folded in), one elementwise pass producing dz, then the tcgen05 dgrad and
+Backward mirrors torch autograd of src/unet_models.py:385-403: per unit a reduction
+(dbeta, dgamma with the ReLU mask folded in), one elementwise pass producing dz, then the wgmma dgrad and
 split-K wgrad GEMMs; decoder ReLU masks are applied in the dgrad epilogues; skip-connection gradients are
 accumulated with TMA reduce-add."""
 import os
@@ -41,8 +41,7 @@ def stream_priority_enabled():
     """MCB_STREAM_PRIORITY (default 1): the captured step's main chain runs on a HIGH-priority stream while the backward's
     side stream (weight-gradient GEMMs, Adam segments, all-reduce launches) keeps the default low priority, so the block
     scheduler serves the critical path (data-gradient GEMMs + BatchNorm-backward) first and the side work fills what is
-    left.  Together with launching every weight-gradient GEMM as soon as its operands exist (no deferral) this measured
-    16.50 -> 16.11 ms/step (gpurun r2); either change alone is a loss (16.84 / 17.73)."""
+    left, together with launching every weight-gradient GEMM as soon as its operands exist (no deferral)."""
     return os.environ.get("MCB_STREAM_PRIORITY", "1") == "1"
 
 
@@ -56,7 +55,7 @@ def graph_capture(graph, dev):
 class _OpList(list):
     """list of _Op; .add(kind, fn, flops, bytes)"""
 
-    # profiling aid (tools/knockout.sh): MCB_KNOCKOUT="kind,kind" drops those launches from the plan so that the step-time
+    # profiling aid: MCB_KNOCKOUT="kind,kind" drops those launches from the plan so that the step-time
     # difference gives their in-graph cost (results are garbage; never set outside profiling)
     _knockout = frozenset(k for k in os.environ.get("MCB_KNOCKOUT", "").split(",") if k)
 

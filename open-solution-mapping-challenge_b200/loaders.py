@@ -1,4 +1,4 @@
-"""Test-time augmentation on the device: mirror of /root/reference/src/loaders.py:401-517
+"""Test-time augmentation on the device: mirror of src/loaders.py:401-517
 (TestTimeAugmentationGenerator, TestTimeAugmentationAggregator, test_time_augmentation_transform /
 _inverse_transform, aggregate_augmentations) for the flip / rot90 variants the pipeline configures
 (src/pipeline_config.py:121-127: flip_ud, flip_lr, rotation, no colour shift -> 16 variants per image).
@@ -27,7 +27,7 @@ METHODS = {"gmean": 0, "mean": 1, "max": 2, "min": 3}
 def tta_specs(flip_ud=True, flip_lr=True, rotation=True, color_shift_runs=False):
     """the spec list of TestTimeAugmentationGenerator._get_tta_data (src/loaders.py:413-432) for one image"""
     if color_shift_runs:
-        raise NotImplementedError("colour-shift TTA variants are random imgaug transforms; not built on the B200 path")
+        raise NotImplementedError("colour-shift TTA variants are random imgaug transforms; not built on the H100 path")
     original = {'ud_flip': False, 'lr_flip': False, 'rotation': 0, 'color_shift': False}
     specs = [original]
     ud_options = [True, False] if flip_ud else [False]
@@ -44,7 +44,7 @@ def spec_code(spec):
     """k | flip << 2 as consumed by the kernels.  `if ud_flip ... elif lr_flip` (src/loaders.py:471-474, 489-492): a spec
     with both flips set applies the up-down flip only — kept."""
     if spec.get('color_shift'):
-        raise NotImplementedError("colour-shift TTA variants are not built on the B200 path")
+        raise NotImplementedError("colour-shift TTA variants are not built on the H100 path")
     rot = int(spec['rotation'])
     if rot % 90 != 0:
         raise NotImplementedError("TTA rotations are multiples of 90 degrees (src/loaders.py:417)")

@@ -1,6 +1,6 @@
-"""Mirror of the reference's model transformers (/root/reference/src/models.py:50-209 over
-/root/reference/src/steps/pytorch/models.py:16-171) and losses (/root/reference/src/models.py:310-454,
-/root/reference/src/steps/pytorch/validation.py:8-28) on the B200 path.
+"""Mirror of the reference's model transformers (src/models.py:50-209 over
+src/steps/pytorch/models.py:16-171) and losses (src/models.py:310-454,
+src/steps/pytorch/validation.py:8-28) on the H100 path.
 
 Same constructor (architecture_config, training_config, callbacks_config), same fit / transform / load / save /
 _fit_loop / _transform surface and attributes (.model, .optimizer, .loss_function, .output_names, .callbacks), so
@@ -131,7 +131,7 @@ def callbacks_unet(callbacks_config):
 def release_captured_graphs(transformer):
     """drop every captured CUDA graph / launch plan of a transformer.  Call it before
     torch.distributed.destroy_process_group(): graphs that captured NCCL collectives keep the communicator busy and the
-    teardown waits on them forever (seen on 2 GPUs, gpurun r2)."""
+    teardown waits on them forever."""
     import gc
     transformer._fused = None
     transformer._fused_cache = {}
@@ -150,7 +150,7 @@ def weight_regularization_unet(model, regularize, weight_decay_conv2d):
 
 
 class Model:
-    """src/steps/pytorch/models.py:16-171 (Model) on the B200 path"""
+    """src/steps/pytorch/models.py:16-171 (Model) on the H100 path"""
 
     def __init__(self, architecture_config, training_config, callbacks_config):
         self.architecture_config = architecture_config
@@ -209,7 +209,7 @@ class Model:
 
     def _to_device(self):
         if not torch.cuda.is_available():
-            raise RuntimeError("the B200 path needs a CUDA device; there is no CPU fallback")
+            raise RuntimeError("the H100 path needs a CUDA device; there is no CPU fallback")
         net = self._net()
         if not net._p32.is_cuda:
             params_before = [p for _, p, _ in net._arena_params()]
@@ -329,7 +329,7 @@ class BasePyTorchUNet(Model):
     def set_model(self):
         encoder = self.architecture_config['model_params']['encoder']
         if encoder not in PRETRAINED_NETWORKS:
-            raise NotImplementedError("the B200 path implements the ResNet34/101/152 encoders (got %r)" % (encoder,))
+            raise NotImplementedError("the H100 path implements the ResNet34/101/152 encoders (got %r)" % (encoder,))
         config = PRETRAINED_NETWORKS[encoder]
         self.model = config['model'](**config['model_config'])
         self._initialize_model_weights = lambda: None
@@ -442,8 +442,8 @@ class FusedTrainStep:
         self.launches = None
         self._staging = None
         self.segments = None
-        # opt-in: on 2 GPUs the three smaller all-reduces + graph segmentation cost more than they hide (22.8 vs 22.3
-        # ms/step, gpurun r1); kept for larger worlds / slower fabrics
+        # opt-in: on 2 GPUs the three smaller all-reduces + graph segmentation can cost more than they hide; kept for
+        # larger worlds / slower fabrics
         if self.world > 1 and os.environ.get("MCB_OVERLAP_ALLREDUCE", "2") == "1" and not self.plan.sync_bn:
             self.segments = self.plan.bwd_segments()
             self._comm_stream = torch.cuda.Stream(device=dev)
@@ -452,7 +452,7 @@ class FusedTrainStep:
         # tensor-bound).  Its step-dependent scalars live in a 3-float device tensor refreshed before every replay.
         # multi-GPU default: the all-reduce of a finished arena segment (decoder | layer4 | layer3 | rest) is issued from
         # INSIDE the backward graph, on the side stream behind that segment's weight-gradient GEMMs, and overlaps the
-        # data-gradient chain of the layers below (gpurun r2, N=2: 16.97 vs 17.21 ms/step with one exposed all-reduce).
+        # data-gradient chain of the layers below.
         # MCB_OVERLAP_ALLREDUCE=0 restores the single all-reduce after the backward graph; NCCL-per-BatchNorm SyncBN
         # (MCB_SYNC_BN=1) needs it because its BatchNorm slots are rescaled after the backward pass.
         ov = os.environ.get("MCB_OVERLAP_ALLREDUCE", "2")

@@ -1,5 +1,5 @@
-"""Mirror of the reference's per-pixel post-processing (/root/reference/src/postprocessing.py:48-258,
-/root/reference/src/utils.py:231-273,328-339) on the GPU.
+"""Mirror of the reference's per-pixel post-processing (src/postprocessing.py:48-258,
+src/utils.py:231-273,328-339) on the GPU.
 
 Two surfaces:
   * module-level functions with the reference's names and signatures, one image in / numpy out — drop-ins for

@@ -1,6 +1,6 @@
 """Input side of the path on the GPU (SURVEY.md 8f-4): mirror of the deterministic parts of
-/root/reference/src/loaders.py:141-171,311-317 (image / target tensors of the padded loaders),
-/root/reference/src/augmentation.py:40-86 (PadFixed) and /root/reference/src/preparation.py:151-195 (two-nearest
+src/loaders.py:141-171,311-317 (image / target tensors of the padded loaders),
+src/augmentation.py:40-86 (PadFixed) and src/preparation.py:151-195 (two-nearest
 building distances, component-size map).
 
 Both loader modes are covered: `crop_and_pad` (PadFixed) and `resize` (transforms.Resize on the PIL image = Pillow's

@@ -1,13 +1,13 @@
 """Mirror of the reference's src/unet_models.py for the ResNet-encoder U-Net, executed by libmcb200.so.
 
 `UNetResNet` keeps the reference's constructor, attribute tree and state_dict keys
-(/root/reference/src/unet_models.py:315-403: encoder.*, conv1..conv5 aliases, center/dec5..dec1 `.block.{0.conv,1}`,
+(src/unet_models.py:315-403: encoder.*, conv1..conv5 aliases, center/dec5..dec1 `.block.{0.conv,1}`,
 dec0.conv, final) so reference checkpoints load and src/pipelines.py / src/models.py drive it unchanged, but:
 
   * parameters live in ONE flat fp32 arena in the kernels' tap-major layout ([ky][kx][cout][cin]); every
     nn.Parameter is a (permuted) view of it, gradients are views of a second arena, and a bf16 operand copy of the
     arena feeds the tensor cores;
-  * forward / backward are static launch plans over preallocated NHWC bf16 activations: tcgen05 implicit-GEMM convs
+  * forward / backward are static launch plans over preallocated NHWC bf16 activations: wgmma implicit-GEMM convs
     with fused bias/ReLU/BN-statistics epilogues, fused BN+residual+ReLU passes, concat-free decoder convs, and are
     replayed as CUDA graphs;
   * there is no torch fallback: without the CUDA library or a CUDA input, forward raises.
@@ -41,7 +41,7 @@ class DecoderBlockV2(nn.Module):
         super().__init__()
         self.in_channels = in_channels
         if not is_deconv:
-            raise NotImplementedError("the B200 path implements the configured is_deconv=True decoder "
+            raise NotImplementedError("the H100 path implements the configured is_deconv=True decoder "
                                       "(src/models.py:32-46); the bilinear-upsample variant is not built")
         self.block = nn.Sequential(ConvRelu(in_channels, middle_channels),
                                    nn.ConvTranspose2d(middle_channels, out_channels, kernel_size=4, stride=2, padding=1),
@@ -115,7 +115,7 @@ class UNetResNet(nn.Module):
         total = 0
         slots = {}
         for name, p, kind in params:
-            assert p.dtype == torch.float32, "the B200 path keeps fp32 master weights (got %s for %s)" % (p.dtype, name)
+            assert p.dtype == torch.float32, "the H100 path keeps fp32 master weights (got %s for %s)" % (p.dtype, name)
             s = _Slot()
             s.off, s.numel, s.shape, s.kind = total, p.numel(), tuple(p.shape), kind
             slots[id(p)] = s
@@ -198,9 +198,9 @@ class UNetResNet(nn.Module):
     # ------------------------------------------------------------------------------------------------ forward
     def _check_input(self, x):
         if not isinstance(x, torch.Tensor) or not x.is_cuda:
-            raise RuntimeError("UNetResNet (B200 path) needs a CUDA tensor; there is no CPU fallback")
+            raise RuntimeError("UNetResNet (H100 path) needs a CUDA tensor; there is no CPU fallback")
         if self._p32 is None or not self._p32.is_cuda:
-            raise RuntimeError("UNetResNet (B200 path): call .cuda() on the model first; there is no CPU fallback")
+            raise RuntimeError("UNetResNet (H100 path): call .cuda() on the model first; there is no CPU fallback")
         if x.dim() != 4 or x.shape[1] != 3:
             raise ValueError("expected input (N, 3, H, W), got %s" % (tuple(x.shape),))
         if x.shape[2] % 64 != 0 or x.shape[3] % 64 != 0:

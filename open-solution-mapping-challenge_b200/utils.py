@@ -1,4 +1,4 @@
-"""Instance emission: mirror of /root/reference/src/utils.py:61-127 (decompose, create_annotations, rle_from_binary,
+"""Instance emission: mirror of src/utils.py:61-127 (decompose, create_annotations, rle_from_binary,
 bounding_box_from_rle) on the GPU.
 
 The reference turns every labelled instance into a full-image uint8 mask on the host and hands it to pycocotools

@@ -2,7 +2,7 @@
 Only tests/, __graft_entry__.smoke() and bench.py's CPU legs import this file.
 
 * COCO run-length encoding.  The reference calls pycocotools (`cocomask.encode`, `cocomask.toBbox`,
-  /root/reference/src/utils.py:118-124); pycocotools is NOT installed here and is not vendored in /root/reference
+  src/utils.py:118-124); pycocotools is NOT installed here and is not vendored in the reference
   (requirements.txt: `pycocotools` unpinned, installed from cocodataset/cocoapi PythonAPI, whose C core is
   common/maskApi.c).  The functions below restate maskApi.c's published algorithms — rleEncode (column-major scan,
   alternating run lengths starting with zeros), rleToString (5-bit groups, continuation bit 0x20, sign rule on bit
@@ -10,10 +10,10 @@ Only tests/, __graft_entry__.smoke() and bench.py's CPU legs import this file.
   (including its full-height rule when a run of ones crosses a column boundary).  Pinned by hand-derived vectors in
   tests/test_instances_cpu.py; no reference output exists to pin against -> "pinned to the published algorithm by
   known-answer vectors".
-* Test-time augmentation (/root/reference/src/loaders.py:437-497): pinned against the reference's own functions
+* Test-time augmentation (src/loaders.py:437-497): pinned against the reference's own functions
   through oracle/ref_shim.py, with `skimage.transform.rotate` at multiples of 90 degrees ASSUMED to be the exact
   quarter-turn permutation (np.rot90) — skimage is not installable here.
-* Non-maximum suppression and mask features (/root/reference/src/postprocessing.py:261-386): plain numpy as the
+* Non-maximum suppression and mask features (src/postprocessing.py:261-386): plain numpy as the
   reference writes them; contour length through cv2 (installed) exactly as the reference calls it.
 """
 import numpy as np

@@ -1,7 +1,9 @@
-"""TEST INFRASTRUCTURE — generates tests/golden/*.npz by running the UNMODIFIED reference (/root/reference, through
-oracle/ref_shim.py) on seeded synthetic inputs.  Run in the build container only:  python -m oracle.make_golden
+"""TEST INFRASTRUCTURE — generates tests/golden/*.npz by running the UNMODIFIED reference (a checkout of
+neptune-ai/open-solution-mapping-challenge at MCB_REFERENCE_ROOT, imported through oracle/ref_shim.py) on seeded
+synthetic inputs:  python -m oracle.make_golden [postproc|unet|configs|conditioned|live ...]
 The fixtures pin the CPU oracle restatements (oracle/post_oracle.py, oracle/unet_oracle.py); the GPU tests then compare
 the CUDA path with the oracle and with these fixtures."""
+import json
 import os
 import sys
 import warnings
@@ -82,7 +84,7 @@ def golden_unet(um, mo):
     print("unet.npz", {k: v.shape for k, v in rec.items() if v.ndim == 0 or "logits" in k})
 
 
-from oracle.make_golden_cases import CONFIG_CASES, CONFIG_GRAD_KEYS, GRAD_HEAD, LOGIT_STRIDE  # noqa: E402
+from oracle.make_golden_cases import CONFIG_CASES, CONFIG_GRAD_KEYS, GRAD_HEAD, LOGIT_STRIDE, save_unet_golden  # noqa: E402
 
 
 def golden_unet_configs(um, mo):
@@ -99,20 +101,20 @@ def golden_unet_configs(um, mo):
         X, T = torch.from_numpy(x), torch.from_numpy(t)
         model.model.eval()
         with torch.no_grad():
-            rec["eval_logits_" + tag] = model.model(X[:1]).numpy()   # eval mode is per image: image 0 is enough
+            # eval mode is per image: image 0 is enough
+            rec["eval_logits_" + tag] = model.model(X[:1]).numpy()[:, :, ::LOGIT_STRIDE, ::LOGIT_STRIDE].copy()
         model.model.train()
         out = model.model(X)
         name, loss_fn, weight = model.loss_function[0]
         loss = loss_fn(out, T) * weight
         loss.backward()
-        rec["train_logits_" + tag] = out.detach().numpy()
+        rec["train_logits_" + tag] = out.detach().numpy()[:, :, ::LOGIT_STRIDE, ::LOGIT_STRIDE].copy()
         rec["loss_" + tag] = np.array(float(loss))
         sd = dict(model.model.named_parameters())
         for k in CONFIG_GRAD_KEYS:
             rec["grad_%s_%s" % (tag, k)] = sd[k].grad.detach().numpy().reshape(-1)[:GRAD_HEAD].copy()
         print(tag, "loss", float(loss), "logit range", float(out.min()), float(out.max()), flush=True)
-    np.savez_compressed(os.path.join(OUT, "unet_configs.npz"), **rec)
-    print("unet_configs.npz", os.path.getsize(os.path.join(OUT, "unet_configs.npz")) >> 10, "KiB")
+    save_unet_golden("configs", rec)
 
 
 def golden_unet_conditioned(um, mo):
@@ -168,15 +170,73 @@ def golden_unet_conditioned(um, mo):
             rec["grad_%s_%s" % (tag, k)] = params[k].grad.detach().numpy().reshape(-1)[:GRAD_HEAD].copy()
         print(tag, "conditioned: loss", float(loss), "logit range", float(out.min()), float(out.max()),
               "eval range", float(rec["eval_logits_" + tag].min()), float(rec["eval_logits_" + tag].max()), flush=True)
-    np.savez_compressed(os.path.join(OUT, "unet_conditioned.npz"), **rec)
-    print("unet_conditioned.npz", os.path.getsize(os.path.join(OUT, "unet_conditioned.npz")) >> 10, "KiB")
+    save_unet_golden("conditioned", rec)
+
+
+def golden_live(um, mo, pp, ut):
+    """what the CPU pins (tests/test_oracle_pins.py, test_input_cpu.py, test_instances_cpu.py) compare the oracles
+    against: the reference's own post-processing, network, preparation and test-time-augmentation functions on the
+    seeded inputs those tests regenerate"""
+    ref_shim.install()
+    import src.loaders as lo
+    import src.preparation as prep
+    from oracle import instances_oracle as I
+    rec = {}
+    for i, p in enumerate(synthetic.probability_maps(2, 48, seed=77, n_rect=8)):
+        a = pp.resize_image(p, (56, 56))
+        c = pp.categorize_multilayer_image(a)
+        l = pp.label_multilayer_image(c)
+        rec["live_resize_%d" % i], rec["live_cat_%d" % i], rec["live_label_%d" % i] = a, c, l
+        for k in (1, 2, 3, 4):
+            rec["live_dilate%d_%d" % (k, i)] = pp.dilate_image(l, k)
+            rec["live_erode%d_%d" % (k, i)] = pp.erode_image(c[1], k)
+    torch.manual_seed(7)
+    ref = um.UNetResNet(34, 2, 32, 0.0, False, True)   # = unet_oracle.make_reference_like_state_dict(34, seed=7)
+    x = torch.randn(1, 3, 64, 64)
+    ref.eval()
+    with torch.no_grad():
+        rec["live_unet_x"], rec["live_unet_logits"] = x.numpy(), ref(x).numpy()
+    # src/preparation.py: distances to the two nearest objects, size matrix
+    rs = np.random.RandomState(1)
+    masks = np.stack([synthetic.rectangles_mask(rs, 40, 52, n_rect=1, lo=4, hi=10)[0] for _ in range(5)])
+    d = np.zeros((40, 52))
+    for m in masks:
+        d = prep.update_distances(d, m)
+    rec["prep_dist_sum"], rec["prep_dist_second"] = prep.clean_distances(d.copy())
+    rec["prep_size_matrix"] = prep.get_size_matrix((masks.sum(0) > 0).astype(np.uint8))
+    # src/loaders.py: test-time augmentation generator / transform / inverse / aggregation; NMS
+    specs = I.tta_specs()
+    gen = lo.TestTimeAugmentationGenerator(flip_ud=True, flip_lr=True, rotation=True, color_shift_runs=False)
+    got = gen.transform(np.array([["a"], ["b"]], dtype=object))
+    rec["tta_params_json"] = np.array(json.dumps(got["tta_params"]))
+    rec["tta_img_ids"] = np.array(got["img_ids"])
+    rs = np.random.RandomState(5)
+    img = rs.randint(0, 255, (12, 12, 3)).astype(np.uint8)
+    fwd, inv, preds = [], [], []
+    for p in specs:
+        fwd.append(np.asarray(lo.test_time_augmentation_transform(img, p)))
+        pr = rs.rand(2, 12, 12).astype(np.float32)
+        inv.append(lo.test_time_augmentation_inverse_transform(pr, p))
+        preds.append(pr)
+    rec["tta_forward"], rec["tta_inverse"] = np.stack(fwd), np.stack(inv)
+    for method in ("gmean", "mean", "max", "min"):
+        agg = lo.TestTimeAugmentationAggregator(method, 2).transform(preds * 2, specs * 2, [0] * 16 + [1] * 16)
+        rec["tta_agg_" + method] = np.stack(agg["aggregated_prediction"])
+    lab = np.zeros((2, 20, 20), np.int32)
+    lab[0, 2:8, 2:8] = 1
+    lab[0, 10:18, 10:18] = 2
+    lab[1, 3:8, 2:8] = 1
+    lab[1, 12:14, 12:14] = 2
+    rec["nms_scores"] = np.array(pp.remove_overlapping_masks(lab, [[0.9, 0.5], [0.8, 0.7]], 0.5)[1])
+    np.savez_compressed(os.path.join(OUT, "live_reference.npz"), **rec)
+    print("live_reference.npz", os.path.getsize(os.path.join(OUT, "live_reference.npz")) >> 10, "KiB")
 
 
 if __name__ == "__main__":
     warnings.filterwarnings("ignore")
     os.makedirs(OUT, exist_ok=True)
     um, mo, pp, ut = ref_shim.reference_modules()
-    which = sys.argv[1:] or ["postproc", "unet", "configs", "conditioned"]
+    which = sys.argv[1:] or ["postproc", "unet", "configs", "conditioned", "live"]
     if "postproc" in which:
         golden_postproc(pp, ut)
     if "unet" in which:
@@ -185,3 +245,5 @@ if __name__ == "__main__":
         golden_unet_configs(um, mo)
     if "conditioned" in which:
         golden_unet_conditioned(um, mo)
+    if "live" in which:
+        golden_live(um, mo, pp, ut)

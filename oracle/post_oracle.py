@@ -1,9 +1,9 @@
 """TEST INFRASTRUCTURE — CPU oracle for the per-pixel mask post-processing.  Never imported by the product path.
 
-Restates, in numpy/scipy, the reference functions of /root/reference/src/postprocessing.py:48-258 and
-/root/reference/src/utils.py:231-273,324-339.  Each function cites the lines it follows.
+Restates, in numpy/scipy, the reference functions of src/postprocessing.py:48-258 and
+src/utils.py:231-273,324-339.  Each function cites the lines it follows.
 
-Third-party algorithms the reference calls but that are absent from /root/reference AND from this image:
+Third-party algorithms the reference calls but that are absent from the reference repository and from its pinned environment:
   * scikit-image (unpinned in environment.yml; the April-2018 conda env resolves to 0.13.x/0.14.x):
       skimage.transform.resize, skimage.morphology.{erosion, dilation, rectangle}
     restated below from skimage's published implementation of that era (they are thin wrappers over scipy.ndimage,

@@ -1,9 +1,9 @@
 """TEST INFRASTRUCTURE — not part of the product path.
 
-Imports the UNMODIFIED reference package (/root/reference/src, read-only) under Python 3.12 / torch 2.11 by
+Imports the UNMODIFIED reference package (the `src` package of a checkout named by MCB_REFERENCE_ROOT, read-only) under Python 3.12 / torch 2.11 by
 installing stub modules for its absent third-party dependencies (SURVEY.md Appendix B).  Used ONLY in the build
 container, by oracle/make_golden.py (to generate tests/golden/*) and by the CPU tests that pin the oracle
-restatements to the real reference.  /root/reference does not exist on the GPU box; nothing GPU-side imports this.
+restatements to the real reference.  Only the fixture generator (oracle/make_golden.py) imports this; no test does.
 
 Stubs that carry behaviour (the skimage calls of src/postprocessing.py:4-5) delegate to oracle/post_oracle.py's
 scipy restatements of skimage's documented implementation; everything else is inert.
@@ -15,11 +15,11 @@ import sys
 import tempfile
 import types
 
-REFERENCE_ROOT = os.environ.get("MCB_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("MCB_REFERENCE_ROOT", "")
 
 
 def available():
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "src"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "src"))
 
 
 class _AttrDict(dict):

@@ -2,7 +2,7 @@
 product path.
 
 A functional restatement (torch CPU, float32) of
-    UNetResNet.forward                      /root/reference/src/unet_models.py:338-403
+    UNetResNet.forward                      src/unet_models.py:338-403
     torchvision resnet34/101/152 blocks     torchvision/models/resnet.py (BasicBlock / Bottleneck; the reference
                                             pins torchvision 0.2.0, this image has 0.26 — same block arithmetic:
                                             stride on the 3x3, BN eps 1e-5 momentum 0.1, 1x1-s2 + BN downsample)

@@ -1,4 +1,4 @@
-"""Parity of the tcgen05 convolution family (forward, data gradient, weight gradient, transposed conv) against
+"""Parity of the wgmma convolution family (forward, data gradient, weight gradient, transposed conv) against
 torch's fp32 CPU convolution — the op the reference calls (nn.Conv2d / nn.ConvTranspose2d, src/unet_models.py:21-34,
 125-150; torchvision resnet blocks) — on bf16-rounded operands.
 
@@ -95,8 +95,8 @@ def test_conv3x3_haloed_tile_path(mcb, cuda, monkeypatch, n, h, w, cin, cout):
     _haloed_tile_checks(cuda, monkeypatch, n, h, w, cin, cout, resident=False)
 
 
-# (MCB_BRES, resident per-tap weights in the haloed path: parity-green on hardware since gpurun r2; it measured slower than
-# the per-tap path on every thin shape, so it stays an opt-in switch -- the tests keep it from rotting)
+# (MCB_BRES, resident per-tap weights in the haloed path: an opt-in switch, off by default -- the tests keep it from
+# rotting)
 @pytest.mark.parametrize("n,h,w,cin,cout", [(2, 32, 16, 64, 64), (1, 32, 24, 32, 32), (3, 16, 16, 32, 32),
                                              (2, 48, 40, 64, 128)])
 def test_conv3x3_haloed_tile_resident_weights(mcb, cuda, monkeypatch, n, h, w, cin, cout):
@@ -105,7 +105,7 @@ def test_conv3x3_haloed_tile_resident_weights(mcb, cuda, monkeypatch, n, h, w, c
 
 def _haloed_tile_checks(cuda, monkeypatch, n, h, w, cin, cout, resident):
     """MCB_HALO=1 forces the haloed-tile 3x3 path (one TMA box per channel chunk serves the nine taps through
-    row-shifted UMMA descriptors; default rule: >= 128 channels on large images): forward (+stats, integer-exact),
+    row-shifted wgmma descriptors; default rule: >= 128 channels on large images): forward (+stats, integer-exact),
     plain / masked data gradient, against the same references as the per-tap path"""
     from mcb200 import ops
     monkeypatch.setenv("MCB_HALO", "1")

@@ -1,11 +1,13 @@
-"""CPU pins of oracle/input_oracle.py against the libraries the reference itself calls (cv2, torchvision, scipy) and,
-in the build container, against src/preparation.py through the shim."""
+"""CPU pins of oracle/input_oracle.py against the libraries the reference itself calls (cv2, torchvision, scipy) and
+against the outputs of the reference's src/preparation.py (tests/golden/live_reference.npz)."""
+import os
+
 import numpy as np
 import pytest
 import torch
 
 from oracle import input_oracle as IO
-from oracle import ref_shim, synthetic
+from oracle import synthetic
 
 
 def test_pad_and_normalize_match_cv2_and_torchvision():
@@ -23,23 +25,18 @@ def test_pad_and_normalize_match_cv2_and_torchvision():
         assert got.dtype == np.float32 and np.array_equal(got, want)
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="reference tree only exists in the build container")
 def test_distances_and_sizes_live_against_reference():
-    ref_shim.install()
-    import src.preparation as prep
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "live_reference.npz"))
     rs = np.random.RandomState(1)
     masks = []
     for _ in range(5):
         m, _ = synthetic.rectangles_mask(rs, 40, 52, n_rect=1, lo=4, hi=10)
         masks.append(m)
     masks = np.stack(masks)
-    d = np.zeros((40, 52))
-    for m in masks:
-        d = prep.update_distances(d, m)
-    want_sum, want_second = prep.clean_distances(d.copy())
+    want_sum, want_second = g["prep_dist_sum"], g["prep_dist_second"]   # prep.update_distances / clean_distances
     got_sum, got_second = IO.two_nearest_distances(masks)
     assert got_sum.dtype == np.float16 and np.array_equal(got_sum, want_sum) and np.array_equal(got_second, want_second)
     one_sum, one_second = IO.two_nearest_distances(masks[:1])
     assert np.array_equal(one_sum, (2 * one_second).astype(np.float16))
     overlay = (masks.sum(0) > 0).astype(np.uint8)
-    assert np.array_equal(IO.get_size_matrix(overlay), prep.get_size_matrix(overlay))
+    assert np.array_equal(IO.get_size_matrix(overlay), g["prep_size_matrix"])

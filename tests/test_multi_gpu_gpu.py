@@ -55,7 +55,7 @@ def _run_two_ranks(sync_bn):
 @pytest.fixture(scope="module")
 def two_gpus(cuda):
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
 
 
 @pytest.mark.timeout(600)

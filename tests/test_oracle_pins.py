@@ -1,7 +1,7 @@
 """CPU tests that PIN the oracle (oracle/post_oracle.py, oracle/unet_oracle.py) to the reference:
   * against the golden fixtures in tests/golden/ (outputs of the unmodified reference, made by oracle/make_golden.py),
   * against the reference's only known-answer vector (src/postprocessing.py:95-111),
-  * and, when /root/reference is present (build container), live against the reference code on fresh seeds."""
+  * and against the reference's own functions on seeded inputs (tests/golden/live_reference.npz)."""
 import os
 
 import numpy as np
@@ -9,7 +9,7 @@ import pytest
 import torch
 
 from oracle import post_oracle as P
-from oracle import ref_shim, synthetic
+from oracle import synthetic
 from oracle import unet_oracle as O
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
@@ -111,44 +111,42 @@ def test_train_step_oracle_matches_reference_fit_loop(gu):
     assert abs(float(loss2) - float(gu["fit_loss2_34"])) < 2e-3 * abs(float(gu["fit_loss2_34"]))
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="reference tree only exists in the build container")
 def test_live_against_reference_code():
-    um, mo, pp, ut = ref_shim.reference_modules()
+    """the reference's resize / categorize / label / dilate / erode and its network (state_dict of
+    torch.manual_seed(7) + UNetResNet(34, ...), which make_reference_like_state_dict(34, seed=7) regenerates), stored by
+    oracle/make_golden.py (live)"""
+    g = np.load(os.path.join(GOLD, "live_reference.npz"))
     probs = synthetic.probability_maps(2, 48, seed=77, n_rect=8)
-    for p in probs:
-        a, b = pp.resize_image(p, (56, 56)), P.resize_image(p, (56, 56))
-        assert np.array_equal(a, b)
-        c = pp.categorize_multilayer_image(a)
+    for i, p in enumerate(probs):
+        b = P.resize_image(p, (56, 56))
+        assert np.array_equal(g["live_resize_%d" % i], b)
+        c = g["live_cat_%d" % i]
         assert np.array_equal(c, P.categorize_multilayer_image(b))
-        l = pp.label_multilayer_image(c)
+        l = g["live_label_%d" % i]
         assert np.array_equal(l, P.label_multilayer_image(c))
         for k in (1, 2, 3, 4):
-            assert np.array_equal(pp.dilate_image(l, k), P.dilate_image(l, k))
-            assert np.array_equal(pp.erode_image(c[1], k), P.erode_image(c[1], k))
+            assert np.array_equal(g["live_dilate%d_%d" % (k, i)], P.dilate_image(l, k))
+            assert np.array_equal(g["live_erode%d_%d" % (k, i)], P.erode_image(c[1], k))
     # network: same state_dict -> identical logits
-    torch.manual_seed(7)
-    ref = um.UNetResNet(34, 2, 32, 0.0, False, True)
-    sd = {k: v.clone() for k, v in ref.state_dict().items()}
-    x = torch.randn(1, 3, 64, 64)
-    ref.eval()
+    sd = O.make_reference_like_state_dict(34, seed=7)
+    x = torch.from_numpy(g["live_unet_x"])
     with torch.no_grad():
-        want = ref(x)
         got = O.UNetOracle(sd, 34).forward(x, training=False)
-    assert torch.equal(want, got)
+    assert torch.equal(torch.from_numpy(g["live_unet_logits"]), got)
 
 
 @pytest.mark.parametrize("case", [0, 1, 2])
 def test_unet_oracle_matches_config_goldens(case):
-    """tests/golden/unet_configs.npz (BASELINE.json configs 1 / 2 / 5: R34 b2 @256, R101 @320, R152 @512) was produced by
-    the UNMODIFIED reference from seed 1234; the seed-regenerated weights + inputs and the oracle network must reproduce
+    """tests/golden/unet_configs_*.npz (BASELINE.json configs 1 / 2 / 5: R34 b2 @256, R101 @320, R152 @512) was produced
+    by the UNMODIFIED reference from seed 1234; the seed-regenerated weights + inputs and the oracle network must reproduce
     its eval logits (image 0), which pins both the fixture's inputs and the oracle at those depths / resolutions."""
-    from oracle.make_golden_cases import CONFIG_CASES
+    from oracle.make_golden_cases import CONFIG_CASES, LOGIT_STRIDE, load_unet_golden
     tag, enc, depth, n, s = CONFIG_CASES[case]
-    g = np.load(os.path.join(GOLD, "unet_configs.npz"))
+    g = load_unet_golden("configs")
     sd = O.make_reference_like_state_dict(depth, seed=1234)
     x, _ = synthetic.train_batch(n, s, seed=1234)
     with torch.no_grad():
-        ev = O.UNetOracle(sd, depth).forward(torch.from_numpy(x[:1]), training=False)
+        ev = O.UNetOracle(sd, depth).forward(torch.from_numpy(x[:1]), training=False)[:, :, ::LOGIT_STRIDE, ::LOGIT_STRIDE]
     ref = g["eval_logits_" + tag]
     assert ev.shape == ref.shape
     assert np.abs(ev.numpy() - ref).max() < 1e-6

@@ -1,4 +1,4 @@
-"""The fused train step (PyTorchUNetWeighted._fit_loop on the B200 path) against the CPU oracle restatement of the
+"""The fused train step (PyTorchUNetWeighted._fit_loop on the H100 path) against the CPU oracle restatement of the
 reference's Model._fit_loop, and the transformer surface (transform -> softmax probabilities)."""
 import numpy as np
 import pytest
@@ -39,6 +39,31 @@ def test_fit_loop_tracks_oracle_for_several_steps(mcb, cuda):
     # BN running statistics follow nn.BatchNorm2d's update
     for k in ("encoder.bn1.running_mean", "encoder.bn1.running_var"):
         assert torch.allclose(got[k].cpu(), sd_o[k], rtol=2e-2, atol=1e-3), k
+
+
+def test_fused_train_steps_are_bitwise_reproducible(mcb, cuda):
+    """the same weights and batches give the same losses and weights, bit for bit: every cross-CTA sum of the step
+    (BatchNorm statistics and their backward, split-K weight gradients, classifier gradients, loss sums) is added in
+    a fixed order, so Adam's sign-like first updates cannot amplify run-to-run rounding differences"""
+    import bench
+    from mcb200.models import PyTorchUNetWeighted
+    x, t = synthetic.train_batch(8, 192, seed=4, n_rect=10)
+    X, T = torch.from_numpy(x).to(cuda), torch.from_numpy(t).to(cuda)
+    runs = []
+    # the seeded state dict and the constructors draw from torch's generator: leave it as the other tests expect it
+    with torch.random.fork_rng(devices=[cuda]):
+        sd = O.make_reference_like_state_dict(34, seed=21)
+        for _ in range(2):
+            model = PyTorchUNetWeighted(**bench.unet_config("ResNet34"))
+            model.model.load_state_dict(sd)
+            losses = [model._fit_loop([X, T])["sum"].detach().cpu().clone() for _ in range(4)]
+            runs.append((losses, {k: v.detach().cpu().clone() for k, v in model.model.state_dict().items()}))
+            del model
+            torch.cuda.empty_cache()
+    (la, sa), (lb, sb) = runs
+    assert all(torch.equal(a, b) for a, b in zip(la, lb)), (la, lb)
+    for k in sa:
+        assert torch.equal(sa[k], sb[k]), k
 
 
 def test_plain_ce_model_and_generic_autograd_path(mcb, cuda):

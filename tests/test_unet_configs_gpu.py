@@ -1,9 +1,9 @@
 """Parity of the CUDA U-Net against the UNMODIFIED reference at the BASELINE.json configurations:
 config 1 verbatim (ResNet34, batch 2, 256x256), the headline net at the headline resolution (ResNet101 @320, batch 2)
-and config 5's net / resolution (ResNet152 @512, batch 1).  Fixtures: tests/golden/unet_configs.npz (raw seed-1234
-initialisation) and tests/golden/unet_conditioned.npz (the same nets on a well-conditioned checkpoint), both produced by
-oracle/make_golden.py from the reference itself; inputs and weights are regenerated from the seed (pinned on the CPU by
-tests/test_oracle_pins.py).
+and config 5's net / resolution (ResNet152 @512, batch 1).  Fixtures: tests/golden/unet_configs_*.npz (raw seed-1234
+initialisation) and tests/golden/unet_conditioned_*.npz (the same nets on a well-conditioned checkpoint), both produced
+by oracle/make_golden.py from the reference itself, logits at every third pixel; inputs and weights are regenerated from
+the seed (pinned on the CPU by tests/test_oracle_pins.py).
 
 What is asserted, and why the two families:
   * north-star bound, 1e-3 max-abs on logits: training-mode logits at every configuration on BOTH checkpoints, eval-mode
@@ -17,7 +17,7 @@ What is asserted, and why the two families:
     these 34 / 101 / 152-layer nets by 14 % .. 99 % relative L2 against the fp32 reference -- measured on the CPU by the
     bit-faithful emulation oracle/emulated_bf16_deviation.py -> tests/golden/emulated_bf16_deviation.json.  The CUDA path
     must not be further from the reference than that emulation (x1.15 + 0.01): its deviation IS the storage format's,
-    tensor by tensor (first hardware run: 0.2679 vs 0.2702, 0.7475 vs 0.7615, 0.9676 vs 0.9870, ... at ResNet152).
+    tensor by tensor.
     At the raw init the deep gradients are numerically chaotic (|grad| 1e-8..1e-10, cosine ~0 between ANY two
     bf16-storage evaluations, DESIGN.md section 3) and only their finiteness is checked.
 """
@@ -30,7 +30,7 @@ import torch
 
 from oracle import synthetic
 from oracle import unet_oracle as O
-from oracle.make_golden_cases import CONFIG_CASES, GRAD_HEAD, LOGIT_STRIDE
+from oracle.make_golden_cases import CONFIG_CASES, GRAD_HEAD, LOGIT_STRIDE, load_unet_golden
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
@@ -41,8 +41,8 @@ def _run(case, family, cuda):
     from mcb200 import models
     from mcb200.unet_models import UNetResNet
     tag, enc, depth, n, s = CONFIG_CASES[case]
-    g = np.load(os.path.join(GOLD, "unet_%s.npz" % family))
-    s3 = LOGIT_STRIDE if family == "conditioned" else 1
+    g = load_unet_golden(family)
+    s3 = LOGIT_STRIDE
     x, t = synthetic.train_batch(n, s, seed=1234)
     sd = (O.conditioned_state_dict(depth, torch.from_numpy(x), seed=1234) if family == "conditioned"
           else O.make_reference_like_state_dict(depth, seed=1234))
@@ -61,7 +61,7 @@ def _run(case, family, cuda):
     loss.backward()
     params = dict(net.named_parameters())
     grads = {}
-    for name in g.files:
+    for name in g:
         if name.startswith("grad_%s_" % tag):
             k = name[len("grad_%s_" % tag):]
             ref = torch.from_numpy(g[name]).double()
