@@ -3,7 +3,11 @@ torch's fp32 CPU convolution — the op the reference calls (nn.Conv2d / nn.Conv
 125-150; torchvision resnet blocks) — on bf16-rounded operands.
 
 Tolerance: outputs are stored as bf16 (8 mantissa bits) after fp32 accumulation, so |err| <= 2^-8 |ref| + small
-accumulation-order noise; integer-valued cases must match exactly."""
+accumulation-order noise; integer-valued cases must match exactly.
+
+These shapes are small: each CTA of the persistent conv kernel runs about one tile, and the weight-gradient ring does
+not wrap.  test_conv_gemm_persistent_gpu.py covers the multi-tile regime of the full-size network (several tiles per
+CTA, every N-tile width, accumulation into existing gradients) with element-wise float64 bounds."""
 import os
 
 import pytest
