@@ -103,6 +103,13 @@ class TrainStep:
         self.opt.step()
         return loss.detach()
 
+    @classmethod
+    def for_encoder(cls, encoder, device):
+        """the train step of a src/models.py registry name.  The reference's AlbuNet (src/unet_models.py:153-221) is
+        UNetResNet(34) without the classifier dropout, which this restatement never applies: the same net"""
+        depth = {"AlbuNet": 34, "ResNet34": 34, "ResNet101": 101, "ResNet152": 152}[encoder]
+        return cls(depth, device)
+
     @torch.no_grad()
     def infer(self, x):
         self.net.eval()

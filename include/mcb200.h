@@ -99,27 +99,32 @@ typedef struct {
 } mcb_conv_wgrad_args;
 int mcb_conv_wgrad(const mcb_conv_wgrad_args* a, void* stream);
 
-/* nn.ConvTranspose2d(kernel_size=4, stride=2, padding=1) (src/unet_models.py:138-139) as four sub-pixel phases */
+/* nn.ConvTranspose2d(kernel_size=4, stride=2, padding=1) (src/unet_models.py:138-139) as four sub-pixel phases, or, with
+   ksize = 3, nn.ConvTranspose2d(kernel_size=3, stride=2, padding=1, output_padding=1) (the UNet11 DecoderBlock,
+   src/unet_models.py:42-53); both map h x w to 2h x 2w.  ksize is the last field so that a zeroed struct (ksize 0)
+   keeps meaning the 4x4 kernel */
 typedef struct {
   const void* x;      /* NHWC bf16 [n][h][w][cin] */
   int n, h, w, cin;
-  const void* weight; /* bf16 [16][cout][cin] */
+  const void* weight; /* bf16 [ksize*ksize][cout][cin] */
   int cout;
   const float* bias;
   int relu;
   void* y;            /* NHWC bf16 [n][2h][2w][cout] */
+  int ksize;          /* 3 or 4; 0 means 4 */
 } mcb_convt_fwd_args;
 int mcb_convt_fwd(const mcb_convt_fwd_args* a, void* stream);
 
 typedef struct {
   const void* dy;     /* NHWC bf16 [n][2h][2w][cout] */
   int n, h, w, cin;
-  const void* weight; /* bf16 [16][cout][cin] */
+  const void* weight; /* bf16 [ksize*ksize][cout][cin] */
   int cout;
   void* dx;           /* NHWC bf16 [n][h][w][cin] */
   const void* relu_mask;
   int accumulate;
   float* dx_channel_sum; /* as in mcb_conv_dgrad_args */
+  int ksize;          /* 3 or 4; 0 means 4 */
 } mcb_convt_dgrad_args;
 int mcb_convt_dgrad(const mcb_convt_dgrad_args* a, void* stream);
 
@@ -127,7 +132,8 @@ typedef struct {
   const void* dy;     /* NHWC bf16 [n][2h][2w][cout] */
   const void* x;      /* NHWC bf16 [n][h][w][cin] */
   int n, h, w, cin, cout;
-  float* dw;          /* fp32 [16][cout][cin], accumulated */
+  float* dw;          /* fp32 [ksize*ksize][cout][cin], accumulated */
+  int ksize;          /* 3 or 4; 0 means 4 */
 } mcb_convt_wgrad_args;
 int mcb_convt_wgrad(const mcb_convt_wgrad_args* a, void* stream);
 

@@ -36,16 +36,17 @@ class ConvWgradArgs(C.Structure):
 
 class ConvtFwdArgs(C.Structure):
     _fields_ = [("x", vp), ("n", ci), ("h", ci), ("w", ci), ("cin", ci), ("weight", vp), ("cout", ci), ("bias", vp),
-                ("relu", ci), ("y", vp)]
+                ("relu", ci), ("y", vp), ("ksize", ci)]
 
 
 class ConvtDgradArgs(C.Structure):
     _fields_ = [("dy", vp), ("n", ci), ("h", ci), ("w", ci), ("cin", ci), ("weight", vp), ("cout", ci), ("dx", vp),
-                ("relu_mask", vp), ("accumulate", ci), ("dx_channel_sum", vp)]
+                ("relu_mask", vp), ("accumulate", ci), ("dx_channel_sum", vp), ("ksize", ci)]
 
 
 class ConvtWgradArgs(C.Structure):
-    _fields_ = [("dy", vp), ("x", vp), ("n", ci), ("h", ci), ("w", ci), ("cin", ci), ("cout", ci), ("dw", vp)]
+    _fields_ = [("dy", vp), ("x", vp), ("n", ci), ("h", ci), ("w", ci), ("cin", ci), ("cout", ci), ("dw", vp),
+                ("ksize", ci)]
 
 
 def check(rc, what=""):

@@ -174,17 +174,26 @@ static int dgrad_s2_taps(int ksize, int py, Tap1D* out) {
   out[0] = {0, 1, 0}; out[1] = {2, 0, 0};
   return 2;
 }
-// transposed conv k=4 s=2 p=1 forward for output parity py: out[2y+py] += in[y+d] W[k]
-static int convt_fwd_taps(int py, Tap1D* out) {
+// transposed conv s=2 p=1 forward for output parity py: out[2y+py] += in[y+d] W[k], from out[2i - 1 + k] += in[i] W[k].
+// k=4: two taps per parity.  k=3 (output_padding 1, same 2x output): parity 0 has the one tap k=1, parity 1 has k=2
+// and k=0 at d=+1, which reads the zero row past the bottom / right edge (TMA out-of-bounds fill)
+static int convt_fwd_taps(int ksize, int py, Tap1D* out) {
+  if (ksize == 3) {
+    if (py == 0) { out[0] = {1, 0, 0}; return 1; }
+    out[0] = {2, 0, 0}; out[1] = {0, 1, 0};
+    return 2;
+  }
   if (py == 0) { out[0] = {1, 0, 0}; out[1] = {3, -1, 0}; }
   else { out[0] = {0, 1, 0}; out[1] = {2, 0, 0}; }
   return 2;
 }
-// transposed conv data gradient: din[y] = sum_k dout[2y - 1 + k] W[k]  (parity view of dout, offset d)
-static int convt_dgrad_taps(Tap1D* out) {
+// transposed conv data gradient: din[y] = sum_k dout[2y - 1 + k] W[k]  (parity view of dout, offset d); the k=3
+// kernel uses the first three taps (= fwd_s2_taps(3): the data gradient of ConvT(3, 2, 1, 1) is a 3x3 stride-2 conv)
+static int convt_dgrad_taps(int ksize, Tap1D* out) {
   out[0] = {0, -1, 1}; out[1] = {1, 0, 0}; out[2] = {2, 0, 1}; out[3] = {3, 1, 0};
-  return 4;
+  return ksize;
 }
+static int convt_ksize(int ksize) { return ksize == 0 ? 4 : ksize; }
 
 static int check_c(int c, const char* what) {
   if (c % 32 != 0) return fail(MCB_ERR_UNSUPPORTED, "%s channels %d not a multiple of 32", what, c);
@@ -379,6 +388,8 @@ extern "C" int mcb_convt_fwd(const mcb_convt_fwd_args* a, void* stream) {
   MCB_REQUIRE(a && a->x && a->weight && a->y, "convt_fwd: null pointer");
   if (int r = check_c(a->cin, "convt_fwd input")) return r;
   if (int r = check_c(a->cout, "convt_fwd output")) return r;
+  const int K = convt_ksize(a->ksize);
+  MCB_REQUIRE(K == 3 || K == 4, "convt_fwd: ksize %d", a->ksize);
   const int H = a->h, W = a->w, N = a->n;
   const int BK = (a->cin % 64 == 0) ? 64 : 32;
   ConvGemmParams p;
@@ -397,19 +408,19 @@ extern "C" int mcb_convt_fwd(const mcb_convt_fwd_args* a, void* stream) {
     for (int px = 0; px < 2; ++px) {
       const int ph = py * 2 + px;
       Tap1D ty[2], tx[2];
-      convt_fwd_taps(py, ty); convt_fwd_taps(px, tx);
+      const int ny = convt_fwd_taps(K, py, ty), nx = convt_fwd_taps(K, px, tx);
       p.tap_start[ph] = nt;
-      for (int i = 0; i < 2; ++i)
-        for (int j = 0; j < 2; ++j) {
+      for (int i = 0; i < ny; ++i)
+        for (int j = 0; j < nx; ++j) {
           TapDesc& t = p.taps[nt++];
-          t.src = 0; t.dx = tx[j].d; t.dy = ty[i].d; t.nchunks = a->cin / BK; t.wk0 = 0; t.wtap = ty[i].k * 4 + tx[j].k;
+          t.src = 0; t.dx = tx[j].d; t.dy = ty[i].d; t.nchunks = a->cin / BK; t.wk0 = 0; t.wtap = ty[i].k * K + tx[j].k;
         }
-      p.tap_count[ph] = 4;
+      p.tap_count[ph] = nt - p.tap_start[ph];
       const int out_cw = BN >= 64 ? 64 : 32;
       if (int r = encode_nhwc_view(&p.tmD[ph], a->y, N, 2 * H, 2 * W, a->cout, 0, a->cout, py, px, out_cw, p.bw, p.bh,
                                    p.bn, out_cw * 2)) return r;
     }
-  if (int r = encode_weight(&p.tmB, a->weight, 16, a->cout, a->cin, BK, BN, BK * 2)) return r;
+  if (int r = encode_weight(&p.tmB, a->weight, K * K, a->cout, a->cin, BK, BN, BK * 2)) return r;
   p.bias = a->bias; p.relu = a->relu;
   return launch_conv(BN, BK, false, p, (int)m_tiles, a->cout / BN, 4, st);
 }
@@ -420,6 +431,8 @@ extern "C" int mcb_convt_dgrad(const mcb_convt_dgrad_args* a, void* stream) {
   MCB_REQUIRE(!(a->relu_mask && a->accumulate), "convt_dgrad: relu_mask with accumulate is ill-defined");
   if (int r = check_c(a->cin, "convt_dgrad dx")) return r;
   if (int r = check_c(a->cout, "convt_dgrad dy")) return r;
+  const int K = convt_ksize(a->ksize);
+  MCB_REQUIRE(K == 3 || K == 4, "convt_dgrad: ksize %d", a->ksize);
   const int H = a->h, W = a->w, N = a->n;  // input (dx) dims; dy is 2H x 2W
   const int BK = (a->cout % 64 == 0) ? 64 : 32;
   ConvGemmParams p;
@@ -435,17 +448,17 @@ extern "C" int mcb_convt_dgrad(const mcb_convt_dgrad_args* a, void* stream) {
     if (int r = encode_nhwc_view(&p.tmA[v], a->dy, N, 2 * H, 2 * W, a->cout, 0, a->cout, v >> 1, v & 1, BK, p.bw,
                                  p.bh, p.bn, BK * 2)) return r;
   Tap1D t1[4];
-  convt_dgrad_taps(t1);
+  const int n1 = convt_dgrad_taps(K, t1);
   int nt = 0;
-  for (int i = 0; i < 4; ++i)
-    for (int j = 0; j < 4; ++j) {
+  for (int i = 0; i < n1; ++i)
+    for (int j = 0; j < n1; ++j) {
       TapDesc& t = p.taps[nt++];
       t.src = t1[i].parity * 2 + t1[j].parity; t.dx = t1[j].d; t.dy = t1[i].d; t.nchunks = a->cout / BK; t.wk0 = 0;
-      t.wtap = t1[i].k * 4 + t1[j].k;
+      t.wtap = t1[i].k * K + t1[j].k;
     }
   p.tap_start[0] = 0; p.tap_count[0] = nt;
   const int bmn_cw = BN >= 64 ? 64 : 32;
-  if (int r = encode_weight(&p.tmB, a->weight, 16, a->cout, a->cin, bmn_cw, BK, bmn_cw * 2)) return r;
+  if (int r = encode_weight(&p.tmB, a->weight, K * K, a->cout, a->cin, bmn_cw, BK, bmn_cw * 2)) return r;
   const int out_cw = BN >= 64 ? 64 : 32;
   if (int r = encode_nhwc_view(&p.tmD[0], a->dx, N, H, W, a->cin, 0, a->cin, -1, -1, out_cw, p.bw, p.bh, p.bn,
                                out_cw * 2)) return r;
@@ -622,6 +635,8 @@ extern "C" int mcb_convt_wgrad(const mcb_convt_wgrad_args* a, void* stream) {
   if (int r = check_c(a->cout, "convt_wgrad dy")) return r;
   if (int r = check_c(a->cin, "convt_wgrad x")) return r;
   MCB_REQUIRE(a->cout % 128 == 0 || a->cout == 64 || a->cout == 32, "convt_wgrad: cout %d", a->cout);
+  const int K = convt_ksize(a->ksize);
+  MCB_REQUIRE(K == 3 || K == 4, "convt_wgrad: ksize %d", a->ksize);
   const int H = a->h, W = a->w, N = a->n;  // input dims; dy is 2H x 2W
   WgradParams p;
   memset(&p, 0, sizeof(p));
@@ -633,13 +648,13 @@ extern "C" int mcb_convt_wgrad(const mcb_convt_wgrad_args* a, void* stream) {
   if (int r = encode_nhwc_view(&p.tmB[0], a->x, N, H, W, a->cin, 0, a->cin, -1, -1, b_cw, p.bw, p.bh, p.bn, b_cw * 2))
     return r;
   Tap1D t1[4];
-  convt_dgrad_taps(t1);
+  const int n1 = convt_dgrad_taps(K, t1);
   int nt = 0;
-  for (int i = 0; i < 4; ++i)
-    for (int j = 0; j < 4; ++j) {
+  for (int i = 0; i < n1; ++i)
+    for (int j = 0; j < n1; ++j) {
       WgradTap& t = p.taps[nt++];
       t.srcA = t1[i].parity * 2 + t1[j].parity; t.ax = t1[j].d; t.ay = t1[i].d;
-      t.srcB = 0; t.bx = 0; t.by = 0; t.wtap = t1[i].k * 4 + t1[j].k;
+      t.srcB = 0; t.bx = 0; t.by = 0; t.wtap = t1[i].k * K + t1[j].k;
     }
   p.ntaps = nt;
   p.dw = a->dw; p.cout = a->cout; p.cin_total = a->cin; p.ci_off = 0;

@@ -22,10 +22,14 @@ from torch import nn, optim
 
 from . import _lib as L
 from . import ops
-from .unet_models import UNetResNet
+from .unet_models import AlbuNet, UNetResNet
 
-# registry of src/models.py:22-47, ResNet entries (pretrained weights need a network: load a checkpoint instead)
+# registry of src/models.py:22-47, AlbuNet and ResNet entries (pretrained weights need a network: load a checkpoint
+# instead)
 PRETRAINED_NETWORKS = {
+    'AlbuNet': {'model': AlbuNet,
+                'model_config': {'num_classes': 2, 'pretrained': False, 'is_deconv': True},
+                'init_weights': False},
     'ResNet34': {'model': UNetResNet,
                  'model_config': {'encoder_depth': 34, 'num_classes': 2, 'num_filters': 32, 'dropout_2d': 0.0,
                                   'pretrained': False, 'is_deconv': True, },
@@ -329,7 +333,8 @@ class BasePyTorchUNet(Model):
     def set_model(self):
         encoder = self.architecture_config['model_params']['encoder']
         if encoder not in PRETRAINED_NETWORKS:
-            raise NotImplementedError("the H100 path implements the ResNet34/101/152 encoders (got %r)" % (encoder,))
+            raise NotImplementedError("the H100 path implements the AlbuNet and ResNet34/101/152 encoders; the VGG11 "
+                                      "and VGG16 U-Nets are not built (got %r)" % (encoder,))
         config = PRETRAINED_NETWORKS[encoder]
         self.model = config['model'](**config['model_config'])
         self._initialize_model_weights = lambda: None

@@ -106,18 +106,24 @@ def conv_wgrad(dy, x, dw, ksize, stride, ci_off=0):
     return dw
 
 
+def _convt_ksize(taps):
+    """packed transposed-conv weights hold k*k taps: 16 -> ConvTranspose2d(4, 2, 1), 9 -> ConvTranspose2d(3, 2, 1, 1)"""
+    assert taps in (9, 16), taps
+    return 3 if taps == 9 else 4
+
+
 def convt_fwd(x, w, bias=None, relu=False, out=None):
     _chk(x); _chk(w)
     n, h, wd, cin = x.shape
     cout = w.shape[1]
-    assert w.shape == (16, cout, cin)
+    assert w.shape[1:] == (cout, cin), (w.shape, cin)
     if out is None:
         out = torch.empty((n, 2 * h, 2 * wd, cout), dtype=torch.bfloat16, device=x.device)
     a = L.ConvtFwdArgs()
     a.x = x.data_ptr(); a.n, a.h, a.w, a.cin = n, h, wd, cin
     a.weight = w.data_ptr(); a.cout = cout
     a.bias = _chk(bias, torch.float32).data_ptr() if bias is not None else None
-    a.relu = int(relu); a.y = _chk(out).data_ptr()
+    a.relu = int(relu); a.y = _chk(out).data_ptr(); a.ksize = _convt_ksize(w.shape[0])
     L.call("mcb_convt_fwd", a)
     return out
 
@@ -137,6 +143,7 @@ def convt_dgrad(dy, w, relu_mask=None, accumulate=False, out=None, channel_sum=N
     a.accumulate = int(accumulate)
     if channel_sum is not None:
         a.dx_channel_sum = _chk(channel_sum, torch.float32).data_ptr()
+    a.ksize = _convt_ksize(w.shape[0])
     L.call("mcb_convt_dgrad", a)
     return out
 
@@ -146,7 +153,7 @@ def convt_wgrad(dy, x, dw):
     n, h, wd, cin = x.shape
     a = L.ConvtWgradArgs()
     a.dy = dy.data_ptr(); a.x = x.data_ptr(); a.n, a.h, a.w, a.cin = n, h, wd, cin
-    a.cout = dw.shape[1]; a.dw = dw.data_ptr()
+    a.cout = dw.shape[1]; a.dw = dw.data_ptr(); a.ksize = _convt_ksize(dw.shape[0])
     L.call("mcb_convt_wgrad", a)
     return dw
 

@@ -1,4 +1,5 @@
-"""Mirror of the reference's src/unet_models.py for the ResNet-encoder U-Net, executed by libmcb200.so.
+"""Mirror of the reference's src/unet_models.py for the ResNet-encoder U-Nets (UNetResNet and AlbuNet), executed by
+libmcb200.so.
 
 `UNetResNet` keeps the reference's constructor, attribute tree and state_dict keys
 (src/unet_models.py:315-403: encoder.*, conv1..conv5 aliases, center/dec5..dec1 `.block.{0.conv,1}`,
@@ -230,3 +231,13 @@ class UNetResNet(nn.Module):
             return UNetFunction.apply(x, self, pl, *[p for _, p, _ in self._arena_params()])
         self.refresh_operands()
         return pl.forward(x).clone()
+
+
+class AlbuNet(UNetResNet):
+    """The reference's AlbuNet (src/unet_models.py:153-221): a ResNet34 encoder under the decoder of UNetResNet(34),
+    without the dropout before the classifier.  Its module tree, state_dict keys and seeded initialisation equal
+    UNetResNet(34)'s, so it runs through the same launch plan."""
+
+    def __init__(self, num_classes=1, num_filters=32, pretrained=False, is_deconv=False):
+        super().__init__(34, num_classes, num_filters=num_filters, dropout_2d=0.0, pretrained=pretrained,
+                         is_deconv=is_deconv)
