@@ -1,6 +1,7 @@
-// conv_gemm.cu — host side of the convolution family: decomposes each conv / transposed conv / gradient into
-// taps + phases, picks pixel tiles, encodes the TMA tensor maps and launches the wgmma kernels of conv_gemm.cuh.
-// Exposed through the C ABI declared in include/mcb200.h.
+// conv_gemm.cu — host side of the convolution family.  Each entry point validates its arguments, sets the epilogue
+// fields and describes its op: the tensors it reads and writes (View) and the per-axis tap rule (TapRule).  plan_conv /
+// plan_wgrad turn that description into taps + phases, pixel tiles and TMA tensor maps and launch the wgmma kernels of
+// conv_gemm.cuh.  Exposed through the C ABI declared in include/mcb200.h.
 #include "host_common.h"
 #include "conv_gemm.cuh"
 #include "../../include/mcb200.h"
@@ -149,50 +150,60 @@ static int pick_bn(int n_total, long m_tiles, int phases) {
   return bn;
 }
 
-// weight tensor map: bf16 [taps][rows = cout][cols = cin_total], viewed as (cin_total, cout, taps)
-static int encode_weight(CUtensorMap* m, const void* w, int taps, int cout, int cin_total, int box_inner, int box_rows,
-                         int swizzle) {
-  uint64_t dims[3] = {(uint64_t)cin_total, (uint64_t)cout, (uint64_t)taps};
-  uint64_t str[2] = {(uint64_t)cin_total * 2, (uint64_t)cin_total * cout * 2};
+// weight tensor map: bf16 [taps][rows][pitch], columns [c_off, c_off + cols) viewed as (cols, rows, taps)
+static int encode_weight(CUtensorMap* m, const void* w, int taps, int rows, int pitch, int c_off, int cols,
+                         int box_inner, int box_rows) {
+  uint64_t dims[3] = {(uint64_t)cols, (uint64_t)rows, (uint64_t)taps};
+  uint64_t str[2] = {(uint64_t)pitch * 2, (uint64_t)pitch * rows * 2};
   uint32_t box[3] = {(uint32_t)box_inner, (uint32_t)box_rows, 1};
-  return encode_tmap(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, w, dims, str, box, swizzle);
+  return encode_tmap(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, static_cast<const char*>(w) + (size_t)c_off * 2, dims, str,
+                     box, box_inner * 2);
 }
 
-// 1-D decomposition helpers ------------------------------------------------------------------------
+// NHWC bf16 tensor
+struct View { const void* p; int n, h, w, c; };
+
+// tensor map of t (slot < 0) or of its 2x2 parity view (py, px) = (slot >> 1, slot & 1); box (box_c, bw, bh, bn)
+static int encode_view(CUtensorMap* m, const View& t, int slot, int box_c, int bw, int bh, int bn) {
+  return encode_nhwc_view(m, t.p, t.n, t.h, t.w, t.c, 0, t.c, slot < 0 ? -1 : slot >> 1, slot < 0 ? -1 : slot & 1,
+                          box_c, bw, bh, bn, box_c * 2);
+}
+
+// 1-D decomposition ------------------------------------------------------------------------------------------------
+// One axis of a convolution with kernel size ksize, padding pad and stride 1 or 2: output o reads input
+// stride * o - pad + k.  gather: the taps of that convolution; scatter: the taps of its data gradient (the transposed
+// conv of stride 2, padding 1 is the data gradient of such a conv).  Taps are listed by increasing kernel index k, or
+// decreasing with k_desc: the order within a phase is the fp32 accumulation order of the kernel.
+struct TapRule { int ksize, pad, stride; bool scatter = false, k_desc = false; };
 struct Tap1D { int k; int d; int parity; };  // kernel index, offset in the (possibly parity) view, source parity
 
-// forward conv, stride 2, k=3, pad=1: input coordinate 2*o - 1 + k
-static int fwd_s2_taps(int ksize, Tap1D* out) {
-  if (ksize == 1) { out[0] = {0, 0, 0}; return 1; }
-  out[0] = {0, -1, 1}; out[1] = {1, 0, 0}; out[2] = {2, 0, 1};
-  return 3;
-}
-// data gradient of a stride-2 conv for output parity py: da[2y+py] = sum_k dz[(2y+py+pad-k)/2] W[k], parity must match
-static int dgrad_s2_taps(int ksize, int py, Tap1D* out) {
-  if (ksize == 1) { if (py == 0) { out[0] = {0, 0, 0}; return 1; } return 0; }
-  if (py == 0) { out[0] = {1, 0, 0}; return 1; }
-  out[0] = {0, 1, 0}; out[1] = {2, 0, 0};
-  return 2;
-}
-// transposed conv s=2 p=1 forward for output parity py: out[2y+py] += in[y+d] W[k], from out[2i - 1 + k] += in[i] W[k].
-// k=4: two taps per parity.  k=3 (output_padding 1, same 2x output): parity 0 has the one tap k=1, parity 1 has k=2
-// and k=0 at d=+1, which reads the zero row past the bottom / right edge (TMA out-of-bounds fill)
-static int convt_fwd_taps(int ksize, int py, Tap1D* out) {
-  if (ksize == 3) {
-    if (py == 0) { out[0] = {1, 0, 0}; return 1; }
-    out[0] = {2, 0, 0}; out[1] = {0, 1, 0};
-    return 2;
+// gather: offset floor((k - pad) / stride) in the input parity view (k - pad) mod stride, for every k.
+// scatter, for parity `parity` of the convolution's input (the data gradient's output): input stride * y + parity
+// receives output y + (parity + pad - k) / stride, for the k where that divides (stride 1: parity 0 and every k)
+static int taps_1d(const TapRule& r, int parity, Tap1D* out) {
+  int n = 0;
+  for (int i = 0; i < r.ksize; ++i) {
+    const int k = r.k_desc ? r.ksize - 1 - i : i;
+    if (!r.scatter) {
+      const int s = k - r.pad, par = (s % r.stride + r.stride) % r.stride;
+      out[n++] = {k, (s - par) / r.stride, par};
+    } else if ((parity + r.pad - k) % r.stride == 0) {
+      out[n++] = {k, (parity + r.pad - k) / r.stride, 0};
+    }
   }
-  if (py == 0) { out[0] = {1, 0, 0}; out[1] = {3, -1, 0}; }
-  else { out[0] = {0, 1, 0}; out[1] = {2, 0, 0}; }
-  return 2;
+  return n;
 }
-// transposed conv data gradient: din[y] = sum_k dout[2y - 1 + k] W[k]  (parity view of dout, offset d); the k=3
-// kernel uses the first three taps (= fwd_s2_taps(3): the data gradient of ConvT(3, 2, 1, 1) is a 3x3 stride-2 conv)
-static int convt_dgrad_taps(int ksize, Tap1D* out) {
-  out[0] = {0, -1, 1}; out[1] = {1, 0, 0}; out[2] = {2, 0, 1}; out[3] = {3, 1, 0};
-  return ksize;
+
+// Calls f(slot, dx, dy, wtap) for the 2-D taps of phase (py, px), y-major: slot = py * 2 + px of the source parity view
+// the tap reads (0 for stride-1 ops), (dx, dy) its offset in that view, wtap its weight tap
+template <class F>
+static void for_each_tap(const TapRule& r, int py, int px, F f) {
+  Tap1D ty[4], tx[4];
+  const int ny = taps_1d(r, py, ty), nx = taps_1d(r, px, tx);
+  for (int i = 0; i < ny; ++i)
+    for (int j = 0; j < nx; ++j) f(ty[i].parity * 2 + tx[j].parity, tx[j].d, ty[i].d, ty[i].k * r.ksize + tx[j].k);
 }
+
 static int convt_ksize(int ksize) { return ksize == 0 ? 4 : ksize; }
 
 static int check_c(int c, const char* what) {
@@ -201,104 +212,23 @@ static int check_c(int c, const char* what) {
   return MCB_OK;
 }
 
-}  // namespace mcb
-
-using namespace mcb;
-
-// =====================================================================================================
-extern "C" int mcb_conv_fwd(const mcb_conv_fwd_args* a, void* stream) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  MCB_REQUIRE(a && a->x[0] && a->weight && a->y, "conv_fwd: null pointer");
-  MCB_REQUIRE(a->ksize == 1 || a->ksize == 3, "conv_fwd: ksize %d", a->ksize);
-  MCB_REQUIRE(a->stride == 1 || a->stride == 2, "conv_fwd: stride %d", a->stride);
-  const int nsrc = a->x[1] ? 2 : 1;
-  MCB_REQUIRE(!(nsrc == 2 && a->stride == 2), "conv_fwd: concat + stride 2 unsupported");
-  const int cin_total = a->cin[0] + (nsrc == 2 ? a->cin[1] : 0);
+// One conv_gemm_kernel launch for an op whose taps follow `rule` along both axes.  GEMM M runs over the pixels of the
+// output view, N over out.c, K over taps x the channels of the A sources.
+//  - gather (forward conv, transposed-conv data gradient): one phase.  A is the concatenated sources a[0 .. nsrc) at
+//    stride 1 (slot = source), or the 2x2 parity views of a[0] at stride 2 (slot = py * 2 + px).
+//  - scatter (conv data gradient, transposed-conv forward): A is a[0].  At stride 2 there is one phase per parity view of
+//    out that receives taps, packed in (py, px) order.
+// Weights are bf16 [ksize^2][rows][w_pitch]: K-major for forward ops (rows = out.c, the A sources' channels side by
+// side), MN-major for data gradients (b_mn: rows = a[0].c, columns [w_off, w_off + out.c)).  aux: a tensor with the
+// geometry of out that the epilogue reads (p.aux_mode), or null.  The caller has set the epilogue fields of p.
+static int plan_conv(ConvGemmParams& p, const TapRule& rule, const View* a, int nsrc, const View& out, const void* aux,
+                     const void* w, int w_pitch, int w_off, bool b_mn, cudaStream_t st) {
+  const bool phased = rule.scatter && rule.stride == 2, parity_a = !rule.scatter && rule.stride == 2;
+  const int Wv = phased ? out.w / 2 : out.w, Hv = phased ? out.h / 2 : out.h, N = out.n;
+  int BK = 64;
   for (int s = 0; s < nsrc; ++s)
-    if (int r = check_c(a->cin[s], "conv_fwd input")) return r;
-  if (int r = check_c(a->cout, "conv_fwd output")) return r;
-  const int BK = (a->cin[0] % 64 == 0 && (nsrc == 1 || a->cin[1] % 64 == 0)) ? 64 : 32;
-  MCB_REQUIRE(!(BK == 32 && nsrc == 2), "conv_fwd: 32-channel concat unsupported");
-  const int H = a->h, W = a->w, N = a->n;
-  MCB_REQUIRE(a->stride == 1 || (H % 2 == 0 && W % 2 == 0), "conv_fwd: stride 2 needs even H, W");
-  const int Ho = H / a->stride, Wo = W / a->stride;
-  const int pad = a->ksize / 2;
-
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  const bool halo = use_halo(a->ksize, a->stride, Wo, Ho, nsrc == 2 ? std::min(a->cin[0], a->cin[1]) : a->cin[0]);
-  if (halo) { p.bw = 8; p.bh = 16; p.bn = 1; }
-  else pick_tile(Wo, Ho, N, 128, 1, &p.bw, &p.bh, &p.bn);
-  p.rows = p.bw * p.bh * p.bn;
-  p.Wv = Wo; p.Hv = Ho; p.Nimg = N;
-  p.tiles_x = (Wo + p.bw - 1) / p.bw;
-  p.tiles_y = (Ho + p.bh - 1) / p.bh;
-  const long m_tiles = (long)p.tiles_x * p.tiles_y * ((N + p.bn - 1) / p.bn);
-  const int BN = pick_bn(a->cout, m_tiles, 1);
-  const int swz = BK * 2;
-
-  int nt = 0;
-  if (a->stride == 1) {
-    for (int s = 0; s < nsrc; ++s)
-      if (int r = encode_nhwc_view(&p.tmA[s], a->x[s], N, H, W, a->cin[s], 0, a->cin[s], -1, -1, BK,
-                                   halo ? kHaloW : p.bw, halo ? kHaloH : p.bh, p.bn, swz)) return r;
-    for (int ky = 0; ky < a->ksize; ++ky)
-      for (int kx = 0; kx < a->ksize; ++kx)
-        for (int s = 0; s < nsrc; ++s) {
-          TapDesc& t = p.taps[nt++];
-          t.src = s; t.dx = kx - pad; t.dy = ky - pad; t.nchunks = a->cin[s] / BK;
-          t.wk0 = (s == 0) ? 0 : a->cin[0]; t.wtap = ky * a->ksize + kx;
-        }
-  } else {
-    Tap1D ty[3], tx[3];
-    const int ny = fwd_s2_taps(a->ksize, ty), nx = fwd_s2_taps(a->ksize, tx);
-    bool used[4] = {false, false, false, false};
-    for (int i = 0; i < ny; ++i)
-      for (int j = 0; j < nx; ++j) {
-        TapDesc& t = p.taps[nt++];
-        t.src = ty[i].parity * 2 + tx[j].parity; used[t.src] = true;
-        t.dx = tx[j].d; t.dy = ty[i].d; t.nchunks = a->cin[0] / BK; t.wk0 = 0;
-        t.wtap = ty[i].k * a->ksize + tx[j].k;
-      }
-    for (int v = 0; v < 4; ++v)
-      if (used[v])
-        if (int r = encode_nhwc_view(&p.tmA[v], a->x[0], N, H, W, a->cin[0], 0, a->cin[0], v >> 1, v & 1, BK, p.bw,
-                                     p.bh, p.bn, swz)) return r;
-  }
-  p.tap_start[0] = 0; p.tap_count[0] = nt;
-  if (int r = encode_weight(&p.tmB, a->weight, a->ksize * a->ksize, a->cout, cin_total, BK, BN, swz)) return r;
-  const int out_cw = BN >= 64 ? 64 : 32;
-  if (int r = encode_nhwc_view(&p.tmD[0], a->y, N, Ho, Wo, a->cout, 0, a->cout, -1, -1, out_cw, p.bw, p.bh, p.bn,
-                               out_cw * 2)) return r;
-  p.bias = a->bias; p.relu = a->relu; p.stats = a->stats; p.stats_c = a->cout;
-  p.scale = a->scale;
-  p.b_resident = (halo && nsrc == 1 && a->cin[0] == BK && env_int("MCB_BRES", 0) == 1) ? 1 : 0;
-  if (a->residual) {
-    p.residual = static_cast<const __nv_bfloat16*>(a->residual);
-    p.mask_H = Ho; p.mask_W = Wo; p.mask_C = a->cout; p.mask_s = 1;
-  }
-  return launch_conv(BN, BK, false, p, (int)m_tiles, a->cout / BN, 1, st, halo);
-}
-
-// =====================================================================================================
-extern "C" int mcb_conv_dgrad(const mcb_conv_dgrad_args* a, void* stream) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  MCB_REQUIRE(a && a->dy && a->weight && a->dx, "conv_dgrad: null pointer");
-  MCB_REQUIRE(a->ksize == 1 || a->ksize == 3, "conv_dgrad: ksize %d", a->ksize);
-  MCB_REQUIRE(a->stride == 1 || a->stride == 2, "conv_dgrad: stride %d", a->stride);
-  MCB_REQUIRE(!(a->relu_mask && a->accumulate), "conv_dgrad: relu_mask with accumulate is ill-defined");
-  MCB_REQUIRE(!(a->relu_mask && a->bn_z), "conv_dgrad: with bn_z the mask is derived from bn_z (relu_mask must be NULL)");
-  if (int r = check_c(a->cout, "conv_dgrad dy")) return r;
-  if (int r = check_c(a->cin, "conv_dgrad dx")) return r;
-  const int H = a->h, W = a->w, N = a->n;
-  const int Ho = H / a->stride, Wo = W / a->stride;
-  const int pad = a->ksize / 2;
-  const int BK = (a->cout % 64 == 0) ? 64 : 32;  // GEMM-K is cout here
-
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  const int Wv = (a->stride == 1) ? W : W / 2, Hv = (a->stride == 1) ? H : H / 2;
-  const bool halo = use_halo(a->ksize, a->stride, Wv, Hv, a->cout);
+    if (a[s].c % 64 != 0) BK = 32;
+  const bool halo = use_halo(rule.ksize, rule.stride, Wv, Hv, nsrc == 2 ? std::min(a[0].c, a[1].c) : a[0].c);
   if (halo) { p.bw = 8; p.bh = 16; p.bn = 1; }
   else pick_tile(Wv, Hv, N, 128, 1, &p.bw, &p.bh, &p.bn);
   p.rows = p.bw * p.bh * p.bn;
@@ -306,176 +236,43 @@ extern "C" int mcb_conv_dgrad(const mcb_conv_dgrad_args* a, void* stream) {
   p.tiles_x = (Wv + p.bw - 1) / p.bw;
   p.tiles_y = (Hv + p.bh - 1) / p.bh;
   const long m_tiles = (long)p.tiles_x * p.tiles_y * ((N + p.bn - 1) / p.bn);
-  int phases = 1;
-  int nt = 0;
-  if (int r = encode_nhwc_view(&p.tmA[0], a->dy, N, Ho, Wo, a->cout, 0, a->cout, -1, -1, BK, halo ? kHaloW : p.bw,
-                               halo ? kHaloH : p.bh, p.bn, BK * 2)) return r;
-  int phase_map[4] = {0, 0, 0, 0};  // launch phase -> (py*2+px)
-  if (a->stride == 1) {
-    for (int ky = 0; ky < a->ksize; ++ky)
-      for (int kx = 0; kx < a->ksize; ++kx) {
+
+  bool used[4] = {false, false, false, false};  // A slots the taps read
+  int phases = 0, nt = 0, phase_slot[4];
+  for (int v = 0; v < (phased ? 4 : 1); ++v) {
+    const int start = nt;
+    // y, then x, then the concat source (the HALO producer indexes tap_begin + t * nsrc + s); concat sources come only
+    // with stride-1 gathers, whose taps all read slot 0
+    for_each_tap(rule, v >> 1, v & 1, [&](int slot, int dx, int dy, int wtap) {
+      for (int s = 0; s < nsrc; ++s) {
         TapDesc& t = p.taps[nt++];
-        t.src = 0; t.dx = pad - kx; t.dy = pad - ky; t.nchunks = a->cout / BK; t.wk0 = 0; t.wtap = ky * a->ksize + kx;
+        t.src = slot + s; t.dx = dx; t.dy = dy; t.nchunks = a[s].c / BK; t.wk0 = s == 0 ? 0 : a[0].c; t.wtap = wtap;
+        used[slot + s] = true;
       }
-    p.tap_start[0] = 0; p.tap_count[0] = nt;
-  } else {
-    MCB_REQUIRE(H % 2 == 0 && W % 2 == 0, "conv_dgrad: stride 2 needs even H, W");
-    phases = 0;
-    for (int py = 0; py < 2; ++py)
-      for (int px = 0; px < 2; ++px) {
-        Tap1D ty[2], tx[2];
-        const int ny = dgrad_s2_taps(a->ksize, py, ty), nx = dgrad_s2_taps(a->ksize, px, tx);
-        if (ny * nx == 0) continue;
-        p.tap_start[phases] = nt;
-        for (int i = 0; i < ny; ++i)
-          for (int j = 0; j < nx; ++j) {
-            TapDesc& t = p.taps[nt++];
-            t.src = 0; t.dx = tx[j].d; t.dy = ty[i].d; t.nchunks = a->cout / BK; t.wk0 = 0;
-            t.wtap = ty[i].k * a->ksize + tx[j].k;
-          }
-        p.tap_count[phases] = nt - p.tap_start[phases];
-        phase_map[phases] = py * 2 + px;
-        ++phases;
-      }
-    if (a->ksize == 1 && !a->accumulate) {
-      // only the (even, even) input pixels receive gradient; the rest is zero
-      MCB_CHECK_CUDA(cudaMemsetAsync(a->dx, 0, (size_t)N * H * W * a->cin * 2, st));
-    }
+    });
+    if (nt == start) continue;
+    p.tap_start[phases] = start; p.tap_count[phases] = nt - start;
+    phase_slot[phases++] = phased ? v : -1;
   }
-  // the kernel derives the mask parity from blockIdx.z as (py, px) = (z >> 1, z & 1); with all four phases present
-  // (3x3) launch order == parity order; the 1x1 case has the single phase (0,0).
-  const int BN = pick_bn(a->cin, m_tiles, phases);
-  const int bmn_cw = BN >= 64 ? 64 : 32;
-  // MN-major B: weight slice [taps][cout][ci_off : ci_off + cin] viewed as (cin inner = N, cout = K rows, taps),
-  // row pitch cin_total; box (bmn_cw, BK, 1)
-  {
-    const char* wb = static_cast<const char*>(a->weight) + (size_t)a->ci_off * 2;
-    uint64_t dims[3] = {(uint64_t)a->cin, (uint64_t)a->cout, (uint64_t)(a->ksize * a->ksize)};
-    uint64_t str[2] = {(uint64_t)a->cin_total * 2, (uint64_t)a->cin_total * a->cout * 2};
-    uint32_t box[3] = {(uint32_t)bmn_cw, (uint32_t)BK, 1};
-    if (int r = encode_tmap(&p.tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, wb, dims, str, box, bmn_cw * 2)) return r;
-  }
-  const int out_cw = BN >= 64 ? 64 : 32;
-  const void* aux = a->bn_z ? a->bn_z : a->relu_mask;  // tensor with the geometry of dx, tiled like the output
-  for (int ph = 0; ph < phases; ++ph) {
-    const int py = (a->stride == 1) ? -1 : (phase_map[ph] >> 1), px = (a->stride == 1) ? -1 : (phase_map[ph] & 1);
-    if (int r = encode_nhwc_view(&p.tmD[ph], a->dx, N, H, W, a->cin, 0, a->cin, py, px, out_cw, p.bw, p.bh, p.bn,
-                                 out_cw * 2)) return r;
-    if (aux)
-      if (int r = encode_nhwc_view(&p.tmX[ph], aux, N, H, W, a->cin, 0, a->cin, py, px, out_cw, p.bw, p.bh, p.bn,
-                                   out_cw * 2)) return r;
-  }
-  p.accumulate = a->accumulate;
-  p.b_resident = (halo && a->cout == BK && env_int("MCB_BRES", 0) == 1) ? 1 : 0;
-  p.aux_mode = a->bn_z ? 2 : (a->relu_mask ? 1 : 0);
-  MCB_REQUIRE(!(a->dx_channel_sum && (!a->relu_mask || a->accumulate)),
-              "conv_dgrad: dx_channel_sum needs relu_mask and a complete (non-accumulated) gradient");
-  if (a->dx_channel_sum) p.bn_dbeta = a->dx_channel_sum;
-  if (a->bn_z) {
-    MCB_REQUIRE(a->bn_mean && a->bn_invstd && a->bn_gamma && a->bn_beta && a->bn_dbeta && a->bn_dgamma,
-                "conv_dgrad: incomplete bn reduction args");
-    MCB_REQUIRE(!a->accumulate, "conv_dgrad: bn reduction needs the complete gradient (no accumulate)");
-    MCB_REQUIRE(!(a->stride == 2 && a->ksize == 1), "conv_dgrad: bn reduction with a 1x1 stride-2 conv is unsupported");
-    p.bn_mean = a->bn_mean; p.bn_invstd = a->bn_invstd; p.bn_gamma = a->bn_gamma; p.bn_beta = a->bn_beta;
-    p.bn_dbeta = a->bn_dbeta; p.bn_dgamma = a->bn_dgamma;
-  }
-  return launch_conv(BN, BK, true, p, (int)m_tiles, a->cin / BN, phases, st, halo);
-}
-
-// =====================================================================================================
-extern "C" int mcb_convt_fwd(const mcb_convt_fwd_args* a, void* stream) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  MCB_REQUIRE(a && a->x && a->weight && a->y, "convt_fwd: null pointer");
-  if (int r = check_c(a->cin, "convt_fwd input")) return r;
-  if (int r = check_c(a->cout, "convt_fwd output")) return r;
-  const int K = convt_ksize(a->ksize);
-  MCB_REQUIRE(K == 3 || K == 4, "convt_fwd: ksize %d", a->ksize);
-  const int H = a->h, W = a->w, N = a->n;
-  const int BK = (a->cin % 64 == 0) ? 64 : 32;
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  pick_tile(W, H, N, 128, 1, &p.bw, &p.bh, &p.bn);
-  p.rows = p.bw * p.bh * p.bn;
-  p.Wv = W; p.Hv = H; p.Nimg = N;
-  p.tiles_x = (W + p.bw - 1) / p.bw;
-  p.tiles_y = (H + p.bh - 1) / p.bh;
-  const long m_tiles = (long)p.tiles_x * p.tiles_y * ((N + p.bn - 1) / p.bn);
-  const int BN = pick_bn(a->cout, m_tiles, 4);
-  if (int r = encode_nhwc_view(&p.tmA[0], a->x, N, H, W, a->cin, 0, a->cin, -1, -1, BK, p.bw, p.bh, p.bn, BK * 2))
-    return r;
-  int nt = 0;
-  for (int py = 0; py < 2; ++py)
-    for (int px = 0; px < 2; ++px) {
-      const int ph = py * 2 + px;
-      Tap1D ty[2], tx[2];
-      const int ny = convt_fwd_taps(K, py, ty), nx = convt_fwd_taps(K, px, tx);
-      p.tap_start[ph] = nt;
-      for (int i = 0; i < ny; ++i)
-        for (int j = 0; j < nx; ++j) {
-          TapDesc& t = p.taps[nt++];
-          t.src = 0; t.dx = tx[j].d; t.dy = ty[i].d; t.nchunks = a->cin / BK; t.wk0 = 0; t.wtap = ty[i].k * K + tx[j].k;
-        }
-      p.tap_count[ph] = nt - p.tap_start[ph];
-      const int out_cw = BN >= 64 ? 64 : 32;
-      if (int r = encode_nhwc_view(&p.tmD[ph], a->y, N, 2 * H, 2 * W, a->cout, 0, a->cout, py, px, out_cw, p.bw, p.bh,
-                                   p.bn, out_cw * 2)) return r;
-    }
-  if (int r = encode_weight(&p.tmB, a->weight, K * K, a->cout, a->cin, BK, BN, BK * 2)) return r;
-  p.bias = a->bias; p.relu = a->relu;
-  return launch_conv(BN, BK, false, p, (int)m_tiles, a->cout / BN, 4, st);
-}
-
-extern "C" int mcb_convt_dgrad(const mcb_convt_dgrad_args* a, void* stream) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  MCB_REQUIRE(a && a->dy && a->weight && a->dx, "convt_dgrad: null pointer");
-  MCB_REQUIRE(!(a->relu_mask && a->accumulate), "convt_dgrad: relu_mask with accumulate is ill-defined");
-  if (int r = check_c(a->cin, "convt_dgrad dx")) return r;
-  if (int r = check_c(a->cout, "convt_dgrad dy")) return r;
-  const int K = convt_ksize(a->ksize);
-  MCB_REQUIRE(K == 3 || K == 4, "convt_dgrad: ksize %d", a->ksize);
-  const int H = a->h, W = a->w, N = a->n;  // input (dx) dims; dy is 2H x 2W
-  const int BK = (a->cout % 64 == 0) ? 64 : 32;
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  pick_tile(W, H, N, 128, 1, &p.bw, &p.bh, &p.bn);
-  p.rows = p.bw * p.bh * p.bn;
-  p.Wv = W; p.Hv = H; p.Nimg = N;
-  p.tiles_x = (W + p.bw - 1) / p.bw;
-  p.tiles_y = (H + p.bh - 1) / p.bh;
-  const long m_tiles = (long)p.tiles_x * p.tiles_y * ((N + p.bn - 1) / p.bn);
-  const int BN = pick_bn(a->cin, m_tiles, 1);
   for (int v = 0; v < 4; ++v)
-    if (int r = encode_nhwc_view(&p.tmA[v], a->dy, N, 2 * H, 2 * W, a->cout, 0, a->cout, v >> 1, v & 1, BK, p.bw,
-                                 p.bh, p.bn, BK * 2)) return r;
-  Tap1D t1[4];
-  const int n1 = convt_dgrad_taps(K, t1);
-  int nt = 0;
-  for (int i = 0; i < n1; ++i)
-    for (int j = 0; j < n1; ++j) {
-      TapDesc& t = p.taps[nt++];
-      t.src = t1[i].parity * 2 + t1[j].parity; t.dx = t1[j].d; t.dy = t1[i].d; t.nchunks = a->cout / BK; t.wk0 = 0;
-      t.wtap = t1[i].k * K + t1[j].k;
-    }
-  p.tap_start[0] = 0; p.tap_count[0] = nt;
-  const int bmn_cw = BN >= 64 ? 64 : 32;
-  if (int r = encode_weight(&p.tmB, a->weight, K * K, a->cout, a->cin, bmn_cw, BK, bmn_cw * 2)) return r;
-  const int out_cw = BN >= 64 ? 64 : 32;
-  if (int r = encode_nhwc_view(&p.tmD[0], a->dx, N, H, W, a->cin, 0, a->cin, -1, -1, out_cw, p.bw, p.bh, p.bn,
-                               out_cw * 2)) return r;
-  p.accumulate = a->accumulate;
-  if (a->relu_mask) {
-    if (int r = encode_nhwc_view(&p.tmX[0], a->relu_mask, N, H, W, a->cin, 0, a->cin, -1, -1, out_cw, p.bw, p.bh, p.bn,
-                                 out_cw * 2)) return r;
-    p.aux_mode = 1;
-  }
-  MCB_REQUIRE(!(a->dx_channel_sum && (!a->relu_mask || a->accumulate)),
-              "convt_dgrad: dx_channel_sum needs relu_mask and a complete (non-accumulated) gradient");
-  p.bn_dbeta = a->dx_channel_sum;
-  return launch_conv(BN, BK, true, p, (int)m_tiles, a->cin / BN, 1, st);
-}
+    if (used[v])
+      if (int r = encode_view(&p.tmA[v], a[parity_a ? 0 : v], parity_a ? v : -1, BK, halo ? kHaloW : p.bw,
+                              halo ? kHaloH : p.bh, p.bn)) return r;
 
-// =====================================================================================================
-namespace mcb {
+  const int BN = pick_bn(out.c, m_tiles, phases);
+  const int cw = BN >= 64 ? 64 : 32;  // channel width of the output / aux boxes and of the MN-major weight box
+  const int wtaps = rule.ksize * rule.ksize;
+  if (int r = b_mn ? encode_weight(&p.tmB, w, wtaps, a[0].c, w_pitch, w_off, out.c, cw, BK)
+                   : encode_weight(&p.tmB, w, wtaps, out.c, w_pitch, 0, w_pitch, BK, BN)) return r;
+  const View aux_view = {aux, out.n, out.h, out.w, out.c};
+  for (int ph = 0; ph < phases; ++ph) {
+    if (int r = encode_view(&p.tmD[ph], out, phase_slot[ph], cw, p.bw, p.bh, p.bn)) return r;
+    if (aux)
+      if (int r = encode_view(&p.tmX[ph], aux_view, phase_slot[ph], cw, p.bw, p.bh, p.bn)) return r;
+  }
+  p.b_resident = (halo && nsrc == 1 && a[0].c == BK && env_int("MCB_BRES", 0) == 1) ? 1 : 0;
+  return launch_conv(BN, BK, b_mn, p, (int)m_tiles, out.c / BN, phases, st, halo);
+}
 
 template <int BN>
 static int launch_wgrad_inst(const WgradParams& p, dim3 grid, size_t smem, cudaStream_t st) {
@@ -565,7 +362,7 @@ static int launch_wgrad(WgradParams& p, int cin_src, cudaStream_t st) {
   return MCB_OK;
 }
 
-static int wgrad_common_setup(WgradParams& p, int Wv, int Hv, int N, int cout, int cin_src) {
+static int wgrad_common_setup(WgradParams& p, int Wv, int Hv, int N, int cout) {
   pick_tile(Wv, Hv, N, 64, 16, &p.bw, &p.bh, &p.bn);
   p.rows = p.bw * p.bh * p.bn;
   if (p.rows % 16 != 0 || p.rows > 64) return fail(MCB_ERR_UNSUPPORTED, "wgrad: no pixel box for %dx%dx%d", Wv, Hv, N);
@@ -575,88 +372,172 @@ static int wgrad_common_setup(WgradParams& p, int Wv, int Hv, int N, int cout, i
   p.tiles_total = p.tiles_x * p.tiles_y * ((N + p.bn - 1) / p.bn);
   p.a_cw = (cout % 64 == 0) ? 64 : 32;
   p.a_chunks = (cout >= 128) ? 2 : 1;
-  (void)cin_src;
   return MCB_OK;
+}
+
+// One wgrad_kernel launch: dW[tap][cout][ci_off + ci] += sum over pixels of dy[.., cout] x[.., ci] at the offsets of the
+// taps of `rule` (a gather).  The taps read x for a conv weight gradient and dy for a transposed-conv one (through the
+// stride-2 conv over dy that is its data gradient); the other operand is read plainly and the pixel tiles cover it.
+// The caller has set dw, cout, cin_total and ci_off.
+static int plan_wgrad(WgradParams& p, const TapRule& rule, const View& dy, const View& x, bool taps_on_dy,
+                      cudaStream_t st) {
+  const View& plain = taps_on_dy ? x : dy;
+  if (int r = wgrad_common_setup(p, plain.w, plain.h, plain.n, dy.c)) return r;
+  bool used_a[4] = {!taps_on_dy, false, false, false}, used_b[4] = {taps_on_dy, false, false, false};
+  bool* used = taps_on_dy ? used_a : used_b;
+  int nt = 0;
+  for_each_tap(rule, 0, 0, [&](int slot, int ox, int oy, int wtap) {
+    WgradTap& t = p.taps[nt++];
+    if (taps_on_dy) { t.srcA = slot; t.ax = ox; t.ay = oy; }
+    else { t.srcB = slot; t.bx = ox; t.by = oy; }
+    t.wtap = wtap;
+    used[slot] = true;
+  });
+  p.ntaps = nt;
+  const bool parity = rule.stride == 2;
+  const int b_cw = (x.c % 64 == 0) ? 64 : 32;
+  for (int v = 0; v < 4; ++v) {
+    if (used_a[v])
+      if (int r = encode_view(&p.tmA[v], dy, taps_on_dy && parity ? v : -1, p.a_cw, p.bw, p.bh, p.bn)) return r;
+    if (used_b[v])
+      if (int r = encode_view(&p.tmB[v], x, !taps_on_dy && parity ? v : -1, b_cw, p.bw, p.bh, p.bn)) return r;
+  }
+  return launch_wgrad(p, x.c, st);
 }
 
 }  // namespace mcb
 
-extern "C" int mcb_conv_wgrad(const mcb_conv_wgrad_args* a, void* stream) {
+using namespace mcb;
+
+// =====================================================================================================
+extern "C" int mcb_conv_fwd(const mcb_conv_fwd_args* a, void* stream) {
+  MCB_REQUIRE(a && a->x[0] && a->weight && a->y, "conv_fwd: null pointer");
+  MCB_REQUIRE(a->ksize == 1 || a->ksize == 3, "conv_fwd: ksize %d", a->ksize);
+  MCB_REQUIRE(a->stride == 1 || a->stride == 2, "conv_fwd: stride %d", a->stride);
+  const int nsrc = a->x[1] ? 2 : 1;
+  MCB_REQUIRE(!(nsrc == 2 && a->stride == 2), "conv_fwd: concat + stride 2 unsupported");
+  for (int s = 0; s < nsrc; ++s)
+    if (int r = check_c(a->cin[s], "conv_fwd input")) return r;
+  if (int r = check_c(a->cout, "conv_fwd output")) return r;
+  MCB_REQUIRE(!(nsrc == 2 && (a->cin[0] % 64 != 0 || a->cin[1] % 64 != 0)), "conv_fwd: 32-channel concat unsupported");
+  MCB_REQUIRE(a->stride == 1 || (a->h % 2 == 0 && a->w % 2 == 0), "conv_fwd: stride 2 needs even H, W");
+  const int Ho = a->h / a->stride, Wo = a->w / a->stride;
+  const View x[2] = {{a->x[0], a->n, a->h, a->w, a->cin[0]}, {a->x[1], a->n, a->h, a->w, a->cin[1]}};
+
+  ConvGemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.bias = a->bias; p.relu = a->relu; p.stats = a->stats; p.stats_c = a->cout;
+  p.scale = a->scale;
+  if (a->residual) {
+    p.residual = static_cast<const __nv_bfloat16*>(a->residual);
+    p.mask_H = Ho; p.mask_W = Wo; p.mask_C = a->cout; p.mask_s = 1;
+  }
+  return plan_conv(p, {a->ksize, a->ksize / 2, a->stride}, x, nsrc, {a->y, a->n, Ho, Wo, a->cout}, nullptr, a->weight,
+                   a->cin[0] + (nsrc == 2 ? a->cin[1] : 0), 0, false, static_cast<cudaStream_t>(stream));
+}
+
+// =====================================================================================================
+extern "C" int mcb_conv_dgrad(const mcb_conv_dgrad_args* a, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  MCB_REQUIRE(a && a->dy && a->weight && a->dx, "conv_dgrad: null pointer");
+  MCB_REQUIRE(a->ksize == 1 || a->ksize == 3, "conv_dgrad: ksize %d", a->ksize);
+  MCB_REQUIRE(a->stride == 1 || a->stride == 2, "conv_dgrad: stride %d", a->stride);
+  MCB_REQUIRE(!(a->relu_mask && a->accumulate), "conv_dgrad: relu_mask with accumulate is ill-defined");
+  MCB_REQUIRE(!(a->relu_mask && a->bn_z), "conv_dgrad: with bn_z the mask is derived from bn_z (relu_mask must be NULL)");
+  if (int r = check_c(a->cout, "conv_dgrad dy")) return r;
+  if (int r = check_c(a->cin, "conv_dgrad dx")) return r;
+  MCB_REQUIRE(a->stride == 1 || (a->h % 2 == 0 && a->w % 2 == 0), "conv_dgrad: stride 2 needs even H, W");
+  MCB_REQUIRE(!(a->dx_channel_sum && (!a->relu_mask || a->accumulate)),
+              "conv_dgrad: dx_channel_sum needs relu_mask and a complete (non-accumulated) gradient");
+  if (a->bn_z) {
+    MCB_REQUIRE(a->bn_mean && a->bn_invstd && a->bn_gamma && a->bn_beta && a->bn_dbeta && a->bn_dgamma,
+                "conv_dgrad: incomplete bn reduction args");
+    MCB_REQUIRE(!a->accumulate, "conv_dgrad: bn reduction needs the complete gradient (no accumulate)");
+    MCB_REQUIRE(!(a->stride == 2 && a->ksize == 1), "conv_dgrad: bn reduction with a 1x1 stride-2 conv is unsupported");
+  }
+
+  ConvGemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.accumulate = a->accumulate;
+  p.aux_mode = a->bn_z ? 2 : (a->relu_mask ? 1 : 0);
+  p.bn_dbeta = a->dx_channel_sum;
+  if (a->bn_z) {
+    p.bn_mean = a->bn_mean; p.bn_invstd = a->bn_invstd; p.bn_gamma = a->bn_gamma; p.bn_beta = a->bn_beta;
+    p.bn_dbeta = a->bn_dbeta; p.bn_dgamma = a->bn_dgamma;
+  }
+  if (a->stride == 2 && a->ksize == 1 && !a->accumulate) {
+    // only the (even, even) input pixels receive gradient; the rest is zero
+    MCB_CHECK_CUDA(cudaMemsetAsync(a->dx, 0, (size_t)a->n * a->h * a->w * a->cin * 2, st));
+  }
+  const View dy = {a->dy, a->n, a->h / a->stride, a->w / a->stride, a->cout};
+  // aux: the tensor the ReLU mask is derived from
+  return plan_conv(p, {a->ksize, a->ksize / 2, a->stride, true}, &dy, 1, {a->dx, a->n, a->h, a->w, a->cin},
+                   a->bn_z ? a->bn_z : a->relu_mask, a->weight, a->cin_total, a->ci_off, true, st);
+}
+
+// =====================================================================================================
+// ConvTranspose2d(ksize, stride 2, padding 1): four sub-pixel phases, the data gradient of a stride-2 conv.  ksize 3
+// (output_padding 1, same 2x output) reads the zero row past the bottom / right edge (TMA out-of-bounds fill).
+extern "C" int mcb_convt_fwd(const mcb_convt_fwd_args* a, void* stream) {
+  MCB_REQUIRE(a && a->x && a->weight && a->y, "convt_fwd: null pointer");
+  if (int r = check_c(a->cin, "convt_fwd input")) return r;
+  if (int r = check_c(a->cout, "convt_fwd output")) return r;
+  const int K = convt_ksize(a->ksize);
+  MCB_REQUIRE(K == 3 || K == 4, "convt_fwd: ksize %d", a->ksize);
+  const View x = {a->x, a->n, a->h, a->w, a->cin};
+  ConvGemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.bias = a->bias; p.relu = a->relu;
+  // the 3x3 kernel sums the two taps of an odd parity as k = 2, then k = 0
+  return plan_conv(p, {K, 1, 2, true, K == 3}, &x, 1, {a->y, a->n, 2 * a->h, 2 * a->w, a->cout}, nullptr, a->weight,
+                   a->cin, 0, false, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int mcb_convt_dgrad(const mcb_convt_dgrad_args* a, void* stream) {
+  MCB_REQUIRE(a && a->dy && a->weight && a->dx, "convt_dgrad: null pointer");
+  MCB_REQUIRE(!(a->relu_mask && a->accumulate), "convt_dgrad: relu_mask with accumulate is ill-defined");
+  if (int r = check_c(a->cin, "convt_dgrad dx")) return r;
+  if (int r = check_c(a->cout, "convt_dgrad dy")) return r;
+  const int K = convt_ksize(a->ksize);
+  MCB_REQUIRE(K == 3 || K == 4, "convt_dgrad: ksize %d", a->ksize);
+  MCB_REQUIRE(!(a->dx_channel_sum && (!a->relu_mask || a->accumulate)),
+              "convt_dgrad: dx_channel_sum needs relu_mask and a complete (non-accumulated) gradient");
+  const View dy = {a->dy, a->n, 2 * a->h, 2 * a->w, a->cout};  // dx is h x w
+  ConvGemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.accumulate = a->accumulate;
+  p.aux_mode = a->relu_mask ? 1 : 0;
+  p.bn_dbeta = a->dx_channel_sum;
+  return plan_conv(p, {K, 1, 2}, &dy, 1, {a->dx, a->n, a->h, a->w, a->cin}, a->relu_mask, a->weight, a->cin, 0, true,
+                   static_cast<cudaStream_t>(stream));
+}
+
+// =====================================================================================================
+extern "C" int mcb_conv_wgrad(const mcb_conv_wgrad_args* a, void* stream) {
   MCB_REQUIRE(a && a->dy && a->x && a->dw, "conv_wgrad: null pointer");
   MCB_REQUIRE(a->ksize == 1 || a->ksize == 3, "conv_wgrad: ksize %d", a->ksize);
   MCB_REQUIRE(a->stride == 1 || a->stride == 2, "conv_wgrad: stride %d", a->stride);
   if (int r = check_c(a->cout, "conv_wgrad dy")) return r;
   if (int r = check_c(a->cin, "conv_wgrad x")) return r;
   MCB_REQUIRE(a->cout % 128 == 0 || a->cout == 64 || a->cout == 32, "conv_wgrad: cout %d", a->cout);
-  const int H = a->h, W = a->w, N = a->n;
-  const int Ho = H / a->stride, Wo = W / a->stride;
-  const int pad = a->ksize / 2;
+  MCB_REQUIRE(a->stride == 1 || (a->h % 2 == 0 && a->w % 2 == 0), "conv_wgrad: stride 2 needs even H, W");
   WgradParams p;
   memset(&p, 0, sizeof(p));
-  if (int r = wgrad_common_setup(p, Wo, Ho, N, a->cout, a->cin)) return r;
-  const int b_cw = (a->cin % 64 == 0) ? 64 : 32;
-  if (int r = encode_nhwc_view(&p.tmA[0], a->dy, N, Ho, Wo, a->cout, 0, a->cout, -1, -1, p.a_cw, p.bw, p.bh, p.bn,
-                               p.a_cw * 2)) return r;
-  int nt = 0;
-  if (a->stride == 1) {
-    if (int r = encode_nhwc_view(&p.tmB[0], a->x, N, H, W, a->cin, 0, a->cin, -1, -1, b_cw, p.bw, p.bh, p.bn,
-                                 b_cw * 2)) return r;
-    for (int ky = 0; ky < a->ksize; ++ky)
-      for (int kx = 0; kx < a->ksize; ++kx) {
-        WgradTap& t = p.taps[nt++];
-        t.srcA = 0; t.ax = 0; t.ay = 0; t.srcB = 0; t.bx = kx - pad; t.by = ky - pad; t.wtap = ky * a->ksize + kx;
-      }
-  } else {
-    MCB_REQUIRE(H % 2 == 0 && W % 2 == 0, "conv_wgrad: stride 2 needs even H, W");
-    Tap1D ty[3], tx[3];
-    const int ny = fwd_s2_taps(a->ksize, ty), nx = fwd_s2_taps(a->ksize, tx);
-    bool used[4] = {false, false, false, false};
-    for (int i = 0; i < ny; ++i)
-      for (int j = 0; j < nx; ++j) {
-        WgradTap& t = p.taps[nt++];
-        t.srcA = 0; t.ax = 0; t.ay = 0;
-        t.srcB = ty[i].parity * 2 + tx[j].parity; used[t.srcB] = true;
-        t.bx = tx[j].d; t.by = ty[i].d; t.wtap = ty[i].k * a->ksize + tx[j].k;
-      }
-    for (int v = 0; v < 4; ++v)
-      if (used[v])
-        if (int r = encode_nhwc_view(&p.tmB[v], a->x, N, H, W, a->cin, 0, a->cin, v >> 1, v & 1, b_cw, p.bw, p.bh,
-                                     p.bn, b_cw * 2)) return r;
-  }
-  p.ntaps = nt;
   p.dw = a->dw; p.cout = a->cout; p.cin_total = a->cin_total; p.ci_off = a->ci_off;
-  return launch_wgrad(p, a->cin, st);
+  const View dy = {a->dy, a->n, a->h / a->stride, a->w / a->stride, a->cout}, x = {a->x, a->n, a->h, a->w, a->cin};
+  return plan_wgrad(p, {a->ksize, a->ksize / 2, a->stride}, dy, x, false, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int mcb_convt_wgrad(const mcb_convt_wgrad_args* a, void* stream) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   MCB_REQUIRE(a && a->dy && a->x && a->dw, "convt_wgrad: null pointer");
   if (int r = check_c(a->cout, "convt_wgrad dy")) return r;
   if (int r = check_c(a->cin, "convt_wgrad x")) return r;
   MCB_REQUIRE(a->cout % 128 == 0 || a->cout == 64 || a->cout == 32, "convt_wgrad: cout %d", a->cout);
   const int K = convt_ksize(a->ksize);
   MCB_REQUIRE(K == 3 || K == 4, "convt_wgrad: ksize %d", a->ksize);
-  const int H = a->h, W = a->w, N = a->n;  // input dims; dy is 2H x 2W
   WgradParams p;
   memset(&p, 0, sizeof(p));
-  if (int r = wgrad_common_setup(p, W, H, N, a->cout, a->cin)) return r;
-  const int b_cw = (a->cin % 64 == 0) ? 64 : 32;
-  for (int v = 0; v < 4; ++v)
-    if (int r = encode_nhwc_view(&p.tmA[v], a->dy, N, 2 * H, 2 * W, a->cout, 0, a->cout, v >> 1, v & 1, p.a_cw, p.bw,
-                                 p.bh, p.bn, p.a_cw * 2)) return r;
-  if (int r = encode_nhwc_view(&p.tmB[0], a->x, N, H, W, a->cin, 0, a->cin, -1, -1, b_cw, p.bw, p.bh, p.bn, b_cw * 2))
-    return r;
-  Tap1D t1[4];
-  const int n1 = convt_dgrad_taps(K, t1);
-  int nt = 0;
-  for (int i = 0; i < n1; ++i)
-    for (int j = 0; j < n1; ++j) {
-      WgradTap& t = p.taps[nt++];
-      t.srcA = t1[i].parity * 2 + t1[j].parity; t.ax = t1[j].d; t.ay = t1[i].d;
-      t.srcB = 0; t.bx = 0; t.by = 0; t.wtap = t1[i].k * K + t1[j].k;
-    }
-  p.ntaps = nt;
   p.dw = a->dw; p.cout = a->cout; p.cin_total = a->cin; p.ci_off = 0;
-  return launch_wgrad(p, a->cin, st);
+  const View dy = {a->dy, a->n, 2 * a->h, 2 * a->w, a->cout}, x = {a->x, a->n, a->h, a->w, a->cin};
+  return plan_wgrad(p, {K, 1, 2}, dy, x, true, static_cast<cudaStream_t>(stream));
 }
