@@ -207,9 +207,11 @@ int mcb_final_conv_fwd(const void* x, const float* w, const float* b, float* log
 int mcb_final_conv_bwd(const void* x, const float* w, const float* dlogits, void* dx, float* dw, float* db, int n,
                        int h, int wd, int c, int k, void* stream);
 
-/* torch.optim.Adam with L2 (src/models.py:57,287-292) over one flat fp32 arena; refreshes the bf16 operand copy */
-int mcb_adam_step(float* p, const float* g, float* m, float* v, void* p_bf16, long n, float lr, float beta1,
-                  float beta2, float eps, float weight_decay, int step, float grad_scale, void* stream);
+/* torch.optim.Adam with L2 (src/models.py:57,287-292) over one flat fp32 arena; refreshes the bf16 operand copy.
+   The betas are double: the bias corrections 1 - beta^t are taken from them in double, as torch does; the moment
+   updates use them rounded to fp32 */
+int mcb_adam_step(float* p, const float* g, float* m, float* v, void* p_bf16, long n, float lr, double beta1,
+                  double beta2, float eps, float weight_decay, int step, float grad_scale, void* stream);
 /* same update with the step-dependent scalars read from DEVICE memory: hyper = {lr, 1-beta1^t, sqrt(1-beta2^t)}
    (fp32[3]), so the launch can be captured once into a CUDA graph and replayed every step */
 int mcb_adam_step_dyn(float* p, const float* g, float* m, float* v, void* p_bf16, long n, const float* hyper,

@@ -97,7 +97,7 @@ _SIGS = {
     "mcb_maxpool2_bwd": [vp, vp, vp, ci, ci, ci, ci, ci, vp],
     "mcb_final_conv_fwd": [vp, vp, vp, vp, ci, ci, ci, ci, ci, vp],
     "mcb_final_conv_bwd": [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp],
-    "mcb_adam_step": [vp, vp, vp, vp, vp, cl, cf, cf, cf, cf, cf, ci, cf, vp],
+    "mcb_adam_step": [vp, vp, vp, vp, vp, cl, cf, C.c_double, C.c_double, cf, cf, ci, cf, vp],
     "mcb_adam_step_dyn": [vp, vp, vp, vp, vp, cl, vp, cf, cf, cf, cf, cf, vp],
     "mcb_cast_f32_bf16": [vp, vp, cl, vp],
     "mcb_loss_partials": [C.POINTER(LossArgs), vp, vp],

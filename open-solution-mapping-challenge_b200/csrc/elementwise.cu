@@ -893,15 +893,16 @@ extern "C" int mcb_final_conv_bwd(const void* x, const float* w, const float* dl
   return MCB_OK;
 }
 
-extern "C" int mcb_adam_step(float* p, const float* g, float* m, float* v, void* p_bf16, long n, float lr, float beta1,
-                             float beta2, float eps, float weight_decay, int step, float grad_scale, void* stream) {
+extern "C" int mcb_adam_step(float* p, const float* g, float* m, float* v, void* p_bf16, long n, float lr, double beta1,
+                             double beta2, float eps, float weight_decay, int step, float grad_scale, void* stream) {
   MCB_REQUIRE(p && g && m && v, "adam_step: null pointer");
   MCB_REQUIRE(step >= 1, "adam_step: step %d", step);
-  // bias corrections in double, like torch.optim.Adam's Python-side arithmetic
-  const double bc1 = 1.0 - pow((double)beta1, (double)step);
-  const double bc2 = 1.0 - pow((double)beta2, (double)step);
-  launch_pdl(adam_kernel, grid_for(n, 256), 256, 0, ST, p, g, m, v, (bf16*)p_bf16, n, lr, beta1, beta2, eps, weight_decay,
-                                                (float)bc1, (float)sqrt(bc2), grad_scale, (const float*)nullptr);
+  // bias corrections in double from the caller's (double) betas, like torch.optim.Adam's Python-side
+  // `1 - beta ** step` and `bias_correction2 ** 0.5`; mcb_adam_step_dyn's hyper carries the same values
+  const double bc1 = 1.0 - pow(beta1, (double)step);
+  const double bc2 = 1.0 - pow(beta2, (double)step);
+  launch_pdl(adam_kernel, grid_for(n, 256), 256, 0, ST, p, g, m, v, (bf16*)p_bf16, n, lr, (float)beta1, (float)beta2, eps,
+             weight_decay, (float)bc1, (float)pow(bc2, 0.5), grad_scale, (const float*)nullptr);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }

@@ -574,9 +574,7 @@ class FusedTrainStep:
                 raise RuntimeError("Adam betas / eps / weight_decay changed after the train step was captured")
             host, ev = self._hyper_ring[t % len(self._hyper_ring)]
             ev.synchronize()
-            host[0] = lr
-            host[1] = 1.0 - betas[0] ** t
-            host[2] = (1.0 - betas[1] ** t) ** 0.5
+            host[0], host[1], host[2] = ops.adam_hyper(lr, betas, t)
             self._hyper.copy_(host, non_blocking=True)
             ev.record()
         first = self.graphs is None and self.use_graphs

@@ -293,6 +293,13 @@ def adam_step(p, g, m, v, p_bf16, step, lr, betas=(0.9, 0.999), eps=1e-8, weight
             betas[0], betas[1], eps, weight_decay, int(step), grad_scale)
 
 
+def adam_hyper(lr, betas, step):
+    """[lr, 1 - beta1^t, (1 - beta2^t)^0.5] for adam_step_dyn's `hyper`: torch.optim.Adam's bias corrections, in
+    double from the caller's betas.  mcb_adam_step computes the same doubles on the host (pow(bc2, 0.5) included), so
+    both entry points give the same bits once the values are rounded to fp32."""
+    return [lr, 1.0 - betas[0] ** step, (1.0 - betas[1] ** step) ** 0.5]
+
+
 def adam_step_dyn(p, g, m, v, p_bf16, hyper, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, grad_scale=1.0):
     """Adam over a (slice of the) flat arena with {lr, 1-b1^t, sqrt(1-b2^t)} read from the device tensor `hyper`"""
     L.fcall("mcb_adam_step_dyn", p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), L.dp(p_bf16), p.numel(),

@@ -1,5 +1,7 @@
 """Unit parity of the HBM-bound kernels (csrc/elementwise.cu, csrc/loss.cu) against torch fp32 on the CPU — the ops
-the reference runs through torch (BatchNorm2d, MaxPool2d, Conv2d 7x7 / 1x1, CrossEntropy/Dice losses, Adam)."""
+the reference runs through torch (BatchNorm2d, MaxPool2d, Conv2d 7x7 / 1x1, CrossEntropy/Dice losses, Adam).
+The batch-32 sizes, where every thread of the capped grid-stride loops runs several iterations, are tested in
+tests/test_elementwise_scale_gpu.py."""
 import math
 
 import numpy as np
