@@ -152,6 +152,14 @@ int mcb_stem_im2col(const float* x_nchw, void* col, int n, int h, int w, void* s
 int mcb_stem_pack_weight(const float* w, void* w_packed, void* stream);
 int mcb_stem_unpack_wgrad(const float* dw_packed, float* dw, void* stream); /* dw += */
 
+/* VGG input conv, encoder.0 = Conv2d(3, 64, 3, padding 1) + ReLU at full resolution (src/unet_models.py:68,90 and
+ * :252,256): im2col into a [n*h*w][32] bf16 matrix (k = (ky*3+kx)*3 + c for k < 27, zero for k = 27..31; pixels outside
+ * the image read zero) fed to mcb_conv_fwd / mcb_conv_wgrad as a 1x1 conv.  The master weight is fp32 [9][64][3];
+ * pack/unpack convert to/from the GEMM operand [64][32].  No data gradient: the input is the image. */
+int mcb_vgg_input_im2col(const float* x_nchw, void* col, int n, int h, int w, void* stream);
+int mcb_vgg_input_pack_weight(const float* w, void* w_packed, void* stream);
+int mcb_vgg_input_unpack_wgrad(const float* dw_packed, float* dw, void* stream); /* dw += */
+
 /* nn.BatchNorm2d (eps 1e-5, momentum 0.1; torchvision resnet blocks).  Training: `stats` is what mcb_conv_fwd
  * accumulated; finalize turns it into the per-channel affine + saved mean / invstd and updates the running stats. */
 int mcb_bn_finalize(const float* stats, long count, const float* gamma, const float* beta, float* running_mean,
@@ -199,6 +207,12 @@ int mcb_channel_sum(const void* x, float* out, long pixels, int c, void* stream)
 int mcb_maxpool2_fwd(const void* x, void* y, int n, int h, int w, int c, void* stream);
 int mcb_maxpool2_bwd(const void* x, const void* dy, void* dx, int accumulate, int n, int h, int w, int c,
                      void* stream);
+/* VGG encoders (src/unet_models.py:90-105, :296-310): y = relu(conv + b) [n, h, w, c] feeds both pool(y) and a decoder
+ * concat.  On entry g holds the concat's data gradient; in place g = bf16(g + routed dpool) * (y > 0) (dpool to the
+ * first maximum of each window), and db += the per-channel sums of the stored bf16 g (the conv's bias gradient, summed
+ * like mcb_conv_dgrad's dx_channel_sum; fixed-order, run-to-run identical).  g must not alias y or dpool. */
+int mcb_maxpool2_bwd_skip_relu(const void* y, const void* dpool, void* g, float* db, int n, int h, int w, int c,
+                               void* stream);
 
 /* final = Conv2d(32, 2, 1) (src/unet_models.py:383,403): NHWC bf16 -> NCHW fp32 logits; backward also applies
  * dec0's ReLU mask (x is dec0's output) */

@@ -86,6 +86,10 @@ _SIGS = {
     "mcb_stem_im2col": [vp, vp, ci, ci, ci, vp],
     "mcb_stem_pack_weight": [vp, vp, vp],
     "mcb_stem_unpack_wgrad": [vp, vp, vp],
+    "mcb_vgg_input_im2col": [vp, vp, ci, ci, ci, vp],
+    "mcb_vgg_input_pack_weight": [vp, vp, vp],
+    "mcb_vgg_input_unpack_wgrad": [vp, vp, vp],
+    "mcb_maxpool2_bwd_skip_relu": [vp, vp, vp, vp, ci, ci, ci, ci, vp],
     "mcb_bn_finalize": [vp, cl, vp, vp, vp, vp, cf, cf, vp, vp, vp, vp, ci, vp],
     "mcb_bn_eval_params": [vp, vp, vp, vp, cf, vp, vp, ci, vp],
     "mcb_bn_apply": [vp, vp, vp, vp, vp, vp, ci, vp, cl, ci, vp],

@@ -130,6 +130,73 @@ __global__ void stem_unpack_wgrad_kernel(const float* __restrict__ dwp, float* _
   dw[i] += dwp[(long)co * 192 + tap * 3 + c];
 }
 
+// ------------------------------------------------------------------------------------------ VGG input conv im2col
+// The VGG encoders' first conv, Conv2d(3, 64, 3, padding 1) at full resolution: a 3-channel NHWC row (6 bytes) is too
+// narrow for TMA, so the conv runs as a 1x1 GEMM over a [N*H*W] x 32 bf16 matrix with k = (ky*3 + kx)*3 + c for
+// k < 27 and zero for k = 27..31; pixels outside the image read zero (padding 1).
+constexpr int VIN_SW = 64;                  // output pixels per strip (of one row)
+constexpr int VIN_COLS = VIN_SW + 2;        // input columns a strip touches
+// One CTA = one strip: the 3 x 3 x 66 input patch is staged in shared memory with coalesced loads, then each thread
+// assembles 16-byte groups of 8 k-values (4 per pixel); consecutive threads write consecutive 16-byte groups.
+__global__ void __launch_bounds__(256) vgg_input_im2col_kernel(const float* __restrict__ x, bf16* __restrict__ col,
+                                                               int N, int H, int W) {
+  mcb::pdl_prologue();
+  __shared__ float s[3][3][VIN_COLS + 1];
+  const int strips = (W + VIN_SW - 1) / VIN_SW;
+  const int strip = blockIdx.x % strips;
+  const int oy = (blockIdx.x / strips) % H;
+  const int n = blockIdx.x / (strips * H);
+  const int ox0 = strip * VIN_SW;
+  for (int e = threadIdx.x; e < 3 * 3 * VIN_COLS; e += blockDim.x) {
+    const int cc = e % VIN_COLS;
+    const int r = (e / VIN_COLS) % 3;
+    const int c = e / (VIN_COLS * 3);
+    const int iy = oy - 1 + r, ix = ox0 - 1 + cc;
+    float v = 0.f;
+    if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = __ldg(x + (((long)n * 3 + c) * H + iy) * W + ix);
+    s[c][r][cc] = v;
+  }
+  __syncthreads();
+  const int npx = min(VIN_SW, W - ox0);
+  const long base = (((long)n * H + oy) * W + ox0) * 4;
+  for (int e = threadIdx.x; e < npx * 4; e += blockDim.x) {
+    const int g = e % 4;
+    const int pl = e / 4;
+    float f[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int k = g * 8 + j;
+      float v = 0.f;
+      if (k < 27) {
+        const int c = k % 3, kx = (k / 3) % 3, ky = k / 9;
+        v = s[c][ky][pl + kx];
+      }
+      f[j] = v;
+    }
+    reinterpret_cast<uint4*>(col)[base + e] = pack8(f);
+  }
+}
+// master weight fp32 [3][3][64][3] (tap-major like every conv) <-> GEMM operand bf16 [64][32]
+__global__ void vgg_input_pack_weight_kernel(const float* __restrict__ w, bf16* __restrict__ wp) {
+  mcb::pdl_prologue();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 64 * 32) return;
+  const int k = i % 32, co = i / 32;
+  float v = 0.f;
+  if (k < 27) {
+    const int c = k % 3, tap = k / 3;
+    v = w[((long)tap * 64 + co) * 3 + c];
+  }
+  wp[i] = __float2bfloat16(v);
+}
+__global__ void vgg_input_unpack_wgrad_kernel(const float* __restrict__ dwp, float* __restrict__ dw) {
+  mcb::pdl_prologue();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 9 * 64 * 3) return;
+  const int c = i % 3, co = (i / 3) % 64, tap = i / 192;
+  dw[i] += dwp[(long)co * 32 + tap * 3 + c];
+}
+
 // ------------------------------------------------------------------------------------------ BatchNorm
 // stats = [sum(C), sumsq(C)] of the bf16 conv output -> per-channel affine (scale, shift) + saved mean / invstd,
 // running statistics updated like nn.BatchNorm2d (momentum, unbiased variance)
@@ -540,6 +607,71 @@ __global__ void maxpool2_bwd_kernel(const uint4* __restrict__ x, const uint4* __
     }
   }
 }
+// Backward of the 2x2 max-pool over an encoder output y = relu(conv + b) that also feeds a decoder concat (VGG
+// encoders).  g holds the concat's data gradient on entry (the decoder runs first in the backward); in place,
+//   g = bf16(g + routed dpool) * (y > 0),
+// the pooled gradient going to the first maximum in window order like maxpool2_bwd_kernel.  The per-channel sums of the
+// STORED bf16 g (the conv's bias gradient; the same values the dgrad epilogue's dx_channel_sum adds) go into this
+// block's row of g_channel_red.  Block = lanes x C8 threads with a fixed channel group per thread, like
+// channel_reduce_kernel; a pooled pixel is one 2x2 window.
+__global__ void maxpool2_bwd_skip_relu_kernel(const uint4* __restrict__ y, const uint4* __restrict__ dpool,
+                                              uint4* __restrict__ g, long pooled, int H, int W, int C8) {
+  mcb::pdl_prologue();
+  extern __shared__ float red[];  // [blockDim.x][8]
+  const int cg = threadIdx.x % C8;
+  const int lane_p = threadIdx.x / C8;
+  const int lanes = blockDim.x / C8;
+  const int Ho = H / 2, Wo = W / 2;
+  float s[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) s[j] = 0.f;
+  for (long p = (long)blockIdx.x * lanes + lane_p; p < pooled; p += (long)gridDim.x * lanes) {
+    const int ox = p % Wo, oy = (p / Wo) % Ho;
+    const long n = p / ((long)Wo * Ho);
+    const long base = ((n * H + 2 * oy) * W + 2 * ox) * C8 + cg;
+    const long idx[4] = {base, base + C8, base + (long)W * C8, base + (long)W * C8 + C8};
+    float v[4][8], o[4][8], d[8];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      unpack8(__ldg(y + idx[k]), v[k]);
+      unpack8(g[idx[k]], o[k]);
+    }
+    unpack8(__ldg(dpool + p * C8 + cg), d);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      int best = 0;
+      float m = v[0][j];
+#pragma unroll
+      for (int k = 1; k < 4; ++k)
+        if (v[k][j] > m) { m = v[k][j]; best = k; }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float t = (k == best) ? o[k][j] + d[j] : o[k][j];
+        o[k][j] = v[k][j] > 0.f ? t : 0.f;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint4 pk = pack8(o[k]);
+      g[idx[k]] = pk;
+      float r[8];
+      unpack8(pk, r);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s[j] += r[j];
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) red[threadIdx.x * 8 + j] = s[j];
+  __syncthreads();
+  // threads 0 .. C8*8-1 each own one channel and sum over the pixel lanes, in lane order, into this block's row
+  float* row = g_channel_red + (size_t)blockIdx.x * (C8 * 8);
+  for (int ch = threadIdx.x; ch < C8 * 8; ch += blockDim.x) {
+    const int gr = ch / 8, j = ch % 8;
+    float t = 0.f;
+    for (int l = 0; l < lanes; ++l) t += red[(l * C8 + gr) * 8 + j];
+    row[ch] = t;
+  }
+}
 
 // ------------------------------------------------------------------------------------------ final 1x1 classifier
 // logits[n][k][h][w] (fp32 NCHW, the reference's output layout) = W[k][:] . x[n][h][w][:] + b[k];  C = 32, K = 2
@@ -699,6 +831,27 @@ extern "C" int mcb_stem_pack_weight(const float* w, void* wp, void* stream) {
 extern "C" int mcb_stem_unpack_wgrad(const float* dwp, float* dw, void* stream) {
   MCB_REQUIRE(dwp && dw, "null pointer");
   launch_pdl(stem_unpack_wgrad_kernel, (49 * 64 * 3 + 255) / 256, 256, 0, ST, dwp, dw);
+  MCB_LAUNCH_CHECK();
+  return MCB_OK;
+}
+extern "C" int mcb_vgg_input_im2col(const float* x, void* col, int n, int h, int w, void* stream) {
+  MCB_REQUIRE(x && col, "null pointer");
+  MCB_REQUIRE(n > 0 && h > 0 && w > 0, "vgg_input_im2col: size %dx%dx%d", n, h, w);
+  const long ctas = (long)n * h * ((w + VIN_SW - 1) / VIN_SW);  // one per strip of a row
+  MCB_REQUIRE(ctas < (1L << 31), "vgg_input_im2col: too many strips");
+  launch_pdl(vgg_input_im2col_kernel, dim3((unsigned)ctas), 256, 0, ST, x, (bf16*)col, n, h, w);
+  MCB_LAUNCH_CHECK();
+  return MCB_OK;
+}
+extern "C" int mcb_vgg_input_pack_weight(const float* w, void* wp, void* stream) {
+  MCB_REQUIRE(w && wp, "null pointer");
+  launch_pdl(vgg_input_pack_weight_kernel, (64 * 32 + 255) / 256, 256, 0, ST, w, (bf16*)wp);
+  MCB_LAUNCH_CHECK();
+  return MCB_OK;
+}
+extern "C" int mcb_vgg_input_unpack_wgrad(const float* dwp, float* dw, void* stream) {
+  MCB_REQUIRE(dwp && dw, "null pointer");
+  launch_pdl(vgg_input_unpack_wgrad_kernel, (9 * 64 * 3 + 255) / 256, 256, 0, ST, dwp, dw);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -862,6 +1015,26 @@ extern "C" int mcb_maxpool2_bwd(const void* x, const void* dy, void* dx, int acc
   const long total = (long)n * (h / 2) * (w / 2) * (c / 8);
   launch_pdl(maxpool2_bwd_kernel, grid_for(total, 256), 256, 0, ST, (const uint4*)x, (const uint4*)dy, (uint4*)dx, accumulate,
                                                             n, h, w, c / 8);
+  MCB_LAUNCH_CHECK();
+  return MCB_OK;
+}
+extern "C" int mcb_maxpool2_bwd_skip_relu(const void* y, const void* dpool, void* g, float* db, int n, int h, int w,
+                                          int c, void* stream) {
+  MCB_REQUIRE(y && dpool && g && db, "maxpool2_bwd_skip_relu: null pointer");
+  // y and dpool are read through the read-only cache while g is rewritten in place
+  MCB_REQUIRE(g != y && g != dpool, "maxpool2_bwd_skip_relu: g aliases y or dpool");
+  MCB_REQUIRE(n > 0 && h > 0 && w > 0 && h % 2 == 0 && w % 2 == 0, "maxpool2_bwd_skip_relu: size %dx%dx%d", n, h, w);
+  int threads, c8;
+  if (int r = reduce_cfg(c, &threads, &c8)) return r;
+  const int lanes = threads / c8;
+  const long pooled = (long)n * (h / 2) * (w / 2);
+  const int grid = (int)std::max(1L, std::min((pooled + lanes * 4 - 1) / (lanes * 4), (long)num_sms() * 4));
+  MCB_REQUIRE((long)grid * c <= kChannelRedCap, "maxpool2_bwd_skip_relu: %d blocks x %d channels exceed the workspace",
+              grid, c);
+  launch_pdl(maxpool2_bwd_skip_relu_kernel, grid, threads, (size_t)threads * 8 * sizeof(float), ST, (const uint4*)y,
+             (const uint4*)dpool, (uint4*)g, pooled, h, w, c8);
+  launch_pdl(channel_red_finish_kernel, det_finish_grid(c), kDetFinishThreads, 0, ST, 0L, grid, (long)c, (long)c,
+             (long)c, db, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }

@@ -1,4 +1,5 @@
-"""Static launch plans for UNetResNet: every kernel launch of one forward (and its backward) over preallocated
+"""Static launch plans for the U-Nets of unet_models (UNetResNet / AlbuNet, and the BatchNorm-free VGG plan of UNet11 /
+UNetVGG16, see Plan._build_vgg): every kernel launch of one forward (and its backward) over preallocated
 NHWC bf16 buffers, replayable as CUDA graphs.
 
 Data flow per conv+BN unit in training:  z = conv(a_prev) [+ per-channel sum / sumsq in the GEMM epilogue]
@@ -313,6 +314,8 @@ class Plan:
 
     # ------------------------------------------------------------------------------------------ network
     def _build(self):
+        if self.net.plan_kind == "vgg":
+            return self._build_vgg()
         net, n, h, w = self.net, self.n, self.h, self.w
         F = self.fwd_ops
         enc = net.encoder
@@ -416,6 +419,160 @@ class Plan:
                 self.dgrad_into(B, g_d0, conv0, d1, relu_mask=d1)
             self._bwd_builders.append(("decoder", build_head))
 
+    # ------------------------------------------------------------------------------------------ VGG encoders
+    def _build_vgg(self):
+        """UNet11 / UNetVGG16 (src/unet_models.py:89-106, :296-312): five stages of conv + bias + ReLU units, each stage
+        output pooled and concatenated into the decoder; no BatchNorm.  Backward: the decoder runs first and stores the
+        skip segment's data gradient of every stage output; the pool backward adds the pooled path, applies the ReLU
+        mask and sums the bias gradient (maxpool2_bwd_skip_relu).  Units inside a stage have one consumer: their mask
+        and bias gradient ride in the next conv's dgrad epilogue."""
+        net, n, h, w = self.net, self.n, self.h, self.w
+        F = self.fwd_ops
+        enc = net.encoder
+        train = self.training
+        skips = []
+        x = None
+        for si, stage in enumerate(net._stages):
+            self._cur_tag = "conv%d" % (si + 1)
+            for ci, idx in enumerate(stage):
+                xin = x
+                x = self._vgg_input_unit(enc[idx]) if xin is None else self._vgg_unit(xin, enc[idx])
+                self.units.append(("conv", "encoder.%d" % idx, () if xin is None else (xin,), x))
+            skips.append(x)
+            x = self._vgg_pool(x)
+        c1, c2, c3, c4, c5 = skips
+        # ---- decoder (src/unet_models.py:99-105, :303-310)
+        center = self._decoder(x, None, net.center, pool_input=True)
+        d5 = self._decoder(center, c5, net.dec5)
+        d4 = self._decoder(d5, c4, net.dec4)
+        d3 = self._decoder(d4, c3, net.dec3)
+        d2 = self._decoder(d3, c2, net.dec2)
+        self.units += [("decoder", "center", (x,), center), ("decoder", "dec5", (center, c5), d5),
+                       ("decoder", "dec4", (d5, c4), d4), ("decoder", "dec3", (d4, c3), d3),
+                       ("decoder", "dec2", (d3, c2), d2)]
+        # dec1 = ConvRelu(32 + 64, 32) over cat[dec2, conv1], then the 1x1 classifier
+        conv = net.dec1.conv
+        w16 = net._packed(conv.weight, net._w16)
+        b = net._vec(conv.bias, net._p32)
+        d1 = self.act(n, h, w, conv.out_channels)
+        ca, cb = d2.shape[3], c1.shape[3]
+        f1 = 2.0 * d1.numel() * (ca + cb) * 9
+        F.add("conv_fwd", lambda: ops.conv_fwd(d2, w16, 3, 1, bias=b, relu=True, x2=c1, out=d1), f1, _nb(d2, c1, w16, d1),
+              "dec %d->%d k3 @%dx%dx%d" % (ca + cb, conv.out_channels, n, h, w))
+        fw, fb = net._vec(net.final.weight, net._p32), net._vec(net.final.bias, net._p32)
+        F.add("final_conv", lambda: ops.final_conv_fwd(d1, fw, fb, self.logits), 2.0 * self.logits.numel() * 32,
+              _nb(d1, self.logits))
+        self.units.append(("decoder", "dec1", (d2, c1), d1))
+        self.named = dict(conv1=c1, conv2=c2, conv3=c3, conv4=c4, conv5=c5, center=center, dec5=d5, dec4=d4, dec3=d3,
+                          dec2=d2, dec1=d1)
+        if train:
+            def build_head(B):
+                g_d1 = self.gbuf(d1)
+                gfw, gfb = net._vec(net.final.weight, net._g32), net._vec(net.final.bias, net._g32)
+                # the classifier's backward also applies dec1's ReLU mask
+                B.add("final_conv", lambda: ops.final_conv_bwd(d1, fw, self.dlogits, g_d1, gfw, gfb),
+                      4.0 * self.logits.numel() * 32, _nb(d1, self.dlogits, g_d1))
+                gb = net._vec(conv.bias, net._g32)
+                gw = net._packed(conv.weight, net._g32)
+                B.add("channel_sum", lambda: ops.channel_sum(g_d1, gb), 0, _nb(g_d1))
+                B.add("conv_wgrad", lambda: ops.conv_wgrad(g_d1, d2, gw, 3, 1, ci_off=0), 2.0 * d1.numel() * ca * 9,
+                      _nb(g_d1, d2), "dec %d->%d k3 @%dx%dx%d" % (ca, conv.out_channels, n, h, w))
+                B.add("conv_wgrad", lambda: ops.conv_wgrad(g_d1, c1, gw, 3, 1, ci_off=ca), 2.0 * d1.numel() * cb * 9,
+                      _nb(g_d1, c1), "dec-skip %d->%d k3 @%dx%dx%d" % (cb, conv.out_channels, n, h, w))
+                self.dgrad_into(B, g_d1, conv, d2, relu_mask=d2, ci_off=0)
+                self.dgrad_into(B, g_d1, conv, c1, relu_mask=None, ci_off=ca)
+            self._bwd_builders.append(("decoder", build_head))
+
+    def _vgg_input_unit(self, conv):
+        """encoder.0 = Conv2d(3, 64, 3, padding 1) + ReLU on the full-resolution image: im2col (27 of 32 columns) + a
+        1x1 GEMM with bias and ReLU; the weight gradient is the 1x1 wgrad, unpacked into the master slot"""
+        net, n, h, w = self.net, self.n, self.h, self.w
+        F = self.fwd_ops
+        cout = conv.out_channels
+        col = self.act(n, h, w, 32)
+        w16 = torch.zeros((1, cout, 32), dtype=BF16, device=self.dev)
+        self._keep.append(w16)
+        master = net._vec(conv.weight, net._p32)
+        b = net._vec(conv.bias, net._p32)
+        y = self.act(n, h, w, cout)
+        fl = 2.0 * n * h * w * cout * 27     # the real 27-wide reduction, as the reference counts it
+        desc = "3->%d k3 (im2col) @%dx%dx%d" % (cout, n, h, w)
+        F.add("im2col", lambda: ops.vgg_input_im2col(self.x_in, col), 0, _nb(self.x_in, col))
+        F.add("misc", lambda: ops.vgg_input_pack_weight(master, w16))
+        F.add("conv_fwd", lambda: ops.conv_fwd(col, w16, 1, 1, bias=b, relu=True, out=y), fl, _nb(col, y), desc)
+        if self.training:
+            self.bias_sum[id(y)] = net._vec(conv.bias, net._g32)
+
+            def build_input(B):
+                g = self.gbuf(y)       # complete, masked, bias gradient summed (by its consumer)
+                gw = torch.zeros((1, cout, 32), dtype=F32, device=self.dev)
+                self._keep.append(gw)
+                g_slot = net._vec(conv.weight, net._g32)
+                B.add("misc", lambda: L.zero(gw))
+                # no desc: stays on the main stream, in order with the zeroing and the unpack (like the ResNet stem)
+                B.add("conv_wgrad", lambda: ops.conv_wgrad(g, col, gw, 1, 1), fl, _nb(g, col))
+                B.add("misc", lambda: ops.vgg_input_unpack_wgrad(gw, g_slot))
+            self._bwd_builders.append((self._cur_tag, build_input))
+        return y
+
+    def _vgg_unit(self, x, conv):
+        """y = relu(conv3x3(x) + b).  x is a pool output (gradient stored plainly) or the previous unit's output (its
+        ReLU mask and bias gradient fused into this unit's dgrad epilogue)"""
+        net = self.net
+        F = self.fwd_ops
+        n, h, w, cin = x.shape
+        cout = conv.out_channels
+        w16 = net._packed(conv.weight, net._w16)
+        b = net._vec(conv.bias, net._p32)
+        y = self.act(n, h, w, cout)
+        fl = 2.0 * y.numel() * cin * 9
+        desc = "%d->%d k3 s1 @%dx%dx%d" % (cin, cout, n, h, w)
+        F.add("conv_fwd", lambda: ops.conv_fwd(x, w16, 3, 1, bias=b, relu=True, out=y), fl, _nb(x, w16, y), desc)
+        if self.training:
+            self.bias_sum[id(y)] = net._vec(conv.bias, net._g32)
+            x_is_unit = id(x) in self.bias_sum
+
+            def build_unit(B):
+                g = self.gbuf(y)
+                gw = net._packed(conv.weight, net._g32)
+                B.add("conv_wgrad", lambda: ops.conv_wgrad(g, x, gw, 3, 1), fl, _nb(g, x, gw), desc)
+                self.dgrad_into(B, g, conv, x, relu_mask=x if x_is_unit else None)
+            self._bwd_builders.append((self._cur_tag, build_unit))
+        return y
+
+    def _vgg_pool(self, y):
+        """2x2 max-pool of a stage output y; its backward completes grad(y) (see _build_vgg)"""
+        F = self.fwd_ops
+        n, h, w, c = y.shape
+        p = self.act(n, h // 2, w // 2, c)
+        F.add("maxpool", lambda: ops.maxpool2_fwd(y, p), 0, _nb(y, p))
+        if self.training:
+            gb = self.bias_sum[id(y)]
+
+            def build_pool(B):
+                if id(y) not in self.written:
+                    raise RuntimeError("plan error: the skip gradient of a VGG stage output must be stored first")
+                d_p, g = self.gbuf(p), self.gbuf(y)
+                self.bias_fused.add(id(y))
+                B.add("maxpool", lambda: ops.maxpool2_bwd_skip_relu(y, d_p, g, gb), 0, _nb(y, d_p, g, g))
+            self._bwd_builders.append((self._cur_tag, build_pool))
+        return p
+
+    def _vgg_segments(self):
+        """[decoder | conv5 stage | conv4 stage | rest], like bwd_segments for the ResNets"""
+        net = self.net
+        tags = self.bwd_tags
+        n = len(tags)
+        i_dec = max(i for i, t in enumerate(tags) if t == "decoder") + 1
+        i_c5 = max(i for i, t in enumerate(tags) if t == "conv5") + 1
+        i_c4 = max(i for i, t in enumerate(tags) if t == "conv4") + 1
+        off = {name: net._slots[id(p)].off for name, p, _ in net._arena_params()}
+        total = net._p32.numel()
+        o_dec = off["center.block.0.conv.weight"]
+        o_c5 = off["encoder.%d.weight" % net._stages[4][0]]
+        o_c4 = off["encoder.%d.weight" % net._stages[3][0]]
+        return [(0, i_dec, o_dec, total), (i_dec, i_c5, o_c5, o_dec), (i_c5, i_c4, o_c4, o_c5), (i_c4, n, 0, o_c4)]
+
     def _res_block(self, x, blk):
         """torchvision BasicBlock / Bottleneck forward + backward plan"""
         train = self.training
@@ -475,12 +632,14 @@ class Plan:
         return out
 
     def _decoder(self, x1, skip, block, pool_input=False):
-        """DecoderBlockV2: relu(conv3x3(cat[x1, skip]) + b) -> relu(convT4x4s2(.) + b)   (src/unet_models.py:136-141)"""
+        """DecoderBlockV2 / DecoderBlock: relu(conv3x3(cat[x1, skip]) + b) -> relu(convT(.) + b) with the 4x4 or the 3x3
+        (output_padding 1) stride-2 transposed conv   (src/unet_models.py:42-53,136-141)"""
         net = self.net
         F = self.fwd_ops
         conv, deconv = block.block[0].conv, block.block[1]
         n, h, w, c1 = x1.shape
         cmid, cout = conv.out_channels, deconv.out_channels
+        kt = deconv.kernel_size[0]
         w16 = net._packed(conv.weight, net._w16)
         b1 = net._vec(conv.bias, net._p32)
         wt16 = net._packed(deconv.weight, net._w16)
@@ -491,7 +650,7 @@ class Plan:
         if self.training:
             self.bias_sum[id(out)] = net._vec(deconv.bias, net._g32)
         fc = 2.0 * mid.numel() * ctot * 9
-        ft = 2.0 * mid.numel() * cout * 16
+        ft = 2.0 * mid.numel() * cout * kt * kt
         F.add("conv_fwd", lambda: ops.conv_fwd(x1, w16, 3, 1, bias=b1, relu=True, x2=skip, out=mid), fc,
               _nb(x1, skip, w16, mid), "dec %d->%d k3 @%dx%dx%d" % (ctot, cmid, n, h, w))
         F.add("convt_fwd", lambda: ops.convt_fwd(mid, wt16, bias=b2, relu=True, out=out), ft, _nb(mid, wt16, out),
@@ -533,13 +692,14 @@ class Plan:
         return self._bn_tab
 
     def _run_fwd(self):
-        if not self.training:
+        if not self.training and self._bns:     # (the VGG nets have no BatchNorm)
             tab = self._bn_table()
             L.fcall("mcb_bn_eval_params_batched", tab.data_ptr(), len(self._bns), self._bn_maxc, BN_EPS)
         if self.training:
             if self.sync_nvlink:
                 L.fcall("mcb_sync_step_bump", self._sync_step.data_ptr())
-            L.zero(self._stats_arena)
+            if self._stats_arena.numel():
+                L.zero(self._stats_arena)
         for op in self.fwd_ops:
             op()
 
@@ -621,6 +781,8 @@ class Plan:
         net = self.net
         tags = self.bwd_tags
         n = len(tags)
+        if net.plan_kind == "vgg":
+            return self._vgg_segments()
         i_dec = max(i for i, t in enumerate(tags) if t == "decoder") + 1
         i_l4 = max(i for i, t in enumerate(tags) if t == "layer4") + 1
         i_l3 = max(i for i, t in enumerate(tags) if t == "layer3") + 1

@@ -333,8 +333,9 @@ class BasePyTorchUNet(Model):
     def set_model(self):
         encoder = self.architecture_config['model_params']['encoder']
         if encoder not in PRETRAINED_NETWORKS:
-            raise NotImplementedError("the H100 path implements the AlbuNet and ResNet34/101/152 encoders; the VGG11 "
-                                      "and VGG16 U-Nets are not built (got %r)" % (encoder,))
+            raise NotImplementedError("the registry holds the AlbuNet and ResNet34/101/152 encoders; the VGG11 and VGG16 "
+                                      "U-Nets are not registered (build mcb200.unet_models.UNet11 / UNetVGG16 and "
+                                      "drive them with FusedTrainStep) (got %r)" % (encoder,))
         config = PRETRAINED_NETWORKS[encoder]
         self.model = config['model'](**config['model_config'])
         self._initialize_model_weights = lambda: None

@@ -201,6 +201,31 @@ def stem_unpack_wgrad(dwp, dw):
     L.fcall("mcb_stem_unpack_wgrad", _chk(dwp, F32).data_ptr(), _chk(dw, F32).data_ptr())
 
 
+def vgg_input_im2col(x, out=None):
+    """fp32 NCHW image -> bf16 (N, H, W, 32) im2col of the 3x3 pad-1 VGG input conv (k = (ky*3 + kx)*3 + c)"""
+    _chk(x, F32)
+    n, c, h, w = x.shape
+    assert c == 3
+    if out is None:
+        out = torch.empty((n, h, w, 32), dtype=torch.bfloat16, device=x.device)
+    assert out.shape == (n, h, w, 32), out.shape
+    L.fcall("mcb_vgg_input_im2col", x.data_ptr(), _chk(out).data_ptr(), n, h, w)
+    return out
+
+
+def vgg_input_pack_weight(w9x64x3, out):
+    """fp32 [9][64][3] master slot -> bf16 (1, 64, 32) GEMM operand"""
+    assert w9x64x3.numel() == 9 * 64 * 3 and out.shape == (1, 64, 32), (w9x64x3.shape, out.shape)
+    L.fcall("mcb_vgg_input_pack_weight", _chk(w9x64x3, F32).data_ptr(), _chk(out).data_ptr())
+    return out
+
+
+def vgg_input_unpack_wgrad(dwp, dw):
+    """dw ([9][64][3] fp32 slot) += the (1, 64, 32) fp32 weight gradient of the im2col GEMM"""
+    assert dwp.shape == (1, 64, 32) and dw.numel() == 9 * 64 * 3, (dwp.shape, dw.shape)
+    L.fcall("mcb_vgg_input_unpack_wgrad", _chk(dwp, F32).data_ptr(), _chk(dw, F32).data_ptr())
+
+
 def bn_finalize(stats, count, gamma, beta, rm, rv, scale, shift, mean, invstd, momentum=0.1, eps=1e-5):
     c = gamma.numel()
     L.fcall("mcb_bn_finalize", stats.data_ptr(), int(count), gamma.data_ptr(), beta.data_ptr(), L.dp(rm), L.dp(rv),
@@ -271,6 +296,17 @@ def maxpool2_bwd(x, dy, dx, accumulate=False):
     n, h, w, c = x.shape
     L.fcall("mcb_maxpool2_bwd", _chk(x).data_ptr(), _chk(dy).data_ptr(), _chk(dx).data_ptr(), int(accumulate), n, h, w, c)
     return dx
+
+
+def maxpool2_bwd_skip_relu(y, dpool, g, db):
+    """y = relu(conv + b) feeding pool(y) and a decoder concat; g (holding the concat's gradient) becomes
+    (g + routed dpool) * (y > 0) in place, db += its per-channel sums"""
+    n, h, w, c = y.shape
+    assert g.shape == y.shape and dpool.shape == (n, h // 2, w // 2, c) and db.numel() == c
+    assert g.data_ptr() not in (y.data_ptr(), dpool.data_ptr()), "g is rewritten in place: it must not alias y or dpool"
+    L.fcall("mcb_maxpool2_bwd_skip_relu", _chk(y).data_ptr(), _chk(dpool).data_ptr(), _chk(g).data_ptr(),
+            _chk(db, F32).data_ptr(), n, h, w, c)
+    return g
 
 
 def final_conv_fwd(x, w, b, logits):

@@ -1,4 +1,4 @@
-"""Mirror of the reference's src/unet_models.py for the ResNet-encoder U-Nets (UNetResNet and AlbuNet), executed by
+"""Mirror of the reference's src/unet_models.py (UNetResNet, AlbuNet, UNet11 and UNetVGG16), executed by
 libmcb200.so.
 
 `UNetResNet` keeps the reference's constructor, attribute tree and state_dict keys
@@ -49,49 +49,31 @@ class DecoderBlockV2(nn.Module):
                                    nn.ReLU(inplace=True))
 
 
+class DecoderBlock(nn.Module):
+    """parameter container for ConvRelu -> ConvTranspose2d(3, 2, 1, output_padding=1) -> ReLU (reference
+    src/unet_models.py:42-53, UNet11's decoder)"""
+
+    def __init__(self, in_channels, middle_channels, out_channels):
+        super().__init__()
+        self.block = nn.Sequential(ConvRelu(in_channels, middle_channels),
+                                   nn.ConvTranspose2d(middle_channels, out_channels, kernel_size=3, stride=2, padding=1,
+                                                      output_padding=1),
+                                   nn.ReLU(inplace=True))
+
+
 class _Slot:
     __slots__ = ("off", "numel", "shape", "kind")
 
 
-class UNetResNet(nn.Module):
-    """PyTorch-facing U-Net with a ResNet-34/101/152 encoder; same signature as the reference class."""
+class _ArenaUNet(nn.Module):
+    """What every U-Net of the H100 path shares: the fp32 parameter arena whose views the nn.Parameters are, the
+    gradient and bf16 operand arenas, device moves, state_dict, the cached launch plans and forward.  A subclass builds
+    the reference's module tree, then calls _init_arenas(); engine.Plan reads `plan_kind` to pick the launch plan."""
+    plan_kind = "resnet"
+    _arch = "UNet"           # name in error messages
+    _size_multiple = 64      # H and W must be multiples of this (the reference's torch.cat fails otherwise)
 
-    def __init__(self, encoder_depth, num_classes, num_filters=32, dropout_2d=0.2, pretrained=False, is_deconv=False):
-        super().__init__()
-        self.num_classes = num_classes
-        self.dropout_2d = dropout_2d
-        self.encoder_depth = encoder_depth
-        self.num_filters = num_filters
-        if pretrained:
-            raise NotImplementedError("pretrained=True downloads ImageNet weights; load a state_dict instead")
-        if encoder_depth == 34:
-            self.encoder = torchvision.models.resnet34(weights=None)
-            bottom = 512
-        elif encoder_depth == 101:
-            self.encoder = torchvision.models.resnet101(weights=None)
-            bottom = 2048
-        elif encoder_depth == 152:
-            self.encoder = torchvision.models.resnet152(weights=None)
-            bottom = 2048
-        else:
-            raise NotImplementedError('only 34, 101, 152 version of Resnet are implemented')
-        self.bottom_channel_nr = bottom
-        self.pool = nn.MaxPool2d(2, 2)
-        self.relu = nn.ReLU(inplace=True)
-        self.conv1 = nn.Sequential(self.encoder.conv1, self.encoder.bn1, self.encoder.relu, self.pool)
-        self.conv2 = self.encoder.layer1
-        self.conv3 = self.encoder.layer2
-        self.conv4 = self.encoder.layer3
-        self.conv5 = self.encoder.layer4
-        nf = num_filters
-        self.center = DecoderBlockV2(bottom, nf * 8 * 2, nf * 8, is_deconv)
-        self.dec5 = DecoderBlockV2(bottom + nf * 8, nf * 8 * 2, nf * 8, is_deconv)
-        self.dec4 = DecoderBlockV2(bottom // 2 + nf * 8, nf * 8 * 2, nf * 8, is_deconv)
-        self.dec3 = DecoderBlockV2(bottom // 4 + nf * 8, nf * 4 * 2, nf * 2, is_deconv)
-        self.dec2 = DecoderBlockV2(bottom // 8 + nf * 2, nf * 2 * 2, nf * 2 * 2, is_deconv)
-        self.dec1 = DecoderBlockV2(nf * 2 * 2, nf * 2 * 2, nf, is_deconv)
-        self.dec0 = ConvRelu(nf, nf)
-        self.final = nn.Conv2d(nf, num_classes, kernel_size=1)
+    def _init_arenas(self):
         self._slots = {}
         self._plans = {}
         self._p32 = self._g32 = self._w16 = None
@@ -199,15 +181,16 @@ class UNetResNet(nn.Module):
     # ------------------------------------------------------------------------------------------------ forward
     def _check_input(self, x):
         if not isinstance(x, torch.Tensor) or not x.is_cuda:
-            raise RuntimeError("UNetResNet (H100 path) needs a CUDA tensor; there is no CPU fallback")
+            raise RuntimeError("%s (H100 path) needs a CUDA tensor; there is no CPU fallback" % self._arch)
         if self._p32 is None or not self._p32.is_cuda:
-            raise RuntimeError("UNetResNet (H100 path): call .cuda() on the model first; there is no CPU fallback")
+            raise RuntimeError("%s (H100 path): call .cuda() on the model first; there is no CPU fallback" % self._arch)
         if x.dim() != 4 or x.shape[1] != 3:
             raise ValueError("expected input (N, 3, H, W), got %s" % (tuple(x.shape),))
-        if x.shape[2] % 64 != 0 or x.shape[3] % 64 != 0:
+        m = self._size_multiple
+        if x.shape[2] % m != 0 or x.shape[3] % m != 0:
             # the reference fails in torch.cat for such sizes (SURVEY.md 0.3)
-            raise RuntimeError("UNetResNet needs H and W divisible by 64, got %dx%d" % (x.shape[2], x.shape[3]))
-        if self.dropout_2d != 0:
+            raise RuntimeError("%s needs H and W divisible by %d, got %dx%d" % (self._arch, m, x.shape[2], x.shape[3]))
+        if getattr(self, "dropout_2d", 0.0) != 0:
             raise NotImplementedError("dropout_2d must be 0.0 (the configured value, src/models.py:32-46)")
 
     def plan(self, n, h, w, training):
@@ -233,6 +216,49 @@ class UNetResNet(nn.Module):
         return pl.forward(x).clone()
 
 
+class UNetResNet(_ArenaUNet):
+    """PyTorch-facing U-Net with a ResNet-34/101/152 encoder; same signature as the reference class."""
+    _arch = "UNetResNet"
+
+    def __init__(self, encoder_depth, num_classes, num_filters=32, dropout_2d=0.2, pretrained=False, is_deconv=False):
+        super().__init__()
+        self.num_classes = num_classes
+        self.dropout_2d = dropout_2d
+        self.encoder_depth = encoder_depth
+        self.num_filters = num_filters
+        if pretrained:
+            raise NotImplementedError("pretrained=True downloads ImageNet weights; load a state_dict instead")
+        if encoder_depth == 34:
+            self.encoder = torchvision.models.resnet34(weights=None)
+            bottom = 512
+        elif encoder_depth == 101:
+            self.encoder = torchvision.models.resnet101(weights=None)
+            bottom = 2048
+        elif encoder_depth == 152:
+            self.encoder = torchvision.models.resnet152(weights=None)
+            bottom = 2048
+        else:
+            raise NotImplementedError('only 34, 101, 152 version of Resnet are implemented')
+        self.bottom_channel_nr = bottom
+        self.pool = nn.MaxPool2d(2, 2)
+        self.relu = nn.ReLU(inplace=True)
+        self.conv1 = nn.Sequential(self.encoder.conv1, self.encoder.bn1, self.encoder.relu, self.pool)
+        self.conv2 = self.encoder.layer1
+        self.conv3 = self.encoder.layer2
+        self.conv4 = self.encoder.layer3
+        self.conv5 = self.encoder.layer4
+        nf = num_filters
+        self.center = DecoderBlockV2(bottom, nf * 8 * 2, nf * 8, is_deconv)
+        self.dec5 = DecoderBlockV2(bottom + nf * 8, nf * 8 * 2, nf * 8, is_deconv)
+        self.dec4 = DecoderBlockV2(bottom // 2 + nf * 8, nf * 8 * 2, nf * 8, is_deconv)
+        self.dec3 = DecoderBlockV2(bottom // 4 + nf * 8, nf * 4 * 2, nf * 2, is_deconv)
+        self.dec2 = DecoderBlockV2(bottom // 8 + nf * 2, nf * 2 * 2, nf * 2 * 2, is_deconv)
+        self.dec1 = DecoderBlockV2(nf * 2 * 2, nf * 2 * 2, nf, is_deconv)
+        self.dec0 = ConvRelu(nf, nf)
+        self.final = nn.Conv2d(nf, num_classes, kernel_size=1)
+        self._init_arenas()
+
+
 class AlbuNet(UNetResNet):
     """The reference's AlbuNet (src/unet_models.py:153-221): a ResNet34 encoder under the decoder of UNetResNet(34),
     without the dropout before the classifier.  Its module tree, state_dict keys and seeded initialisation equal
@@ -241,3 +267,84 @@ class AlbuNet(UNetResNet):
     def __init__(self, num_classes=1, num_filters=32, pretrained=False, is_deconv=False):
         super().__init__(34, num_classes, num_filters=num_filters, dropout_2d=0.0, pretrained=pretrained,
                          is_deconv=is_deconv)
+
+
+class _VGGUNet(_ArenaUNet):
+    """VGG-encoder U-Nets: every conv is conv + bias + ReLU (no BatchNorm), five 2x2 max-pools, and every pooled
+    stage output also feeds a decoder concat.  `_stages` lists the encoder (torchvision vgg.features) indices of each
+    stage's convs; engine.Plan builds the VGG launch plan from it."""
+    plan_kind = "vgg"
+    _size_multiple = 32
+    _stages = ()
+
+    def _vgg_features(self, builder, pretrained):
+        if pretrained:
+            raise NotImplementedError("pretrained=True downloads ImageNet weights; load a state_dict instead")
+        # the whole torchvision VGG, classifier included, as the reference builds it: the seeded initialisation consumes
+        # the random stream in the same order
+        return builder(weights=None).features
+
+
+class UNet11(_VGGUNet):
+    """The reference's UNet11 (src/unet_models.py:56-106): VGG11 encoder, DecoderBlock (3x3 transposed conv) decoder,
+    dec1 = ConvRelu over cat[dec2 (32), conv1 (64)]; same signature, module tree and state_dict keys."""
+    _arch = "UNet11"
+    _stages = ((0,), (3,), (6, 8), (11, 13), (16, 18))
+
+    def __init__(self, num_classes=1, num_filters=32, pretrained=False):
+        super().__init__()
+        self.num_classes = num_classes
+        self.pool = nn.MaxPool2d(2, 2)
+        self.encoder = self._vgg_features(torchvision.models.vgg11, pretrained)
+        self.relu = self.encoder[1]
+        self.conv1 = self.encoder[0]
+        self.conv2 = self.encoder[3]
+        self.conv3s = self.encoder[6]
+        self.conv3 = self.encoder[8]
+        self.conv4s = self.encoder[11]
+        self.conv4 = self.encoder[13]
+        self.conv5s = self.encoder[16]
+        self.conv5 = self.encoder[18]
+        nf = num_filters
+        self.center = DecoderBlock(nf * 8 * 2, nf * 8 * 2, nf * 8)
+        self.dec5 = DecoderBlock(nf * (16 + 8), nf * 8 * 2, nf * 8)
+        self.dec4 = DecoderBlock(nf * (16 + 8), nf * 8 * 2, nf * 4)
+        self.dec3 = DecoderBlock(nf * (8 + 4), nf * 4 * 2, nf * 2)
+        self.dec2 = DecoderBlock(nf * (4 + 2), nf * 2 * 2, nf)
+        self.dec1 = ConvRelu(nf * (2 + 1), nf)
+        self.final = nn.Conv2d(nf, num_classes, kernel_size=1)
+        self._init_arenas()
+
+
+class UNetVGG16(_VGGUNet):
+    """The reference's UNetVGG16 (src/unet_models.py:224-312): VGG16 encoder, DecoderBlockV2 decoder, dec1 = ConvRelu
+    over cat[dec2 (32), conv1 (64)]; same signature, module tree and state_dict keys.  The H100 path builds the
+    configured variant (src/models.py:25-28): is_deconv=True, dropout_2d=0."""
+    _arch = "UNetVGG16"
+    _stages = ((0, 2), (5, 7), (10, 12, 14), (17, 19, 21), (24, 26, 28))
+
+    def __init__(self, num_classes=1, num_filters=32, dropout_2d=0.2, pretrained=False, is_deconv=False):
+        super().__init__()
+        if not is_deconv:
+            raise NotImplementedError("the H100 path implements the configured is_deconv=True decoder "
+                                      "(src/models.py:25-28); the bilinear-upsample variant is not built")
+        self.num_classes = num_classes
+        self.dropout_2d = dropout_2d
+        self.pool = nn.MaxPool2d(2, 2)
+        self.encoder = self._vgg_features(torchvision.models.vgg16, pretrained)
+        self.relu = nn.ReLU(inplace=True)
+        e = self.encoder
+        self.conv1 = nn.Sequential(e[0], self.relu, e[2], self.relu)
+        self.conv2 = nn.Sequential(e[5], self.relu, e[7], self.relu)
+        self.conv3 = nn.Sequential(e[10], self.relu, e[12], self.relu, e[14], self.relu)
+        self.conv4 = nn.Sequential(e[17], self.relu, e[19], self.relu, e[21], self.relu)
+        self.conv5 = nn.Sequential(e[24], self.relu, e[26], self.relu, e[28], self.relu)
+        nf = num_filters
+        self.center = DecoderBlockV2(512, nf * 8 * 2, nf * 8, is_deconv)
+        self.dec5 = DecoderBlockV2(512 + nf * 8, nf * 8 * 2, nf * 8, is_deconv)
+        self.dec4 = DecoderBlockV2(512 + nf * 8, nf * 8 * 2, nf * 8, is_deconv)
+        self.dec3 = DecoderBlockV2(256 + nf * 8, nf * 4 * 2, nf * 2, is_deconv)
+        self.dec2 = DecoderBlockV2(128 + nf * 2, nf * 2 * 2, nf, is_deconv)
+        self.dec1 = ConvRelu(64 + nf, nf)
+        self.final = nn.Conv2d(nf, num_classes, kernel_size=1)
+        self._init_arenas()
