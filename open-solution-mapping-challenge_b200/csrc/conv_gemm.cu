@@ -37,9 +37,30 @@ static void pick_tile(int Wv, int Hv, int N, int max_rows, int row_mult, int* pb
   *pbw = bbw; *pbh = bbh; *pbn = bbn;
 }
 
-static int env_int(const char* name, int dflt) {
-  const char* v = getenv(name);
-  return v ? atoi(v) : dflt;
+// Launch rules.  The integer expressions that use these constants fix every launch's BN, stages and splits, and with
+// them the fp32 summation order: rewriting one can change a rounding, a split count and so the results' last bits.
+constexpr int kSmemBudget = 227 * 1024;               // dynamic shared memory of one CTA (the sm_90 maximum)
+constexpr int kMaxStagesHalo = 9, kMaxStages = 6;     // operand ring depth, haloed / per-tap path
+constexpr int kHaloMinChannels = 128;                 // haloed tile from this many channels per tap
+constexpr int kBn256MinWaveX10 = 6;                   // 256-wide N tiles down to 0.6 of a wave
+constexpr int kWgradWavesX10 = 10;                    // weight-gradient grid: one wave
+constexpr int kWgradMinKb = 6;                        // K blocks (pixel tiles) per weight-gradient CTA, at least
+constexpr int kWgradKbTarget = 64;                    // ... and aimed at for short reductions
+constexpr int kWgradMinWaveX10 = 4;                   // ... keeping at least 0.4 of a wave busy
+
+// Test hooks: they force a regime that a test's shapes would not reach under the launch rules.  Unset (the default),
+// the rules decide, and that is the only path the library takes in use.  Read on every launch, so that a test can
+// change them between calls.
+//   MCB_FORCE_BN      N tile width (ignored unless it divides the N extent)
+//   MCB_HALO          0 never the haloed 3x3 tile, 1 whenever it covers >= 80% of the view, 2 (default) use_halo's rule
+//   MCB_WGRAD_SPLITS  split-K count of the weight-gradient GEMMs
+struct TestHooks { int force_bn, halo, wgrad_splits; };
+static TestHooks test_hooks() {
+  auto get = [](const char* name, int dflt) {
+    const char* v = getenv(name);
+    return v ? atoi(v) : dflt;
+  };
+  return {get("MCB_FORCE_BN", 0), get("MCB_HALO", 2), get("MCB_WGRAD_SPLITS", 0)};
 }
 
 template <int BN, int BK, bool B_MN, bool HALO>
@@ -47,10 +68,10 @@ static int launch_conv_inst(const ConvGemmParams& p, dim3 grid, size_t smem, cud
   static bool attr_set = false;
   if (!attr_set) {
     MCB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, BK, B_MN, HALO>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
     attr_set = true;
   }
-  launch_pdl(conv_gemm_kernel<BN, BK, B_MN, HALO>, grid, kConvThreads, smem, st, p);
+  conv_gemm_kernel<BN, BK, B_MN, HALO><<<grid, kConvThreads, smem, st>>>(p);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -76,13 +97,7 @@ static int launch_conv(int BN, int BK, bool b_mn, ConvGemmParams& p, int m_tiles
   const int aux_bytes = p.aux_mode != 0 ? 2 * 128 * (BN >= 64 ? 64 : 32) * 2 : 0;  // one aux chunk per MMA warpgroup
   const int fixed = out_bytes + aux_bytes + kStatBytes + 1024 /*align*/ + 1536 /*barriers, row table*/ +
                     (halo ? 2 * a_bytes : 0);
-  const int budget = std::min(env_int("MCB_SMEM_BUDGET_KB", 227) * 1024, 232448);
-  int stages = std::max(2, std::min(env_int("MCB_MAX_STAGES", halo ? 9 : 6), (budget - fixed) / stage));
-  if (p.b_resident) {
-    // resident weights need one ring slot per tap, a single N tile and a single phase
-    if (halo && n_tiles == 1 && phases == 1 && (budget - fixed) / stage >= 9) stages = 9;
-    else p.b_resident = 0;
-  }
+  const int stages = std::max(2, std::min(halo ? kMaxStagesHalo : kMaxStages, (kSmemBudget - fixed) / stage));
   p.stages = stages;
   p.m_tiles = m_tiles; p.n_tiles = n_tiles; p.phases = phases;
   const size_t smem = (size_t)stages * stage + fixed;
@@ -105,14 +120,14 @@ static int launch_conv(int BN, int BK, bool b_mn, ConvGemmParams& p, int m_tiles
   // per-channel sums of the CTAs' rows, in CTA order (detsum.cuh)
   const int rows = (int)grid.x;
   if (p.aux_mode == 0) {
-    launch_pdl(conv_red_finish_kernel, det_finish_grid(2L * nch), kDetFinishThreads, 0, st, 0L, rows,
-               (long)p.red_stride, 2L * nch, (long)nch, p.stats + p.n_off, (long)p.stats_c);
+    conv_red_finish_kernel<<<det_finish_grid(2L * nch), kDetFinishThreads, 0, st>>>(
+        0L, rows, (long)p.red_stride, 2L * nch, (long)nch, p.stats + p.n_off, (long)p.stats_c);
   } else {
-    launch_pdl(conv_red_finish_kernel, det_finish_grid(nch), kDetFinishThreads, 0, st, 0L, rows, (long)p.red_stride,
-               (long)nch, (long)nch, p.bn_dbeta + p.n_off, 0L);
+    conv_red_finish_kernel<<<det_finish_grid(nch), kDetFinishThreads, 0, st>>>(
+        0L, rows, (long)p.red_stride, (long)nch, (long)nch, p.bn_dbeta + p.n_off, 0L);
     if (p.aux_mode == 2)
-      launch_pdl(conv_red_finish_kernel, det_finish_grid(nch), kDetFinishThreads, 0, st, (long)nch, rows,
-                 (long)p.red_stride, (long)nch, (long)nch, p.bn_dgamma + p.n_off, 0L);
+      conv_red_finish_kernel<<<det_finish_grid(nch), kDetFinishThreads, 0, st>>>(
+          (long)nch, rows, (long)p.red_stride, (long)nch, (long)nch, p.bn_dgamma + p.n_off, 0L);
   }
   MCB_LAUNCH_CHECK();
   return MCB_OK;
@@ -122,14 +137,11 @@ static int launch_conv(int BN, int BK, bool b_mn, ConvGemmParams& p, int m_tiles
 // k_channels = channels per tap of the GEMM-K dimension.  The haloed tile saves the nine per-tap fetches where they make
 // the kernel L2-bound (>= 128 channels on large images whose extent the 8x16 tile divides); on thin layers the
 // per-tile issue cost dominates and ragged small images waste rows.
-// MCB_HALO: 0 never, 1 whenever the tile covers >= 80%, 2 (default) the rule above.
+// (MCB_HALO overrides the rule in tests: see test_hooks)
 static bool use_halo(int ksize, int stride, int W, int H, int k_channels) {
-  const int mode = env_int("MCB_HALO", 2);
+  const int mode = test_hooks().halo;
   if (ksize != 3 || stride != 1 || mode == 0) return false;
-  // experimental (MCB_BRES=1, off by default): one-chunk layers (32 / 64 channels) take the haloed tile with
-  // RESIDENT weights -- one TMA load and 18 / 36 back-to-back MMAs per tile instead of 18 loads and 9 barrier waits
-  if (env_int("MCB_BRES", 0) == 1 && k_channels <= 64 && W % 8 == 0 && H % 16 == 0) return true;
-  if (mode == 2) return k_channels >= env_int("MCB_HALO_MINC", 128) && W % 8 == 0 && H % 16 == 0 && W >= 80;
+  if (mode == 2) return k_channels >= kHaloMinChannels && W % 8 == 0 && H % 16 == 0 && W >= 80;
   const double eff = (double)W * H / ((double)((W + 7) / 8) * 8 * ((H + 15) / 16) * 16);
   return eff >= 0.8;
 }
@@ -143,9 +155,9 @@ static int pick_bn(int n_total, long m_tiles, int phases) {
   const long sms = num_sms();
   // (fat tiles beat many thin ones: go below 128 only when even 128-wide tiles leave most SMs idle; one round of
   // 256-wide tiles beats two rounds of 128-wide ones until the tile count falls below ~0.6 of a wave)
-  if (bn > 128 && m_tiles * phases * (n_total / bn) * 10 < sms * env_int("MCB_BN256_MIN_WAVE_X10", 6)) bn = 128;
+  if (bn > 128 && m_tiles * phases * (n_total / bn) * 10 < sms * kBn256MinWaveX10) bn = 128;
   if (bn > 64 && n_total % 64 == 0 && m_tiles * phases * (n_total / bn) < sms / 3) bn = 64;
-  int forced = env_int("MCB_FORCE_BN", 0);
+  const int forced = test_hooks().force_bn;
   if (forced && n_total % forced == 0) bn = forced;
   return bn;
 }
@@ -270,7 +282,6 @@ static int plan_conv(ConvGemmParams& p, const TapRule& rule, const View* a, int 
     if (aux)
       if (int r = encode_view(&p.tmX[ph], aux_view, phase_slot[ph], cw, p.bw, p.bh, p.bn)) return r;
   }
-  p.b_resident = (halo && nsrc == 1 && a[0].c == BK && env_int("MCB_BRES", 0) == 1) ? 1 : 0;
   return launch_conv(BN, BK, b_mn, p, (int)m_tiles, out.c / BN, phases, st, halo);
 }
 
@@ -278,10 +289,10 @@ template <int BN>
 static int launch_wgrad_inst(const WgradParams& p, dim3 grid, size_t smem, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    MCB_CHECK_CUDA(cudaFuncSetAttribute(wgrad_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    MCB_CHECK_CUDA(cudaFuncSetAttribute(wgrad_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
     attr_set = true;
   }
-  launch_pdl(wgrad_kernel<BN>, grid, kGemmThreads, smem, st, p);
+  wgrad_kernel<BN><<<grid, kGemmThreads, smem, st>>>(p);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -317,21 +328,17 @@ static int launch_wgrad(WgradParams& p, int cin_src, cudaStream_t st) {
   // streams are L2/HBM-bound and want every SM busy.  So: exactly ONE resident wave of CTAs (never a ragged second
   // wave; the 384-thread CTA takes the whole register file, one CTA per SM) and at least `min_kb` K blocks per CTA.
   const long base = (long)m_tiles * n_tiles * p.ntaps;
-  const long cap = (long)num_sms() * env_int("MCB_WGRAD_WAVES_X10", 10) / 10;
+  const long cap = (long)num_sms() * kWgradWavesX10 / 10;
   int splits = (int)std::max(1L, std::min((long)p.tiles_total, cap / std::max(1L, base)));
-  const int min_kb = env_int("MCB_WGRAD_MIN_KB", 6);
-  splits = std::max(1, std::min(splits, std::max(1, p.tiles_total / min_kb)));
+  splits = std::max(1, std::min(splits, std::max(1, p.tiles_total / kWgradMinKb)));
   // short reductions (deep layers: few pixel tiles, many weights) are bound by the fp32 red.add epilogues, not by the
-  // operand streams: aim for `kb_target` K blocks per CTA, but keep at least 0.4 of a wave busy (on the full step
+  // operand streams: aim for kWgradKbTarget K blocks per CTA, but keep at least 0.4 of a wave busy (on the full step
   // these GEMMs share the SMs with the BatchNorm-backward kernels)
-  const int kb_target = env_int("MCB_WGRAD_KB_TARGET", 64);
-  if (kb_target > 0) {
-    const long lo_cap = cap * env_int("MCB_WGRAD_MIN_WAVE_X10", 4) / 10;
-    const int lo = (int)std::max(1L, lo_cap / std::max(1L, base));
-    const int want = std::max(1, p.tiles_total / kb_target);
-    splits = std::max(1, std::min(splits, std::max(lo, want)));
-  }
-  int forced = env_int("MCB_WGRAD_SPLITS", 0);
+  const long lo_cap = cap * kWgradMinWaveX10 / 10;
+  const int lo = (int)std::max(1L, lo_cap / std::max(1L, base));
+  const int want = std::max(1, p.tiles_total / kWgradKbTarget);
+  splits = std::max(1, std::min(splits, std::max(lo, want)));
+  const int forced = test_hooks().wgrad_splits;
   if (forced > 0) splits = std::min(forced, p.tiles_total);
   // several splits store their partial products in split-ordered rows of the workspace (summed deterministically below)
   p.cin_src = cin_src;
@@ -341,9 +348,8 @@ static int launch_wgrad(WgradParams& p, int cin_src, cudaStream_t st) {
   p.splits = splits;
   const int b_cw = BN >= 64 ? 64 : 32;
   const int stage = 2 * 64 * 128 + (BN / b_cw) * 64 * b_cw * 2;
-  const int budget = env_int("MCB_SMEM_BUDGET_KB", 227) * 1024;
   const int per = (p.tiles_total + splits - 1) / splits;
-  p.stages = std::max(2, std::min(std::min(per, 8), budget / stage));
+  p.stages = std::max(2, std::min(std::min(per, 8), kSmemBudget / stage));
   const size_t smem = (size_t)p.stages * stage + 1024 + 512;
   dim3 grid(n_tiles, m_tiles, p.ntaps * splits);
   int r;
@@ -356,8 +362,8 @@ static int launch_wgrad(WgradParams& p, int cin_src, cudaStream_t st) {
   if (r || splits == 1) return r;
   // the splits that own pixel tiles, summed in split order into dW[tap][cout][ci_off + ci] (detsum.cuh)
   const int rows = (p.tiles_total + per - 1) / per;
-  launch_pdl(wgrad_red_finish_kernel, det_finish_grid(p.slice), kDetFinishThreads, 0, st, p.ws_off, rows, p.slice, p.slice,
-             (long)cin_src, p.dw + p.ci_off, (long)p.cin_total);
+  wgrad_red_finish_kernel<<<det_finish_grid(p.slice), kDetFinishThreads, 0, st>>>(
+      p.ws_off, rows, p.slice, p.slice, (long)cin_src, p.dw + p.ci_off, (long)p.cin_total);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }

@@ -53,8 +53,6 @@ struct ConvGemmParams {
   int tiles_x, tiles_y;
   int m_tiles, n_tiles, phases;  // persistent tile space: phases x m_tiles x n_tiles
   int stages;
-  int b_resident;  // HALO only, experimental: the 9 per-tap weight tiles are loaded ONCE per CTA into ring slots 0..8
-                   // (single N tile, one channel chunk) instead of once per pixel tile
   int n_off;  // first N (weight row / column) coordinate of this launch (concat source slice for dgrad)
   // epilogue:  v = acc * scale[c] + bias[c] + residual[pix][c];  v = relu(v);  v = mask ? v : 0
   const float* scale;              // per-channel multiplier (inference-mode BatchNorm folded into the epilogue), or null
@@ -196,7 +194,6 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
     tc::prefetch_tmap(&p.tmA[0]);
   }
   __syncthreads();
-  pdl_prologue();  // everything above touched only shared memory / kernel parameters
 
   if (warp < 4) {
     tc::regs_dealloc<kProducerRegs>();
@@ -240,15 +237,10 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
             }
             for (int t = 0; t < 9; ++t) {
               const TapDesc tap = p.taps[tap_begin + t * nsrc + sidx];
-              int s = ring_s;
+              const int s = ring_s;
               const uint32_t ph = ring_ph;
               if (++ring_s == stages) { ring_s = 0; ring_ph ^= 1; }
-              if (p.b_resident) {
-                if (ag != 0) continue;   // weights of tap t already sit in slot t
-                s = t;
-              } else {
-                tc::mbar_wait(&empty_bar[s], ph ^ 1);
-              }
+              tc::mbar_wait(&empty_bar[s], ph ^ 1);
               uint8_t* sb = smem + (size_t)s * STAGE_BYTES;
               if (tc::elect_one()) {
                 tc::mbar_expect_tx(&full_bar[s], B_BYTES);
@@ -379,19 +371,14 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
             const uint32_t a_base = tc::smem_u32(a_ring + (size_t)as * A_BYTES) + (uint32_t)(wg * 8 * kHaloW * A_ROW_BYTES);
             for (int tt = 0; tt < 9; ++tt, ++i) {
               const TapDesc tap = p.taps[tap_begin + tt * nsrc + sidx];
-              int s = ring_s;
+              const int s = ring_s;
               const uint32_t ph = ring_ph;
               if (++ring_s == stages) { ring_s = 0; ring_ph ^= 1; }
-              if (p.b_resident) {
-                s = tt;
-                if (ag == 0) tc::mbar_wait(&full_bar[s], 0);   // first tile of this CTA only
-              } else {
-                tc::mbar_wait(&full_bar[s], ph);
-              }
+              tc::mbar_wait(&full_bar[s], ph);
               const uint32_t sa = a_base + (uint32_t)(((1 + tap.dy) * kHaloW + (1 + tap.dx)) * A_ROW_BYTES);
               mma_block(tc::make_smem_desc(sa, 16, kHaloW * A_ROW_BYTES, A_LAYOUT),
                         b_desc(tc::smem_u32(smem + (size_t)s * STAGE_BYTES)), i == 0);
-              prev_s = p.b_resident ? -1 : s;
+              prev_s = s;
               prev_as = (tt == 8) ? as : -1;
             }
           }
@@ -658,7 +645,6 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgrad_kernel(const __grid_con
     tc::fence_barrier_init();
   }
   __syncthreads();
-  pdl_prologue();  // everything above touched only shared memory / kernel parameters
   if (num_kb == 0) return;
 
   if (warp < 4) {

@@ -34,6 +34,5 @@ inline dim3 det_finish_grid(long n) { return dim3((unsigned)((n + 7) / 8)); }
   static __device__ T WS[CAP];                                                                                    \
   __global__ void __launch_bounds__(mcb::kDetFinishThreads)                                                       \
       FINISH(long ws_off, int rows, long row_stride, long n, long inner, T* out, long out_stride) {               \
-    mcb::pdl_prologue();                                                                                          \
     mcb::det_finish_body<T>(WS + ws_off, rows, row_stride, n, inner, out, out_stride);                            \
   }

@@ -37,7 +37,6 @@ static inline int grid_for(long work_items, int threads, int per_sm = 8) {
 // ------------------------------------------------------------------------------------------ layout conversion
 __global__ void nchw_f32_to_nhwc_bf16_kernel(const float* __restrict__ x, bf16* __restrict__ y, int N, int C, int H,
                                              int W) {
-  mcb::pdl_prologue();
   const long total = (long)N * H * W * C;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int c = i % C;
@@ -50,7 +49,6 @@ __global__ void nchw_f32_to_nhwc_bf16_kernel(const float* __restrict__ x, bf16* 
 }
 __global__ void nhwc_bf16_to_nchw_f32_kernel(const bf16* __restrict__ x, float* __restrict__ y, int N, int C, int H,
                                              int W) {
-  mcb::pdl_prologue();
   const long total = (long)N * H * W * C;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int w = i % W;
@@ -71,7 +69,6 @@ constexpr int STEM_COLS = 2 * STEM_SW + 5;       // input columns a strip touche
 // thread assembles 16-byte groups of 8 k-values; consecutive threads write consecutive 16-byte groups.
 __global__ void __launch_bounds__(256) stem_im2col_kernel(const float* __restrict__ x, bf16* __restrict__ col, int N,
                                                           int H, int W) {
-  mcb::pdl_prologue();
   __shared__ float s[3][7][STEM_COLS + 1];
   const int Ho = H / 2, Wo = W / 2;
   const int strips = (Wo + STEM_SW - 1) / STEM_SW;
@@ -111,7 +108,6 @@ __global__ void __launch_bounds__(256) stem_im2col_kernel(const float* __restric
 }
 // master stem weight fp32 [7][7][64][3] (tap-major like every conv) <-> GEMM operand bf16 [64][192]
 __global__ void stem_pack_weight_kernel(const float* __restrict__ w, bf16* __restrict__ wp) {
-  mcb::pdl_prologue();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= 64 * 192) return;
   const int k = i % 192, co = i / 192;
@@ -123,7 +119,6 @@ __global__ void stem_pack_weight_kernel(const float* __restrict__ w, bf16* __res
   wp[i] = __float2bfloat16(v);
 }
 __global__ void stem_unpack_wgrad_kernel(const float* __restrict__ dwp, float* __restrict__ dw) {
-  mcb::pdl_prologue();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= 49 * 64 * 3) return;
   const int c = i % 3, co = (i / 3) % 64, tap = i / 192;
@@ -140,7 +135,6 @@ constexpr int VIN_COLS = VIN_SW + 2;        // input columns a strip touches
 // assembles 16-byte groups of 8 k-values (4 per pixel); consecutive threads write consecutive 16-byte groups.
 __global__ void __launch_bounds__(256) vgg_input_im2col_kernel(const float* __restrict__ x, bf16* __restrict__ col,
                                                                int N, int H, int W) {
-  mcb::pdl_prologue();
   __shared__ float s[3][3][VIN_COLS + 1];
   const int strips = (W + VIN_SW - 1) / VIN_SW;
   const int strip = blockIdx.x % strips;
@@ -178,7 +172,6 @@ __global__ void __launch_bounds__(256) vgg_input_im2col_kernel(const float* __re
 }
 // master weight fp32 [3][3][64][3] (tap-major like every conv) <-> GEMM operand bf16 [64][32]
 __global__ void vgg_input_pack_weight_kernel(const float* __restrict__ w, bf16* __restrict__ wp) {
-  mcb::pdl_prologue();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= 64 * 32) return;
   const int k = i % 32, co = i / 32;
@@ -190,7 +183,6 @@ __global__ void vgg_input_pack_weight_kernel(const float* __restrict__ w, bf16* 
   wp[i] = __float2bfloat16(v);
 }
 __global__ void vgg_input_unpack_wgrad_kernel(const float* __restrict__ dwp, float* __restrict__ dw) {
-  mcb::pdl_prologue();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= 9 * 64 * 3) return;
   const int c = i % 3, co = (i / 3) % 64, tap = i / 192;
@@ -205,7 +197,6 @@ __global__ void bn_finalize_kernel(const float* __restrict__ stats, float count,
                                    float* __restrict__ running_var, float momentum, float eps,
                                    float* __restrict__ scale, float* __restrict__ shift, float* __restrict__ mean_out,
                                    float* __restrict__ invstd_out, int C) {
-  mcb::pdl_prologue();
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const float mean = stats[c] / count;
@@ -226,7 +217,6 @@ __global__ void bn_finalize_kernel(const float* __restrict__ stats, float count,
 __global__ void bn_eval_params_kernel(const float* __restrict__ gamma, const float* __restrict__ beta,
                                       const float* __restrict__ rm, const float* __restrict__ rv, float eps,
                                       float* __restrict__ scale, float* __restrict__ shift, int C) {
-  mcb::pdl_prologue();
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const float sc = gamma[c] * rsqrtf(rv[c] + eps);
@@ -237,7 +227,6 @@ __global__ void bn_eval_params_kernel(const float* __restrict__ gamma, const flo
 // every BatchNorm of the net in one launch (inference): table rows = {gamma, beta, running_mean, running_var, scale,
 // shift, C} as 64-bit values; blockIdx.y = BN index
 __global__ void bn_eval_params_batched_kernel(const long long* __restrict__ table, float eps) {
-  mcb::pdl_prologue();
   const long long* row = table + (long long)blockIdx.y * 7;
   const float* gamma = reinterpret_cast<const float*>(row[0]);
   const float* beta = reinterpret_cast<const float*>(row[1]);
@@ -261,7 +250,6 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const uint4* __restrict__
                                                        const float* __restrict__ shift, const uint4* __restrict__ r,
                                                        const float* __restrict__ rscale, const float* __restrict__ rshift,
                                                        int relu, uint4* __restrict__ y, long total8, int C8) {
-  mcb::pdl_prologue();
   const long stride = (long)gridDim.x * blockDim.x;
   long i = blockIdx.x * (long)blockDim.x + threadIdx.x;
   const int c0 = (int)(i % C8) * 8;
@@ -343,7 +331,6 @@ __global__ void __launch_bounds__(256) bn_train_apply_kernel(const uint4* __rest
                                                              const uint4* __restrict__ r, BNTrain rbn, int relu,
                                                              uint4* __restrict__ y, long total8, int C8, float count,
                                                              float eps, float momentum) {
-  mcb::pdl_prologue();
   const long stride = (long)gridDim.x * blockDim.x;
   long i = blockIdx.x * (long)blockDim.x + threadIdx.x;
   const int c0 = (int)(i % C8) * 8;
@@ -399,7 +386,6 @@ __global__ void channel_reduce_kernel(const uint4* __restrict__ a, const uint4* 
                                       const uint4* __restrict__ z, const float* __restrict__ mean,
                                       const float* __restrict__ invstd, float* __restrict__ out0,
                                       float* __restrict__ out1, long pixels, int C8) {
-  mcb::pdl_prologue();
   extern __shared__ float red[];  // [2][256][8]
   const int cg = threadIdx.x % C8;
   const int lane_p = threadIdx.x / C8;
@@ -489,7 +475,6 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const uint4* __restri
                                                            const float* __restrict__ dbeta, const float* __restrict__ dgamma,
                                                            float inv_count, uint4* __restrict__ dz, uint4* __restrict__ g_out,
                                                            long total8, int C8) {
-  mcb::pdl_prologue();
   const long stride = (long)gridDim.x * blockDim.x;
   long i = blockIdx.x * (long)blockDim.x + threadIdx.x;
   const int c0 = (int)(i % C8) * 8;
@@ -548,7 +533,6 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const uint4* __restri
 
 // ------------------------------------------------------------------------------------------ 2x2 max-pool
 __global__ void maxpool2_fwd_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int N, int H, int W, int C8) {
-  mcb::pdl_prologue();
   const int Ho = H / 2, Wo = W / 2;
   const long total = (long)N * Ho * Wo * C8;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -571,7 +555,6 @@ __global__ void maxpool2_fwd_kernel(const uint4* __restrict__ x, uint4* __restri
 // dx = (store | accumulate) routed gradient
 __global__ void maxpool2_bwd_kernel(const uint4* __restrict__ x, const uint4* __restrict__ dy, uint4* __restrict__ dx,
                                     int accumulate, int N, int H, int W, int C8) {
-  mcb::pdl_prologue();
   const int Ho = H / 2, Wo = W / 2;
   const long total = (long)N * Ho * Wo * C8;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -616,7 +599,6 @@ __global__ void maxpool2_bwd_kernel(const uint4* __restrict__ x, const uint4* __
 // channel_reduce_kernel; a pooled pixel is one 2x2 window.
 __global__ void maxpool2_bwd_skip_relu_kernel(const uint4* __restrict__ y, const uint4* __restrict__ dpool,
                                               uint4* __restrict__ g, long pooled, int H, int W, int C8) {
-  mcb::pdl_prologue();
   extern __shared__ float red[];  // [blockDim.x][8]
   const int cg = threadIdx.x % C8;
   const int lane_p = threadIdx.x / C8;
@@ -678,7 +660,6 @@ __global__ void maxpool2_bwd_skip_relu_kernel(const uint4* __restrict__ y, const
 __global__ void final_conv_fwd_kernel(const uint4* __restrict__ x, const float* __restrict__ w,
                                       const float* __restrict__ b, float* __restrict__ logits, long pixels_per_img,
                                       long pixels, int C, int K) {
-  mcb::pdl_prologue();
   extern __shared__ float sw[];  // K*C + K
   for (int i = threadIdx.x; i < K * C + K; i += blockDim.x) sw[i] = (i < K * C) ? w[i] : b[i - K * C];
   __syncthreads();
@@ -702,7 +683,6 @@ __global__ void final_conv_bwd_kernel(const uint4* __restrict__ x, const float* 
                                       const float* __restrict__ dlogits, uint4* __restrict__ dx,
                                       float* __restrict__ dw, float* __restrict__ db, long pixels_per_img,
                                       long pixels, int C, int K) {
-  mcb::pdl_prologue();
   extern __shared__ float sm[];  // K*C weights, then per warp K*C + K accumulators
   float* sw = sm;
   float* sacc = sm + K * C;
@@ -769,7 +749,6 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
                             float* __restrict__ v, bf16* __restrict__ p_bf16, long n, float lr, float beta1,
                             float beta2, float eps, float wd, float bc1, float bc2_sqrt, float grad_scale,
                             const float* __restrict__ hyper) {
-  mcb::pdl_prologue();
   if (hyper != nullptr) {
     lr = __ldg(hyper);
     bc1 = __ldg(hyper + 1);
@@ -789,7 +768,6 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
   }
 }
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ x, bf16* __restrict__ y, long n) {
-  mcb::pdl_prologue();
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
     y[i] = __float2bfloat16(x[i]);
 }
@@ -802,14 +780,14 @@ using namespace mcb;
 extern "C" int mcb_nchw_f32_to_nhwc_bf16(const float* x, void* y, int n, int c, int h, int w, void* stream) {
   MCB_REQUIRE(x && y, "null pointer");
   const long total = (long)n * c * h * w;
-  launch_pdl(nchw_f32_to_nhwc_bf16_kernel, grid_for(total, 256), 256, 0, ST, x, (bf16*)y, n, c, h, w);
+  nchw_f32_to_nhwc_bf16_kernel<<<grid_for(total, 256), 256, 0, ST>>>(x, (bf16*)y, n, c, h, w);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
 extern "C" int mcb_nhwc_bf16_to_nchw_f32(const void* x, float* y, int n, int c, int h, int w, void* stream) {
   MCB_REQUIRE(x && y, "null pointer");
   const long total = (long)n * c * h * w;
-  launch_pdl(nhwc_bf16_to_nchw_f32_kernel, grid_for(total, 256), 256, 0, ST, (const bf16*)x, y, n, c, h, w);
+  nhwc_bf16_to_nchw_f32_kernel<<<grid_for(total, 256), 256, 0, ST>>>((const bf16*)x, y, n, c, h, w);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -818,19 +796,19 @@ extern "C" int mcb_stem_im2col(const float* x, void* col, int n, int h, int w, v
   MCB_REQUIRE(h % 2 == 0 && w % 2 == 0, "stem_im2col: odd size");
   const long ctas = (long)n * (h / 2) * (((w / 2) + STEM_SW - 1) / STEM_SW);  // one per strip of an output row
   MCB_REQUIRE(ctas < (1L << 31), "stem_im2col: too many strips");
-  launch_pdl(stem_im2col_kernel, dim3((unsigned)ctas), 256, 0, ST, x, (bf16*)col, n, h, w);
+  stem_im2col_kernel<<<dim3((unsigned)ctas), 256, 0, ST>>>(x, (bf16*)col, n, h, w);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
 extern "C" int mcb_stem_pack_weight(const float* w, void* wp, void* stream) {
   MCB_REQUIRE(w && wp, "null pointer");
-  launch_pdl(stem_pack_weight_kernel, (64 * 192 + 255) / 256, 256, 0, ST, w, (bf16*)wp);
+  stem_pack_weight_kernel<<<(64 * 192 + 255) / 256, 256, 0, ST>>>(w, (bf16*)wp);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
 extern "C" int mcb_stem_unpack_wgrad(const float* dwp, float* dw, void* stream) {
   MCB_REQUIRE(dwp && dw, "null pointer");
-  launch_pdl(stem_unpack_wgrad_kernel, (49 * 64 * 3 + 255) / 256, 256, 0, ST, dwp, dw);
+  stem_unpack_wgrad_kernel<<<(49 * 64 * 3 + 255) / 256, 256, 0, ST>>>(dwp, dw);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -839,19 +817,19 @@ extern "C" int mcb_vgg_input_im2col(const float* x, void* col, int n, int h, int
   MCB_REQUIRE(n > 0 && h > 0 && w > 0, "vgg_input_im2col: size %dx%dx%d", n, h, w);
   const long ctas = (long)n * h * ((w + VIN_SW - 1) / VIN_SW);  // one per strip of a row
   MCB_REQUIRE(ctas < (1L << 31), "vgg_input_im2col: too many strips");
-  launch_pdl(vgg_input_im2col_kernel, dim3((unsigned)ctas), 256, 0, ST, x, (bf16*)col, n, h, w);
+  vgg_input_im2col_kernel<<<dim3((unsigned)ctas), 256, 0, ST>>>(x, (bf16*)col, n, h, w);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
 extern "C" int mcb_vgg_input_pack_weight(const float* w, void* wp, void* stream) {
   MCB_REQUIRE(w && wp, "null pointer");
-  launch_pdl(vgg_input_pack_weight_kernel, (64 * 32 + 255) / 256, 256, 0, ST, w, (bf16*)wp);
+  vgg_input_pack_weight_kernel<<<(64 * 32 + 255) / 256, 256, 0, ST>>>(w, (bf16*)wp);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
 extern "C" int mcb_vgg_input_unpack_wgrad(const float* dwp, float* dw, void* stream) {
   MCB_REQUIRE(dwp && dw, "null pointer");
-  launch_pdl(vgg_input_unpack_wgrad_kernel, (9 * 64 * 3 + 255) / 256, 256, 0, ST, dwp, dw);
+  vgg_input_unpack_wgrad_kernel<<<(9 * 64 * 3 + 255) / 256, 256, 0, ST>>>(dwp, dw);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -860,8 +838,8 @@ extern "C" int mcb_bn_finalize(const float* stats, long count, const float* gamm
                                float* running_mean, float* running_var, float momentum, float eps, float* scale,
                                float* shift, float* mean, float* invstd, int c, void* stream) {
   MCB_REQUIRE(stats && gamma && beta && scale && shift && mean && invstd, "bn_finalize: null pointer");
-  launch_pdl(bn_finalize_kernel, (c + 127) / 128, 128, 0, ST, stats, (float)count, gamma, beta, running_mean, running_var,
-                                                      momentum, eps, scale, shift, mean, invstd, c);
+  bn_finalize_kernel<<<(c + 127) / 128, 128, 0, ST>>>(
+      stats, (float)count, gamma, beta, running_mean, running_var, momentum, eps, scale, shift, mean, invstd, c);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -869,14 +847,14 @@ extern "C" int mcb_bn_eval_params(const float* gamma, const float* beta, const f
                                   const float* running_var, float eps, float* scale, float* shift, int c,
                                   void* stream) {
   MCB_REQUIRE(gamma && beta && running_mean && running_var && scale && shift, "bn_eval_params: null pointer");
-  launch_pdl(bn_eval_params_kernel, (c + 127) / 128, 128, 0, ST, gamma, beta, running_mean, running_var, eps, scale, shift, c);
+  bn_eval_params_kernel<<<(c + 127) / 128, 128, 0, ST>>>(gamma, beta, running_mean, running_var, eps, scale, shift, c);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
 extern "C" int mcb_bn_eval_params_batched(const long long* table, int n_bn, int max_c, float eps, void* stream) {
   MCB_REQUIRE(table && n_bn > 0 && max_c > 0, "bn_eval_params_batched: bad arguments");
   dim3 grid((max_c + 255) / 256, n_bn);
-  launch_pdl(bn_eval_params_batched_kernel, grid, 256, 0, ST, table, eps);
+  bn_eval_params_batched_kernel<<<grid, 256, 0, ST>>>(table, eps);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -889,14 +867,14 @@ extern "C" int mcb_bn_apply(const void* z, const float* scale, const float* shif
   const long total8 = pixels * (c / 8);
   const int grid = grid_for((total8 + 1) / 2, 256);
   if (residual == nullptr)
-    launch_pdl(bn_apply_kernel<0>, grid, 256, 0, ST, (const uint4*)z, scale, shift, nullptr, nullptr, nullptr, relu, (uint4*)y,
-                                             total8, c / 8);
+    bn_apply_kernel<0><<<grid, 256, 0, ST>>>(
+        (const uint4*)z, scale, shift, nullptr, nullptr, nullptr, relu, (uint4*)y, total8, c / 8);
   else if (res_scale == nullptr)
-    launch_pdl(bn_apply_kernel<1>, grid, 256, 0, ST, (const uint4*)z, scale, shift, (const uint4*)residual, nullptr, nullptr,
-                                             relu, (uint4*)y, total8, c / 8);
+    bn_apply_kernel<1><<<grid, 256, 0, ST>>>(
+        (const uint4*)z, scale, shift, (const uint4*)residual, nullptr, nullptr, relu, (uint4*)y, total8, c / 8);
   else
-    launch_pdl(bn_apply_kernel<2>, grid, 256, 0, ST, (const uint4*)z, scale, shift, (const uint4*)residual, res_scale,
-                                             res_shift, relu, (uint4*)y, total8, c / 8);
+    bn_apply_kernel<2><<<grid, 256, 0, ST>>>(
+        (const uint4*)z, scale, shift, (const uint4*)residual, res_scale, res_shift, relu, (uint4*)y, total8, c / 8);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -921,11 +899,14 @@ extern "C" int mcb_bn_train_apply_global(const void* z, const mcb_bn_train* bn, 
                            res_bn->mean, res_bn->invstd};
   const float count = (float)stat_count;
   if (residual == nullptr)
-    launch_pdl(bn_train_apply_kernel<0>, grid, 256, 0, ST, (const uint4*)z, b, nullptr, rb, relu, (uint4*)y, total8, c / 8, count, eps, momentum);
+    bn_train_apply_kernel<0><<<grid, 256, 0, ST>>>(
+        (const uint4*)z, b, nullptr, rb, relu, (uint4*)y, total8, c / 8, count, eps, momentum);
   else if (res_bn == nullptr)
-    launch_pdl(bn_train_apply_kernel<1>, grid, 256, 0, ST, (const uint4*)z, b, (const uint4*)residual, rb, relu, (uint4*)y, total8, c / 8, count, eps, momentum);
+    bn_train_apply_kernel<1><<<grid, 256, 0, ST>>>(
+        (const uint4*)z, b, (const uint4*)residual, rb, relu, (uint4*)y, total8, c / 8, count, eps, momentum);
   else
-    launch_pdl(bn_train_apply_kernel<2>, grid, 256, 0, ST, (const uint4*)z, b, (const uint4*)residual, rb, relu, (uint4*)y, total8, c / 8, count, eps, momentum);
+    bn_train_apply_kernel<2><<<grid, 256, 0, ST>>>(
+        (const uint4*)z, b, (const uint4*)residual, rb, relu, (uint4*)y, total8, c / 8, count, eps, momentum);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -944,10 +925,10 @@ extern "C" int mcb_channel_sum(const void* x, float* out, long pixels, int c, vo
   const int lanes = threads / c8;
   const int grid = (int)std::max(1L, std::min((pixels + lanes * 4 - 1) / (lanes * 4), (long)num_sms() * 4));
   MCB_REQUIRE((long)grid * 2 * c <= kChannelRedCap, "channel_sum: %d blocks x %d channels exceed the workspace", grid, c);
-  launch_pdl(channel_reduce_kernel<0>, grid, threads, (size_t)threads * 8 * 2 * sizeof(float), ST, 
+  channel_reduce_kernel<0><<<grid, threads, (size_t)threads * 8 * 2 * sizeof(float), ST>>>(
       (const uint4*)x, nullptr, nullptr, nullptr, nullptr, out, nullptr, pixels, c8);
-  launch_pdl(channel_red_finish_kernel, det_finish_grid(c), kDetFinishThreads, 0, ST, 0L, grid, 2L * c, (long)c,
-             (long)c, out, 0L);
+  channel_red_finish_kernel<<<det_finish_grid(c), kDetFinishThreads, 0, ST>>>(
+      0L, grid, 2L * c, (long)c, (long)c, out, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -959,12 +940,12 @@ extern "C" int mcb_bn_bwd_reduce(const void* dy, const void* y_mask, const void*
   const int lanes = threads / c8;
   const int grid = (int)std::max(1L, std::min((pixels + lanes * 4 - 1) / (lanes * 4), (long)num_sms() * 4));
   MCB_REQUIRE((long)grid * 2 * c <= kChannelRedCap, "bn_bwd_reduce: %d blocks x %d channels exceed the workspace", grid, c);
-  launch_pdl(channel_reduce_kernel<1>, grid, threads, (size_t)threads * 8 * 2 * sizeof(float), ST, 
+  channel_reduce_kernel<1><<<grid, threads, (size_t)threads * 8 * 2 * sizeof(float), ST>>>(
       (const uint4*)dy, (const uint4*)y_mask, (const uint4*)z, mean, invstd, dbeta, dgamma, pixels, c8);
-  launch_pdl(channel_red_finish_kernel, det_finish_grid(c), kDetFinishThreads, 0, ST, 0L, grid, 2L * c, (long)c,
-             (long)c, dbeta, 0L);
-  launch_pdl(channel_red_finish_kernel, det_finish_grid(c), kDetFinishThreads, 0, ST, (long)c, grid, 2L * c, (long)c,
-             (long)c, dgamma, 0L);
+  channel_red_finish_kernel<<<det_finish_grid(c), kDetFinishThreads, 0, ST>>>(
+      0L, grid, 2L * c, (long)c, (long)c, dbeta, 0L);
+  channel_red_finish_kernel<<<det_finish_grid(c), kDetFinishThreads, 0, ST>>>(
+      (long)c, grid, 2L * c, (long)c, (long)c, dgamma, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -986,9 +967,9 @@ extern "C" int mcb_bn_bwd_apply_global(const void* dy, const void* y_mask, const
   const int grid = grid_for((total8 + 1) / 2, 256);
   const float ic = 1.0f / (float)stat_count;
 #define MCB_BWD(MASK, GOUT)                                                                                         \
-  launch_pdl(bn_bwd_apply_kernel<MASK, GOUT>, grid, 256, 0, ST, (const uint4*)dy, (const uint4*)y_mask, (const uint4*)z, mean, \
-                                                        invstd, gamma, dbeta, dgamma, ic, (uint4*)dz, (uint4*)g_out,  \
-                                                        total8, c / 8)
+  bn_bwd_apply_kernel<MASK, GOUT><<<grid, 256, 0, ST>>>(                                                            \
+      (const uint4*)dy, (const uint4*)y_mask, (const uint4*)z, mean, invstd, gamma, dbeta, dgamma, ic, (uint4*)dz,  \
+      (uint4*)g_out, total8, c / 8)
   const int gout = g_out == nullptr ? 0 : (g_accumulate ? 2 : 1);
   if (y_mask != nullptr) {
     if (gout == 0) MCB_BWD(true, 0); else if (gout == 1) MCB_BWD(true, 1); else MCB_BWD(true, 2);
@@ -1004,7 +985,7 @@ extern "C" int mcb_maxpool2_fwd(const void* x, void* y, int n, int h, int w, int
   MCB_REQUIRE(x && y, "maxpool2_fwd: null pointer");
   MCB_REQUIRE(c % 8 == 0 && h % 2 == 0 && w % 2 == 0, "maxpool2_fwd: shape");
   const long total = (long)n * (h / 2) * (w / 2) * (c / 8);
-  launch_pdl(maxpool2_fwd_kernel, grid_for(total, 256), 256, 0, ST, (const uint4*)x, (uint4*)y, n, h, w, c / 8);
+  maxpool2_fwd_kernel<<<grid_for(total, 256), 256, 0, ST>>>((const uint4*)x, (uint4*)y, n, h, w, c / 8);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -1013,8 +994,8 @@ extern "C" int mcb_maxpool2_bwd(const void* x, const void* dy, void* dx, int acc
   MCB_REQUIRE(x && dy && dx, "maxpool2_bwd: null pointer");
   MCB_REQUIRE(c % 8 == 0 && h % 2 == 0 && w % 2 == 0, "maxpool2_bwd: shape");
   const long total = (long)n * (h / 2) * (w / 2) * (c / 8);
-  launch_pdl(maxpool2_bwd_kernel, grid_for(total, 256), 256, 0, ST, (const uint4*)x, (const uint4*)dy, (uint4*)dx, accumulate,
-                                                            n, h, w, c / 8);
+  maxpool2_bwd_kernel<<<grid_for(total, 256), 256, 0, ST>>>(
+      (const uint4*)x, (const uint4*)dy, (uint4*)dx, accumulate, n, h, w, c / 8);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -1031,10 +1012,10 @@ extern "C" int mcb_maxpool2_bwd_skip_relu(const void* y, const void* dpool, void
   const int grid = (int)std::max(1L, std::min((pooled + lanes * 4 - 1) / (lanes * 4), (long)num_sms() * 4));
   MCB_REQUIRE((long)grid * c <= kChannelRedCap, "maxpool2_bwd_skip_relu: %d blocks x %d channels exceed the workspace",
               grid, c);
-  launch_pdl(maxpool2_bwd_skip_relu_kernel, grid, threads, (size_t)threads * 8 * sizeof(float), ST, (const uint4*)y,
-             (const uint4*)dpool, (uint4*)g, pooled, h, w, c8);
-  launch_pdl(channel_red_finish_kernel, det_finish_grid(c), kDetFinishThreads, 0, ST, 0L, grid, (long)c, (long)c,
-             (long)c, db, 0L);
+  maxpool2_bwd_skip_relu_kernel<<<grid, threads, (size_t)threads * 8 * sizeof(float), ST>>>(
+      (const uint4*)y, (const uint4*)dpool, (uint4*)g, pooled, h, w, c8);
+  channel_red_finish_kernel<<<det_finish_grid(c), kDetFinishThreads, 0, ST>>>(
+      0L, grid, (long)c, (long)c, (long)c, db, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -1044,7 +1025,7 @@ extern "C" int mcb_final_conv_fwd(const void* x, const float* w, const float* b,
   MCB_REQUIRE(x && w && b && logits, "final_conv_fwd: null pointer");
   MCB_REQUIRE(c % 8 == 0 && k >= 1 && k <= 4, "final_conv_fwd: c %d k %d", c, k);
   const long ppi = (long)h * wd, pixels = ppi * n;
-  launch_pdl(final_conv_fwd_kernel, grid_for(pixels, 256), 256, (size_t)(k * c + k) * sizeof(float), ST, 
+  final_conv_fwd_kernel<<<grid_for(pixels, 256), 256, (size_t)(k * c + k) * sizeof(float), ST>>>(
       (const uint4*)x, w, b, logits, ppi, pixels, c, k);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
@@ -1056,12 +1037,12 @@ extern "C" int mcb_final_conv_bwd(const void* x, const float* w, const float* dl
   const long ppi = (long)h * wd, pixels = ppi * n;
   const int grid = grid_for(pixels, 128, 4), n_acc = k * c + k;
   MCB_REQUIRE((long)grid * n_acc <= kFinalRedCap, "final_conv_bwd: %d blocks exceed the workspace", grid);
-  launch_pdl(final_conv_bwd_kernel, grid, 128, (size_t)(k * c + 4 * n_acc) * sizeof(float), ST, 
+  final_conv_bwd_kernel<<<grid, 128, (size_t)(k * c + 4 * n_acc) * sizeof(float), ST>>>(
       (const uint4*)x, w, dlogits, (uint4*)dx, dw, db, ppi, pixels, c, k);
-  launch_pdl(final_red_finish_kernel, det_finish_grid(k * c), kDetFinishThreads, 0, ST, 0L, grid, (long)n_acc,
-             (long)(k * c), (long)(k * c), dw, 0L);
-  launch_pdl(final_red_finish_kernel, det_finish_grid(k), kDetFinishThreads, 0, ST, (long)(k * c), grid, (long)n_acc,
-             (long)k, (long)k, db, 0L);
+  final_red_finish_kernel<<<det_finish_grid(k * c), kDetFinishThreads, 0, ST>>>(
+      0L, grid, (long)n_acc, (long)(k * c), (long)(k * c), dw, 0L);
+  final_red_finish_kernel<<<det_finish_grid(k), kDetFinishThreads, 0, ST>>>(
+      (long)(k * c), grid, (long)n_acc, (long)k, (long)k, db, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -1074,8 +1055,9 @@ extern "C" int mcb_adam_step(float* p, const float* g, float* m, float* v, void*
   // `1 - beta ** step` and `bias_correction2 ** 0.5`; mcb_adam_step_dyn's hyper carries the same values
   const double bc1 = 1.0 - pow(beta1, (double)step);
   const double bc2 = 1.0 - pow(beta2, (double)step);
-  launch_pdl(adam_kernel, grid_for(n, 256), 256, 0, ST, p, g, m, v, (bf16*)p_bf16, n, lr, (float)beta1, (float)beta2, eps,
-             weight_decay, (float)bc1, (float)pow(bc2, 0.5), grad_scale, (const float*)nullptr);
+  adam_kernel<<<grid_for(n, 256), 256, 0, ST>>>(
+      p, g, m, v, (bf16*)p_bf16, n, lr, (float)beta1, (float)beta2, eps, weight_decay, (float)bc1, (float)pow(bc2, 0.5),
+      grad_scale, (const float*)nullptr);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -1084,14 +1066,14 @@ extern "C" int mcb_adam_step_dyn(float* p, const float* g, float* m, float* v, v
                                  float grad_scale, void* stream) {
   MCB_REQUIRE(p && g && m && v && hyper, "adam_dyn: null pointer");
   if (n == 0) return MCB_OK;
-  launch_pdl(adam_kernel, grid_for(n, 256), 256, 0, ST, p, g, m, v, (bf16*)p_bf16, n, 0.f, beta1, beta2, eps,
-             weight_decay, 1.f, 1.f, grad_scale, hyper);
+  adam_kernel<<<grid_for(n, 256), 256, 0, ST>>>(
+      p, g, m, v, (bf16*)p_bf16, n, 0.f, beta1, beta2, eps, weight_decay, 1.f, 1.f, grad_scale, hyper);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
 extern "C" int mcb_cast_f32_bf16(const float* x, void* y, long n, void* stream) {
   MCB_REQUIRE(x && y, "cast: null pointer");
-  launch_pdl(cast_f32_bf16_kernel, grid_for(n, 256), 256, 0, ST, x, (bf16*)y, n);
+  cast_f32_bf16_kernel<<<grid_for(n, 256), 256, 0, ST>>>(x, (bf16*)y, n);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }

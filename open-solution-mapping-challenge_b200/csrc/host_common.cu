@@ -1,6 +1,5 @@
 // host_common.cu — error string, driver entry point lookup, tensor-map encoding.
 #include "host_common.h"
-#include <stdlib.h>
 #include <string.h>
 #include <mutex>
 
@@ -81,15 +80,6 @@ int encode_nhwc_view(CUtensorMap* out, const void* base, int N, int H, int W, in
   }
   uint32_t box[4] = {(uint32_t)box_c, (uint32_t)bw, (uint32_t)bh, (uint32_t)bn};
   return encode_tmap(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, b, dims, str, box, swizzle_bytes);
-}
-
-bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MCB_PDL");
-    v = (e && atoi(e) != 0) ? 1 : 0;  // opt-in: measured neutral-to-slower inside CUDA graphs (DESIGN.md)
-  }
-  return v == 1;
 }
 
 int num_sms() {

@@ -45,36 +45,4 @@ int encode_nhwc_view(CUtensorMap* out, const void* base, int N, int H, int W, in
 
 int num_sms();
 
-// ---- programmatic dependent launch (PDL) -------------------------------------------------------------------------
-// Every kernel of the train step is launched with programmatic stream serialization: the next kernel of the stream may
-// be scheduled (and run its prologue: barrier init, descriptor prefetch) while this one drains, and
-// blocks in griddepcontrol.wait until its predecessors have completed and flushed memory.  Each kernel executes
-// pdl_prologue() before its first global-memory access.  Opt-in with MCB_PDL=1: inside the CUDA-graph replay of the
-// train step it has not paid off, so the default launches without the attribute.
-bool pdl_enabled();
-
-template <typename... KArgs, typename... Args>
-static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                                     Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-
-#ifdef __CUDACC__
-// let the dependents be scheduled, then wait for the producers of this kernel's inputs
-__device__ __forceinline__ void pdl_prologue() {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-}
-#endif
-
 }  // namespace mcb

@@ -32,7 +32,6 @@ MCB_DET_WORKSPACE(double, g_loss_red, kLossRedCap, loss_red_finish_kernel)
 
 __global__ void loss_partials_kernel(const float* __restrict__ logits, const float* __restrict__ target, LossCfg cfg,
                                      double* __restrict__ sums, long ppi, long pixels, int tch) {
-  mcb::pdl_prologue();
   float aI = 0.f, aP = 0.f, aT = 0.f, aS = 0.f;
   for (long p = blockIdx.x * (long)blockDim.x + threadIdx.x; p < pixels; p += (long)gridDim.x * blockDim.x) {
     const long n = p / ppi, q = p % ppi;
@@ -71,7 +70,6 @@ __global__ void loss_grad_kernel(const float* __restrict__ logits, const float* 
                                  const double* __restrict__ sums, double global_pixels, float grad_scale,
                                  float* __restrict__ dlogits, float* __restrict__ loss_out, long ppi, long pixels,
                                  int tch) {
-  mcb::pdl_prologue();
   const double I = sums[0], P = sums[1], T = sums[2], S = sums[3];
   const double Dn = P + T + (double)cfg.smooth + (double)cfg.eps;
   const double num = 2.0 * I + (double)cfg.smooth;
@@ -109,7 +107,6 @@ __global__ void loss_grad_kernel(const float* __restrict__ logits, const float* 
 
 // numpy softmax over the class axis of NCHW logits (src/utils.py:231-273 as used at src/models.py:88-92)
 __global__ void softmax2_kernel(const float* __restrict__ logits, float* __restrict__ probs, long ppi, long pixels) {
-  mcb::pdl_prologue();
   for (long p = blockIdx.x * (long)blockDim.x + threadIdx.x; p < pixels; p += (long)gridDim.x * blockDim.x) {
     const long n = p / ppi, q = p % ppi;
     const float z0 = logits[(n * 2) * ppi + q], z1 = logits[(n * 2 + 1) * ppi + q];
@@ -147,10 +144,10 @@ extern "C" int mcb_loss_partials(const mcb_loss_args* a, double* sums, void* str
   const long ppi = (long)a->h * a->w, pixels = ppi * a->n;
   const int grid = loss_grid(pixels);
   MCB_REQUIRE((long)grid * 4 <= kLossRedCap, "loss_partials: %d blocks exceed the workspace", grid);
-  launch_pdl(loss_partials_kernel, grid, 256, 0, static_cast<cudaStream_t>(stream), 
+  loss_partials_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       a->logits, a->target, make_cfg(a), sums, ppi, pixels, a->mode == 0 ? 3 : 1);
-  launch_pdl(loss_red_finish_kernel, det_finish_grid(4), kDetFinishThreads, 0, static_cast<cudaStream_t>(stream), 0L,
-             grid, 4L, 4L, 4L, sums, 0L);
+  loss_red_finish_kernel<<<det_finish_grid(4), kDetFinishThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      0L, grid, 4L, 4L, 4L, sums, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
@@ -160,7 +157,7 @@ extern "C" int mcb_loss_grad(const mcb_loss_args* a, const double* sums, long gl
   MCB_REQUIRE(a && a->logits && a->target && sums && dlogits, "loss_grad: null pointer");
   MCB_REQUIRE(a->mode == 0 || a->mode == 1, "loss: mode %d", a->mode);
   const long ppi = (long)a->h * a->w, pixels = ppi * a->n;
-  launch_pdl(loss_grad_kernel, loss_grid(pixels), 256, 0, static_cast<cudaStream_t>(stream), 
+  loss_grad_kernel<<<loss_grid(pixels), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       a->logits, a->target, make_cfg(a), sums, (double)global_pixels, grad_scale, dlogits, loss_out, ppi, pixels,
       a->mode == 0 ? 3 : 1);
   MCB_LAUNCH_CHECK();
@@ -170,7 +167,7 @@ extern "C" int mcb_loss_grad(const mcb_loss_args* a, const double* sums, long gl
 extern "C" int mcb_softmax2(const float* logits, float* probs, int n, int h, int w, void* stream) {
   MCB_REQUIRE(logits && probs, "softmax2: null pointer");
   const long ppi = (long)h * w, pixels = ppi * n;
-  launch_pdl(softmax2_kernel, loss_grid(pixels), 256, 0, static_cast<cudaStream_t>(stream), logits, probs, ppi, pixels);
+  softmax2_kernel<<<loss_grid(pixels), 256, 0, static_cast<cudaStream_t>(stream)>>>(logits, probs, ppi, pixels);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }

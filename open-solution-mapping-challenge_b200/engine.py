@@ -38,31 +38,18 @@ def _nb(*tensors):
 _SIDE_KINDS = frozenset(("conv_wgrad", "convt_wgrad"))
 
 
-def stream_priority_enabled():
-    """MCB_STREAM_PRIORITY (default 1): the captured step's main chain runs on a HIGH-priority stream while the backward's
-    side stream (weight-gradient GEMMs, Adam segments, all-reduce launches) keeps the default low priority, so the block
-    scheduler serves the critical path (data-gradient GEMMs + BatchNorm-backward) first and the side work fills what is
-    left, together with launching every weight-gradient GEMM as soon as its operands exist (no deferral)."""
-    return os.environ.get("MCB_STREAM_PRIORITY", "1") == "1"
-
-
 def graph_capture(graph, dev):
-    """torch.cuda.graph context on the high-priority capture stream (see stream_priority_enabled)"""
-    if stream_priority_enabled():
-        return torch.cuda.graph(graph, stream=torch.cuda.Stream(device=dev, priority=-1))
-    return torch.cuda.graph(graph)
+    """torch.cuda.graph context on a HIGH-priority capture stream: the captured step's main chain runs at high priority
+    while the backward's side stream (weight-gradient GEMMs, Adam segments, all-reduce launches) keeps the default low
+    priority, so the block scheduler serves the critical path (data-gradient GEMMs + BatchNorm-backward) first and the
+    side work, forked as soon as its operands exist (Plan._run_bwd), fills what is left."""
+    return torch.cuda.graph(graph, stream=torch.cuda.Stream(device=dev, priority=-1))
 
 
 class _OpList(list):
     """list of _Op; .add(kind, fn, flops, bytes)"""
 
-    # profiling aid: MCB_KNOCKOUT="kind,kind" drops those launches from the plan so that the step-time
-    # difference gives their in-graph cost (results are garbage; never set outside profiling)
-    _knockout = frozenset(k for k in os.environ.get("MCB_KNOCKOUT", "").split(",") if k)
-
     def add(self, kind, fn, flops=0.0, nbytes=0.0, desc=""):
-        if kind in self._knockout:
-            return
         self.append(_Op(kind, fn, flops, nbytes, desc))
 
 
@@ -703,72 +690,43 @@ class Plan:
         for op in self.fwd_ops:
             op()
 
-    def _run_bwd(self, first=0, last=None, hooks=None):
-        """backward layers [first, last) in execution (reverse-forward) order; the gradient arena is zeroed with the
-        first layer.  hooks = {layer_index: fn}: fn() runs ON THE SIDE STREAM once every launch of the layers before
-        `layer_index` (main chain and weight-gradient GEMMs) is ordered before it -- used for per-segment optimizer
-        updates that overlap the rest of the backward pass."""
-        if first == 0:
-            L.zero(self.net._g32)
-            if self.sync_nvlink:
-                L.zero(self._dstats_loc)
-        # Weight/bias-gradient launches are leaves of the backward graph (they only add into the gradient arena): they
-        # go to a side stream, forked after their producer and joined at the end, so the tensor-core-bound wgrad GEMMs
-        # overlap the HBM-bound BatchNorm-backward kernels of the layers below instead of queueing behind them.
+    def _run_bwd(self, hooks=None):
+        """all backward layers in execution (reverse-forward) order, after zeroing the gradient arena.
+        hooks = {layer_index: fn}: fn() runs ON THE SIDE STREAM once every launch of the layers before `layer_index`
+        (main chain and weight-gradient GEMMs) is ordered before it -- used for per-segment optimizer updates and
+        all-reduces that overlap the rest of the backward pass."""
+        L.zero(self.net._g32)
+        if self.sync_nvlink:
+            L.zero(self._dstats_loc)
+        # Weight/bias-gradient launches are leaves of the backward graph (they only add into the gradient arena): each
+        # goes to the low-priority side stream, forked right after its producer and joined at the end, so the
+        # tensor-core-bound wgrad GEMMs overlap the HBM-bound BatchNorm-backward kernels of the layers below instead of
+        # queueing behind them, and the high-priority main chain (graph_capture) is served first.
         # (No buffer is recycled inside a step, so the only hazards are the recorded producer -> consumer edges.)
-        use_side = os.environ.get("MCB_SIDE_WGRAD", "1") == "1"
         main = torch.cuda.current_stream()
-        if use_side and self._side is None:
+        if self._side is None:
             self._side = torch.cuda.Stream(device=self.dev)
         forked = False
-        pending = []
-        # with prioritised streams the side work cannot delay the main chain, so it starts as early as possible;
-        # without them a weight-gradient GEMM is held back until the next data-gradient GEMM has been launched
-        defer = os.environ.get("MCB_SIDE_DEFER", "0" if stream_priority_enabled() else "1") == "1"
 
-        def flush():
+        def on_side(fn):
             nonlocal forked
-            if not pending:
-                return
             ev = torch.cuda.Event()
             ev.record(main)
             self._side.wait_event(ev)
             with torch.cuda.stream(self._side):
-                for q in pending:
-                    q()
-            pending.clear()
+                fn()
             forked = True
 
-        def run_hook(idx):
-            nonlocal forked
-            if hooks and idx in hooks:
-                if not use_side:
-                    hooks[idx]()
-                    return
-                flush()
-                ev = torch.cuda.Event()
-                ev.record(main)
-                self._side.wait_event(ev)
-                with torch.cuda.stream(self._side):
-                    hooks[idx]()
-                forked = True
-
-        n_layers = len(self.bwd_layers) if last is None else last
-        for li, layer in enumerate(self.bwd_layers[first:last], start=first):
-            run_hook(li)
+        for li, layer in enumerate(self.bwd_layers):
+            if hooks and li in hooks:
+                on_side(hooks[li])
             for op in layer:
-                if use_side and op.kind in _SIDE_KINDS and op.desc:
-                    pending.append(op)
-                    if not defer:
-                        flush()
+                if op.kind in _SIDE_KINDS and op.desc:
+                    on_side(op)
                 else:
                     op()
-                    # a deferred wgrad starts right AFTER the next data-gradient GEMM (which needs whole SMs), i.e.
-                    # next to the BatchNorm-backward kernels that follow it
-                    if op.kind in ("conv_dgrad", "convt_dgrad"):
-                        flush()
-        flush()
-        run_hook(n_layers)
+        if hooks and len(self.bwd_layers) in hooks:
+            on_side(hooks[len(self.bwd_layers)])
         if forked:
             ev = torch.cuda.Event()
             ev.record(self._side)
@@ -793,11 +751,8 @@ class Plan:
         o_l3 = off["encoder.layer3.0.conv1.weight"]
         return [(0, i_dec, o_dec, total), (i_dec, i_l4, o_l4, o_dec), (i_l4, i_l3, o_l3, o_l4), (i_l3, n, 0, o_l3)]
 
-    def forward(self, x, use_graph=True):
+    def forward(self, x):
         self.x_in.copy_(x)
-        if not use_graph:
-            self._run_fwd()
-            return self.logits
         if self.graph_fwd is None:
             self._run_fwd()  # eager warm-up (sets kernel attributes, validates arguments)
             torch.cuda.synchronize()
@@ -809,11 +764,8 @@ class Plan:
         self.graph_fwd.replay()
         return self.logits
 
-    def backward(self, dlogits, use_graph=True):
+    def backward(self, dlogits):
         self.dlogits.copy_(dlogits)
-        if not use_graph:
-            self._run_bwd()
-            return
         if self.graph_bwd is None:
             self._run_bwd()
             torch.cuda.synchronize()

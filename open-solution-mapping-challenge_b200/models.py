@@ -444,27 +444,17 @@ class FusedTrainStep:
         self.graphs = None
         self.pixels = n * h * w
         net.refresh_operands()
-        self.use_graphs = os.environ.get("MCB_NO_GRAPH", "0") != "1"
         self.launches = None
         self._staging = None
-        self.segments = None
-        # opt-in: on 2 GPUs the three smaller all-reduces + graph segmentation can cost more than they hide; kept for
-        # larger worlds / slower fabrics
-        if self.world > 1 and os.environ.get("MCB_OVERLAP_ALLREDUCE", "2") == "1" and not self.plan.sync_bn:
-            self.segments = self.plan.bwd_segments()
-            self._comm_stream = torch.cuda.Stream(device=dev)
         # single GPU: the Adam update of a finished arena segment (decoder | layer4 | rest) rides on the backward's side
         # stream, inside the graph, overlapping the data-gradient GEMMs of the layers below (HBM-bound next to
         # tensor-bound).  Its step-dependent scalars live in a 3-float device tensor refreshed before every replay.
-        # multi-GPU default: the all-reduce of a finished arena segment (decoder | layer4 | layer3 | rest) is issued from
+        # multi-GPU: the all-reduce of a finished arena segment (decoder | layer4 | layer3 | rest) is issued from
         # INSIDE the backward graph, on the side stream behind that segment's weight-gradient GEMMs, and overlaps the
-        # data-gradient chain of the layers below.
-        # MCB_OVERLAP_ALLREDUCE=0 restores the single all-reduce after the backward graph; NCCL-per-BatchNorm SyncBN
-        # (MCB_SYNC_BN=1) needs it because its BatchNorm slots are rescaled after the backward pass.
-        ov = os.environ.get("MCB_OVERLAP_ALLREDUCE", "2")
-        self.inline_allreduce = (self.world > 1 and ov == "2" and self.segments is None
-                                 and not (self.plan.sync_bn and not self.plan.sync_nvlink))
-        self.adam_in_graph = self.world == 1 and os.environ.get("MCB_ADAM_SIDE", "1") == "1"
+        # data-gradient chain of the layers below.  NCCL-per-BatchNorm SyncBN (MCB_SYNC_BN=1) instead takes a single
+        # all-reduce after the backward graph, because its BatchNorm slots are rescaled after the backward pass.
+        self.inline_allreduce = self.world > 1 and not (self.plan.sync_bn and not self.plan.sync_nvlink)
+        self.adam_in_graph = self.world == 1
         self._hyper = torch.zeros(3, dtype=torch.float32, device=dev)
         # pinned staging ring: a slot is rewritten only after the copy that last read it has executed
         self._hyper_ring = [(torch.zeros(3, dtype=torch.float32).pin_memory(), torch.cuda.Event()) for _ in range(8)]
@@ -480,52 +470,41 @@ class FusedTrainStep:
         L.zero(self.sums)
         ops.loss_partials(self.plan.logits, self.target, self.sums, mode=self.loss_mode, **self.loss_cfg)
 
-    def _seg_backward(self, seg=None):
-        """seg None: whole backward; else one of plan.bwd_segments() (multi-GPU: the gradient all-reduce of a finished
-        segment overlaps the next segment's kernels)"""
-        if seg is None or seg[0] == 0:
-            ops.loss_grad(self.plan.logits, self.target, self.sums, self.plan.dlogits, self.loss,
-                          global_pixels=self.pixels * self.world, mode=self.loss_mode, **self.loss_cfg)
-        if seg is None:
-            hooks = None
-            if self.adam_in_graph:
-                net = self.net
-                betas, eps, wd = self._adam_cfg
+    def _seg_backward(self):
+        ops.loss_grad(self.plan.logits, self.target, self.sums, self.plan.dlogits, self.loss,
+                      global_pixels=self.pixels * self.world, mode=self.loss_mode, **self.loss_cfg)
+        hooks = None
+        if self.adam_in_graph:
+            net = self.net
+            betas, eps, wd = self._adam_cfg
 
-                def upd(lo, hi):
-                    return lambda: ops.adam_step_dyn(net._p32[lo:hi], net._g32[lo:hi], self.opt.m[lo:hi], self.opt.v[lo:hi],
-                                                     net._w16[lo:hi], self._hyper, betas, eps, wd, 1.0)
-                hooks = {last: upd(lo, hi) for _, last, lo, hi in self.plan.bwd_segments()}
-            works = []
-            if self.inline_allreduce:
-                # MCB_OVERLAP_ALLREDUCE=2 (experimental, not yet run on hardware): the all-reduce of a finished arena
-                # segment is issued from INSIDE the single backward graph, on the side stream behind that segment's
-                # weight-gradient GEMMs, and overlaps the data-gradient chain of the layers below; the main stream joins
-                # the collectives at the end of the graph
-                g32 = self.net._g32
-                hooks = {last: (lambda lo=lo, hi=hi: works.append(dist.all_reduce(g32[lo:hi], async_op=True)))
-                         for _, last, lo, hi in self.plan.bwd_segments()}
-            self.plan._run_bwd(hooks=hooks)
-            for wk in works:
-                wk.wait()
-        else:
-            self.plan._run_bwd(seg[0], seg[1])
+            def upd(lo, hi):
+                return lambda: ops.adam_step_dyn(net._p32[lo:hi], net._g32[lo:hi], self.opt.m[lo:hi], self.opt.v[lo:hi],
+                                                 net._w16[lo:hi], self._hyper, betas, eps, wd, 1.0)
+            hooks = {last: upd(lo, hi) for _, last, lo, hi in self.plan.bwd_segments()}
+        works = []
+        if self.inline_allreduce:
+            # the all-reduce of a finished arena segment is issued from INSIDE the single backward graph, on the side
+            # stream behind that segment's weight-gradient GEMMs, and overlaps the data-gradient chain of the layers
+            # below; the main stream joins the collectives at the end of the graph.  (Multi-GPU runs have not been
+            # measured on the H100.)
+            g32 = self.net._g32
+            hooks = {last: (lambda lo=lo, hi=hi: works.append(dist.all_reduce(g32[lo:hi], async_op=True)))
+                     for _, last, lo, hi in self.plan.bwd_segments()}
+        self.plan._run_bwd(hooks=hooks)
+        for wk in works:
+            wk.wait()
 
     def _adam(self, lr, betas, eps, weight_decay):
         net = self.net
         ops.adam_step(net._p32, net._g32, self.opt.m, self.opt.v, net._w16, self.opt.t, lr, betas, eps, weight_decay, 1.0)
 
     def _capture(self):
-        segs = [self._seg_forward]
-        if self.segments is None:
-            segs.append(self._seg_backward)
-        else:
-            segs += [(lambda sg=sg: self._seg_backward(sg)) for sg in self.segments]
         gs = []
         from .engine import graph_capture
-        for seg in segs:
+        for seg in (self._seg_forward, self._seg_backward):
             g = torch.cuda.CUDAGraph()
-            with graph_capture(g, self.dev):      # main chain on a high-priority stream (engine.stream_priority_enabled)
+            with graph_capture(g, self.dev):      # main chain on a high-priority stream
                 seg()
             gs.append(g)
         self.graphs = gs
@@ -578,7 +557,7 @@ class FusedTrainStep:
             host[0], host[1], host[2] = ops.adam_hyper(lr, betas, t)
             self._hyper.copy_(host, non_blocking=True)
             ev.record()
-        first = self.graphs is None and self.use_graphs
+        first = self.graphs is None
         marks = self.phase_marks            # bench.py: CUDA events at the phase boundaries of a step (None = off)
 
         def mark(name):
@@ -587,7 +566,7 @@ class FusedTrainStep:
                 e.record()
                 marks.append((name, e))
         mark("start")
-        if first or not self.use_graphs:
+        if first:
             self._seg_forward()
         else:
             self.graphs[0].replay()
@@ -597,38 +576,16 @@ class FusedTrainStep:
         if self.world > 1:
             dist.all_reduce(self.sums)
         mark("loss sums")
-        eager = first or not self.use_graphs
-        if self.segments is None:
-            if eager:
-                self._seg_backward()
-            else:
-                self.graphs[1].replay()
-            if self.world > 1 and not self.inline_allreduce:
-                if self.plan.sync_bn and not self.plan.sync_nvlink:
-                    # the BatchNorm slots already hold GLOBAL sums (engine.Plan.sync_bn_grads): pre-divide so that the
-                    # arena-wide SUM below leaves them unchanged
-                    torch._foreach_mul_(self.plan.bn_grad_slices(), 1.0 / self.world)
-                dist.all_reduce(self.net._g32)   # gradients of the global-batch loss = sum of the per-rank contributions
+        if first:
+            self._seg_backward()
         else:
-            # bucketed gradient all-reduce: segment k's arena range is reduced on the NCCL stream while segment k+1 runs
-            main = torch.cuda.current_stream()
-            works = []
-            for k, sg in enumerate(self.segments):
-                if eager:
-                    self._seg_backward(sg)
-                else:
-                    self.graphs[1 + k].replay()
-                grad_slice = self.net._g32[sg[2]:sg[3]]
-                if k + 1 < len(self.segments):
-                    ev = torch.cuda.Event()
-                    ev.record(main)
-                    with torch.cuda.stream(self._comm_stream):
-                        self._comm_stream.wait_event(ev)
-                        works.append(dist.all_reduce(grad_slice, async_op=True))
-                else:
-                    works.append(dist.all_reduce(grad_slice, async_op=True))
-            for wk in works:
-                wk.wait()
+            self.graphs[1].replay()
+        if self.world > 1 and not self.inline_allreduce:
+            if self.plan.sync_bn and not self.plan.sync_nvlink:
+                # the BatchNorm slots already hold GLOBAL sums (engine.Plan.sync_bn_grads): pre-divide so that the
+                # arena-wide SUM below leaves them unchanged
+                torch._foreach_mul_(self.plan.bn_grad_slices(), 1.0 / self.world)
+            dist.all_reduce(self.net._g32)   # gradients of the global-batch loss = sum of the per-rank contributions
         mark("backward (+ in-graph Adam / all-reduce)")
         if not self.adam_in_graph:
             self._adam(lr, betas, eps, weight_decay)

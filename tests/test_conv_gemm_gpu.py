@@ -96,25 +96,15 @@ def test_conv_fwd_integer_exact(mcb, cuda):
 @pytest.mark.parametrize("n,h,w,cin,cout", [(2, 32, 16, 64, 128), (1, 32, 24, 128, 64), (1, 16, 16, 32, 32),
                                              (2, 20, 20, 64, 64)])
 def test_conv3x3_haloed_tile_path(mcb, cuda, monkeypatch, n, h, w, cin, cout):
-    _haloed_tile_checks(cuda, monkeypatch, n, h, w, cin, cout, resident=False)
+    _haloed_tile_checks(cuda, monkeypatch, n, h, w, cin, cout)
 
 
-# (MCB_BRES, resident per-tap weights in the haloed path: an opt-in switch, off by default -- the tests keep it from
-# rotting)
-@pytest.mark.parametrize("n,h,w,cin,cout", [(2, 32, 16, 64, 64), (1, 32, 24, 32, 32), (3, 16, 16, 32, 32),
-                                             (2, 48, 40, 64, 128)])
-def test_conv3x3_haloed_tile_resident_weights(mcb, cuda, monkeypatch, n, h, w, cin, cout):
-    _haloed_tile_checks(cuda, monkeypatch, n, h, w, cin, cout, resident=True)
-
-
-def _haloed_tile_checks(cuda, monkeypatch, n, h, w, cin, cout, resident):
+def _haloed_tile_checks(cuda, monkeypatch, n, h, w, cin, cout):
     """MCB_HALO=1 forces the haloed-tile 3x3 path (one TMA box per channel chunk serves the nine taps through
     row-shifted wgmma descriptors; default rule: >= 128 channels on large images): forward (+stats, integer-exact),
     plain / masked data gradient, against the same references as the per-tap path"""
     from mcb200 import ops
     monkeypatch.setenv("MCB_HALO", "1")
-    if resident:
-        monkeypatch.setenv("MCB_BRES", "1")
     g = torch.Generator().manual_seed(11 + h + cin)
     x = torch.randint(-1, 2, (n, cin, h, w), generator=g).float()
     wt = (torch.rand(cout, cin, 3, 3, generator=g) < 0.1).float() * torch.randint(-1, 2, (cout, cin, 3, 3), generator=g)

@@ -107,11 +107,6 @@ def test_gradient_buffers_first_store_then_accumulate(mcb):
     assert kinds["bn_bwd_reduce"] == n_bn - n_blocks
 
 
-def test_knockout_switch_is_off_by_default():
-    from mcb200.engine import _OpList
-    assert _OpList._knockout == frozenset()
-
-
 def test_four_backward_segments_for_the_overlapped_all_reduce(net101, plan101):
     """decoder | layer4 | layer3 | layer2 + layer1 + stem: layer3's 23 blocks (the largest parameter group after the
     decoder) reduce while the shallow layers still run"""
@@ -122,11 +117,3 @@ def test_four_backward_segments_for_the_overlapped_all_reduce(net101, plan101):
     assert set(tags[segs[2][0]:segs[2][1]]) == {"layer3"} and set(tags[segs[3][0]:segs[3][1]]) == {"layer2", "layer1", "stem"}
     sizes = [s[3] - s[2] for s in segs]
     assert sizes[2] > sizes[3] and sizes[0] > sizes[3]      # the exposed last segment is the smallest
-
-
-def test_stream_priority_defaults(monkeypatch):
-    from mcb200 import engine
-    monkeypatch.delenv("MCB_STREAM_PRIORITY", raising=False)
-    assert engine.stream_priority_enabled()
-    monkeypatch.setenv("MCB_STREAM_PRIORITY", "0")
-    assert not engine.stream_priority_enabled()
