@@ -37,6 +37,12 @@ constexpr int CRF_THREADS = CRF_T * (CRF_T / CRF_ROWS);   // 256
 // 73 KB per CTA -> three CTAs per SM within the 227 KB of shared memory an SM offers
 constexpr size_t CRF_SMEM = (size_t)CRF_S * CRF_S * (sizeof(float4) + sizeof(float2) + sizeof(float2)) +
                             (size_t)CRF_S * CRF_T * sizeof(float2);
+// The window drops every tap beyond R.  The heaviest dropped tap, at distance R + 1 along an axis, weighs
+// exp(-(R+1)^2 / (2 sxy^2)); it must stay <= 1e-7, i.e. sxy <= 7 / sqrt(2 ln 1e7) = 1.2329.  Mean-field iterations
+// amplify the truncation: on noise images at the default compatibilities and 5 iterations the output moves by up to
+// ~400x the dropped tap's weight, so at the bound the result stays within ~4e-5 of a full-window filter (1.3 already
+// gives 1.7e-4).  Wider kernels are refused instead of silently truncated.
+constexpr double CRF_MAX_DROPPED_TAP = 1e-7;
 
 __constant__ float c_g1g[CRF_D];    // 1-D spatial weights exp(-d^2 / (2 sxy^2)), Gaussian kernel
 __constant__ float c_g1b[CRF_D];    // ... bilateral kernel
@@ -237,6 +243,12 @@ extern "C" int mcb_dense_crf(const float* probs, const uint8_t* rgb, float* out,
   MCB_REQUIRE(probs && rgb && out && workspace, "dense_crf: null pointer");
   MCB_REQUIRE(iterations >= 1, "dense_crf: iterations %d", iterations);
   MCB_REQUIRE(sxy_gaussian > 0.f && sxy_bilateral > 0.f && srgb > 0.f, "dense_crf: kernel widths must be positive");
+  for (const float sxy : {sxy_gaussian, sxy_bilateral}) {
+    const double dropped = exp(-0.5 * (double)((CRF_R + 1) * (CRF_R + 1)) / ((double)sxy * sxy));
+    if (dropped > CRF_MAX_DROPPED_TAP)
+      return fail(MCB_ERR_UNSUPPORTED, "dense_crf: sxy %g is too wide for the %dx%d window (largest sxy: %.4f)",
+                  (double)sxy, CRF_D, CRF_D, (CRF_R + 1) / sqrt(2.0 * log(1.0 / CRF_MAX_DROPPED_TAP)));
+  }
   float g1g[CRF_D], g1b[CRF_D], e1b[CRF_D];
   const double log2e = 1.4426950408889634;
   for (int d = -CRF_R; d <= CRF_R; ++d) {

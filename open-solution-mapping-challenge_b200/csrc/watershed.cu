@@ -14,7 +14,9 @@
 namespace mcb {
 
 constexpr int WS_T = 32;
-constexpr int WS_INF = 0x3fffffff;
+constexpr int WS_INF = 0x3fffffff;          // cost / dist: unreached
+constexpr unsigned WS_NO_LABEL = 0xffffffffu; // label stage: unreached.  Labels are compared as unsigned, so every
+                                              // positive int32 marker label (up to 2^31 - 1) sorts below it
 constexpr int WS_MAX_TILES = 1024;   // tile-activity table in shared memory (larger planes sweep every tile)
 
 template <int STAGE>
@@ -26,6 +28,9 @@ __device__ void ws_stage(const int* __restrict__ lev, int* __restrict__ cost, in
   __shared__ int s_dist[WS_T + 2][WS_T + 2];  // stage 3
   __shared__ int s_flag;
   int* var = STAGE == 1 ? cost : (STAGE == 2 ? dist : lab);
+  const int var_inf = STAGE == 3 ? (int)WS_NO_LABEL : WS_INF;
+  // stages 1-2 relax signed costs / distances, stage 3 relaxes labels as unsigned values (see WS_NO_LABEL)
+  auto less = [](int a, int b) { return STAGE == 3 ? (unsigned)a < (unsigned)b : a < b; };
   const int tx = threadIdx.x % WS_T, ty = threadIdx.x / WS_T;
   const int tiles_x = (W + WS_T - 1) / WS_T, tiles_y = (H + WS_T - 1) / WS_T;
   const int ntiles = tiles_x * tiles_y;
@@ -41,7 +46,7 @@ __device__ void ws_stage(const int* __restrict__ lev, int* __restrict__ cost, in
         const int y = y0 + sy - 1, x = x0 + sx - 1;
         const bool in = (y >= 0 && y < H && x >= 0 && x < W);
         const long p = (long)y * W + x;
-        s_var[sy][sx] = in ? var[p] : WS_INF;
+        s_var[sy][sx] = in ? var[p] : var_inf;
         if (STAGE >= 2) s_cost[sy][sx] = in ? cost[p] : WS_INF;
         if (STAGE == 3) s_dist[sy][sx] = in ? dist[p] : WS_INF;
       }
@@ -74,12 +79,12 @@ __device__ void ws_stage(const int* __restrict__ lev, int* __restrict__ cost, in
               if (STAGE == 2) {
                 if (tight) nv = min(nv, s_var[ny[k]][nx[k]] + (s_var[ny[k]][nx[k]] < WS_INF ? 1 : 0));
               } else {
-                if (tight && s_dist[ny[k]][nx[k]] + 1 == my_dist) nv = min(nv, s_var[ny[k]][nx[k]]);
+                if (tight && s_dist[ny[k]][nx[k]] + 1 == my_dist && less(s_var[ny[k]][nx[k]], nv)) nv = s_var[ny[k]][nx[k]];
               }
             }
           }
         }
-        const bool ch = active && nv < s_var[ty + 1][tx + 1];
+        const bool ch = active && less(nv, s_var[ty + 1][tx + 1]);
         const int any = __syncthreads_or(ch ? 1 : 0);
         if (ch) s_var[ty + 1][tx + 1] = nv;
         if (!any) break;
@@ -119,7 +124,7 @@ __global__ void __launch_bounds__(WS_T* WS_T) watershed_kernel(const T* __restri
     lev[i] = l;
     cost[i] = m > 0 ? 0 : WS_INF;
     dist[i] = m > 0 ? 0 : WS_INF;
-    lab[i] = m > 0 ? m : WS_INF;
+    lab[i] = m > 0 ? m : (int)WS_NO_LABEL;
   }
   __syncthreads();
   // tiles without a single mask / marker pixel never hold an active pixel in any stage: mark them once, skip them in
@@ -145,7 +150,7 @@ __global__ void __launch_bounds__(WS_T* WS_T) watershed_kernel(const T* __restri
   ws_stage<3>(lev, cost, dist, lab, mk, ms, H, W, tile_on);
   __syncthreads();
   for (long i = threadIdx.x; i < hw; i += blockDim.x)
-    if (lab[i] >= WS_INF) lab[i] = 0;
+    if (lab[i] == (int)WS_NO_LABEL) lab[i] = 0;
 }
 
 }  // namespace mcb
