@@ -244,6 +244,9 @@ typedef struct {
   float w0, sigma;     /* neptune.yaml:55-56 */
   float size_c;        /* C = sqrt(image_h*image_w)/2 from the CONFIGURED size (src/models.py:373-381) */
   float dice_weight, ce_weight, dice_smooth;
+  int dice_activation; /* mode 0's Dice probability of class 1 (src/models.py:438-443): 0 softmax, 1 sigmoid(z1); any
+                          other value is rejected.  Mode 1 ignores it.  It is the last field so that a zeroed struct
+                          keeps meaning the softmax Dice */
 } mcb_loss_args;
 int mcb_loss_partials(const mcb_loss_args* a, double* sums, void* stream);
 int mcb_loss_grad(const mcb_loss_args* a, const double* sums, long global_pixels, float grad_scale, float* dlogits,

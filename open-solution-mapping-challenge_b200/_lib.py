@@ -76,7 +76,7 @@ def call(name, args=None, *extra):
 class LossArgs(C.Structure):
     _fields_ = [("logits", vp), ("target", vp), ("n", ci), ("h", ci), ("w", ci), ("mode", ci), ("w0", C.c_float),
                 ("sigma", C.c_float), ("size_c", C.c_float), ("dice_weight", C.c_float), ("ce_weight", C.c_float),
-                ("dice_smooth", C.c_float)]
+                ("dice_smooth", C.c_float), ("dice_activation", ci)]
 
 
 cl, cf = C.c_long, C.c_float

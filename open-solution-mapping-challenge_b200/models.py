@@ -88,12 +88,12 @@ def multiclass_segmentation_loss(output, target):
 def mixed_dice_cross_entropy_loss(output, target, dice_weight=0.5, dice_loss=None, cross_entropy_weight=0.5,
                                   cross_entropy_loss=None, smooth=0, dice_activation='softmax', w0=50.0, sigma=10.0,
                                   imsize=(256, 256)):
-    """src/models.py:384-418 in the configuration PyTorchUNetWeighted builds (src/models.py:149-161): softmax Dice on
-    class 1 + distance/size-weighted cross entropy; target (N,3,H,W) = [mask, distances, sizes]"""
-    if dice_activation != 'softmax':
-        raise NotImplementedError('only the configured softmax Dice is implemented')
+    """src/models.py:384-418 in the configuration PyTorchUNetWeighted builds (src/models.py:149-161): Dice on class 1
+    (of the softmax, or of the sigmoid of the class-1 logit) + distance/size-weighted cross entropy; target (N,3,H,W) =
+    [mask, distances, sizes]"""
+    ops.dice_activation_code(dice_activation)
     cfg = dict(w0=w0, sigma=sigma, size_c=_size_c(imsize), dice_weight=dice_weight, ce_weight=cross_entropy_weight,
-               dice_smooth=smooth)
+               dice_smooth=smooth, dice_activation=dice_activation)
     return _FusedLoss.apply(output, target, 0, cfg)
 
 
@@ -354,17 +354,21 @@ class PyTorchUNetWeighted(BasePyTorchUNet):
     """src/models.py:149-161"""
 
     def __init__(self, architecture_config, training_config, callbacks_config, callbacks=None):
+        dice = architecture_config['dice']
+        activation = dice.get('dice_activation', 'softmax')
+        # checked here, not at the first loss call as in the reference: the fused train step and the autograd loss must
+        # both compute the configured Dice, so no step may run on a config neither implements
+        ops.dice_activation_code(activation)
         super().__init__(architecture_config, training_config, callbacks_config, callbacks)
         wce = architecture_config['weighted_cross_entropy']
-        dice = architecture_config['dice']
         lw = architecture_config['loss_weights']
         loss = partial(mixed_dice_cross_entropy_loss, dice_weight=lw['dice_mask'], cross_entropy_weight=lw['bce_mask'],
-                       smooth=dice['smooth'], dice_activation=dice.get('dice_activation', 'softmax'), w0=wce['w0'],
-                       sigma=wce['sigma'], imsize=tuple(wce['imsize']))
+                       smooth=dice['smooth'], dice_activation=activation, w0=wce['w0'], sigma=wce['sigma'],
+                       imsize=tuple(wce['imsize']))
         self.loss_function = [('multichannel_map', loss, 1.0)]
         self._fused_loss = (0, dict(w0=float(wce['w0']), sigma=float(wce['sigma']), size_c=_size_c(wce['imsize']),
                                     dice_weight=float(lw['dice_mask']), ce_weight=float(lw['bce_mask']),
-                                    dice_smooth=float(dice['smooth'])))
+                                    dice_smooth=float(dice['smooth']), dice_activation=activation))
 
 
 class _StreamMixin:

@@ -347,6 +347,17 @@ def cast_bf16(x, out):
     return out
 
 
+DICE_ACTIVATIONS = ("softmax", "sigmoid")   # mcb_loss_args.dice_activation 0, 1
+
+
+def dice_activation_code(name):
+    """the mcb_loss_args.dice_activation of an activation name; the reference's error for any other
+    (src/models.py:438-443)"""
+    if name not in DICE_ACTIVATIONS:
+        raise NotImplementedError('only sigmoid and softmax are implemented')
+    return DICE_ACTIVATIONS.index(name)
+
+
 def _loss_args(logits, target, mode, cfg):
     a = L.LossArgs()
     n, k, h, w = logits.shape
@@ -357,6 +368,7 @@ def _loss_args(logits, target, mode, cfg):
     a.w0 = cfg.get("w0", 50.0); a.sigma = cfg.get("sigma", 10.0); a.size_c = cfg.get("size_c", 128.0)
     a.dice_weight = cfg.get("dice_weight", 0.2); a.ce_weight = cfg.get("ce_weight", 1.0)
     a.dice_smooth = cfg.get("dice_smooth", 1.0)
+    a.dice_activation = dice_activation_code(cfg.get("dice_activation", "softmax"))
     return a
 
 
