@@ -1,5 +1,5 @@
-"""Static launch plans for the U-Nets of unet_models (UNetResNet / AlbuNet, and the BatchNorm-free VGG plan of UNet11 /
-UNetVGG16, see Plan._build_vgg): every kernel launch of one forward (and its backward) over preallocated
+"""Static launch plans for the U-Nets of unet_models (UNetResNet / AlbuNet through ResNetPlan, and the BatchNorm-free
+UNet11 / UNetVGG16 through VGGPlan): every kernel launch of one forward (and its backward) over preallocated
 NHWC bf16 buffers, replayable as CUDA graphs.
 
 Data flow per conv+BN unit in training:  z = conv(a_prev) [+ per-channel sum / sumsq in the GEMM epilogue]
@@ -19,13 +19,20 @@ from . import ops
 BF16 = torch.bfloat16
 F32 = torch.float32
 
+# the only launch kinds a builder may mark `side`: weight-gradient GEMMs, which only add into the gradient arena
+_SIDE_KINDS = frozenset(("conv_wgrad", "convt_wgrad"))
+
 
 class _Op:
-    """one launch (or a tiny group) with its algorithmic cost, for the per-kernel breakdown in bench.py"""
-    __slots__ = ("kind", "fn", "flops", "bytes", "desc")
+    """one launch (or a tiny group) with its algorithmic cost, for the per-kernel breakdown in bench.py.  `side`: a
+    weight-gradient launch that Plan._run_bwd forks onto the side stream (nothing later in the step reads its output)"""
+    __slots__ = ("kind", "fn", "flops", "bytes", "desc", "side")
 
-    def __init__(self, kind, fn, flops=0.0, nbytes=0.0, desc=""):
+    def __init__(self, kind, fn, flops=0.0, nbytes=0.0, desc="", side=False):
+        if side and kind not in _SIDE_KINDS:
+            raise RuntimeError("plan error: a %s launch cannot run on the side stream" % kind)
         self.kind, self.fn, self.flops, self.bytes, self.desc = kind, fn, float(flops), float(nbytes), desc
+        self.side = side
 
     def __call__(self):
         return self.fn()
@@ -35,7 +42,9 @@ def _nb(*tensors):
     return float(sum(t.numel() * t.element_size() for t in tensors if t is not None))
 
 
-_SIDE_KINDS = frozenset(("conv_wgrad", "convt_wgrad"))
+def _conv_desc(x, cout, k, s):
+    """breakdown label of a k x k / stride s conv over x"""
+    return "%d->%d k%d s%d @%dx%dx%d" % ((x.shape[3], cout, k, s) + tuple(x.shape[:3]))
 
 
 def graph_capture(graph, dev):
@@ -47,10 +56,10 @@ def graph_capture(graph, dev):
 
 
 class _OpList(list):
-    """list of _Op; .add(kind, fn, flops, bytes)"""
+    """list of _Op; .add(kind, fn, flops, bytes, desc, side)"""
 
-    def add(self, kind, fn, flops=0.0, nbytes=0.0, desc=""):
-        self.append(_Op(kind, fn, flops, nbytes, desc))
+    def add(self, kind, fn, flops=0.0, nbytes=0.0, desc="", side=False):
+        self.append(_Op(kind, fn, flops, nbytes, desc, side))
 
 
 class _BN:
@@ -60,6 +69,10 @@ class _BN:
 
 
 class Plan:
+    """What every launch plan shares: activation and gradient buffers, the BatchNorm units, the decoder blocks and the
+    classifier tail, backward registration, the arena segments and execution.  A subclass per encoder family builds
+    the network in _build() and names its three segment boundaries in _segment_bounds()."""
+
     def __init__(self, net, n, h, w, training):
         self.net, self.n, self.h, self.w, self.training = net, n, h, w, training
         self.dev = net._p32.device
@@ -69,7 +82,7 @@ class Plan:
         self.written = set()       # gradient buffers that already hold a contribution
         self._keep = []            # keeps tensors referenced by closures alive
         self._bns = []
-        self._bwd_builders = []    # one per forward unit; run in REVERSE so store/accumulate modes follow run order
+        self._bwd_builders = []    # (tag, builder) per forward unit; run in REVERSE so store/accumulate modes follow run order
         self.units = []            # (kind, state_dict prefix, inputs, output) per forward unit, for per-unit parity tests
         total_c = sum(m.num_features for m in net.modules() if isinstance(m, nn.BatchNorm2d))
         n_bn = sum(1 for m in net.modules() if isinstance(m, nn.BatchNorm2d))
@@ -127,6 +140,20 @@ class Plan:
             self.bwd_tags.append(tag)
         self.launches_fwd = len(self.fwd_ops)
         self.launches_bwd = sum(len(l) for l in self.bwd_layers)
+        # inference folds every BatchNorm into a per-channel affine: one launch refreshes all of them from the running
+        # statistics, over rows [gamma, beta, running_mean, running_var, scale, shift, C]
+        self._bn_tab = None
+        if self._bns and not training:
+            rows = [[b.gamma.data_ptr(), b.beta.data_ptr(), b.mod.running_mean.data_ptr(), b.mod.running_var.data_ptr(),
+                     b.scale.data_ptr(), b.shift.data_ptr(), b.c] for b in self._bns]
+            self._bn_tab = torch.tensor(rows, dtype=torch.int64, device=self.dev)
+
+    def _build(self):
+        raise NotImplementedError
+
+    def _segment_bounds(self):
+        """the family's three backward segment boundaries, deepest-first: [(bwd tag, first arena parameter)]"""
+        raise NotImplementedError
 
     # ------------------------------------------------------------------------------------------ helpers
     def act(self, n, h, w, c):
@@ -147,6 +174,12 @@ class Plan:
         acc = id(a) in self.written
         self.written.add(id(a))
         return acc
+
+    def on_backward(self, tag, builder):
+        """register builder(B), which appends one forward unit's backward launches to B; `tag` names the unit's group
+        for bwd_segments.  Inference plans have no backward."""
+        if self.training:
+            self._bwd_builders.append((tag, builder))
 
     def bn_state(self, mod):
         net = self.net
@@ -189,7 +222,7 @@ class Plan:
         w16 = net._packed(conv.weight, net._w16)
         F = self.fwd_ops
         cflops = 2.0 * z.numel() * cin * k * k
-        desc = "%d->%d k%d s%d @%dx%dx%d" % (cin, cout, k, s, n, h, w)
+        desc = _conv_desc(x, cout, k, s)
         if self.training:
             F.add("conv_fwd", lambda: ops.conv_fwd(x, w16, k, s, stats=bn.stats, out=z), cflops, _nb(x, w16, z), desc)
             self.sync_stats(F, bn)
@@ -258,7 +291,6 @@ class Plan:
         net = self.net
         k, s = conv.kernel_size[0], conv.stride[0]
         dz = self.act(*z.shape)
-        w16 = net._packed(conv.weight, net._w16)
         gw = net._packed(conv.weight, net._g32)
         if not reduced:  # else: the dgrad that produced dy already accumulated dbeta / dgamma in its epilogue
             B.add("bn_bwd_reduce", lambda: ops.bn_bwd_reduce(dy, ymask, z, bn.mean, bn.invstd, bn.dbeta, bn.dgamma),
@@ -267,9 +299,8 @@ class Plan:
         B.add("bn_bwd_apply", lambda: ops.bn_bwd_apply(dy, ymask, z, bn.mean, bn.invstd, bn.gamma, bn.app_dbeta,
                                                       bn.app_dgamma, dz, g_out, g_out_acc, self.bn_scale), 0,
               _nb(dy, ymask, z, dz, g_out))
-        desc = "%d->%d k%d s%d @%dx%dx%d" % (x.shape[3], dz.shape[3], k, s, x.shape[0], x.shape[1], x.shape[2])
         B.add("conv_wgrad", lambda: ops.conv_wgrad(dz, x, gw, k, s), 2.0 * dz.numel() * x.shape[3] * k * k,
-              _nb(dz, x, gw), desc)
+              _nb(dz, x, gw), _conv_desc(x, dz.shape[3], k, s), side=True)
         return dz
 
     def dgrad_into(self, B, dz, conv, x, relu_mask=None, ci_off=0, bn_reduce=None):
@@ -299,389 +330,98 @@ class Plan:
               "%d<-%d k%d s%d @%dx%dx%d%s" % (cin, dz.shape[3], k, s, x.shape[0], x.shape[1], x.shape[2],
                                               " acc" if acc else ""))
 
-    # ------------------------------------------------------------------------------------------ network
-    def _build(self):
-        if self.net.plan_kind == "vgg":
-            return self._build_vgg()
-        net, n, h, w = self.net, self.n, self.h, self.w
-        F = self.fwd_ops
-        enc = net.encoder
-        train = self.training
-
-        # ---- stem: 7x7/s2 conv as im2col + GEMM, BN, ReLU, 2x2 max-pool (src/unet_models.py:360-363)
-        col = self.act(n, h // 2, w // 2, 192)
-        stem_w16 = torch.zeros((1, 64, 192), dtype=BF16, device=self.dev)
-        self._keep.append(stem_w16)
-        stem_master = net._vec(enc.conv1.weight, net._p32)
-        F.add("stem_im2col", lambda: ops.stem_im2col(self.x_in, col), 0, _nb(self.x_in, col))
-        F.add("misc", lambda: ops.stem_pack_weight(stem_master, stem_w16))
-        sflops = 2.0 * n * (h // 2) * (w // 2) * 64 * 147
-        z0 = self.act(n, h // 2, w // 2, 64)
-        bn0 = self.bn_state(enc.bn1)
-        if train:
-            F.add("conv_fwd", lambda: ops.conv_fwd(col, stem_w16, 1, 1, stats=bn0.stats, out=z0), sflops, _nb(col, z0))
-            self.sync_stats(F, bn0)
-            a0 = self.act(*z0.shape)
-            self.bn_apply_op(z0, bn0, a0, True)
-        else:
-            F.add("conv_fwd", lambda: ops.conv_fwd(col, stem_w16, 1, 1, bias=bn0.shift, relu=True, scale=bn0.scale,
-                                                   out=z0), sflops, _nb(col, z0))
-            a0 = z0
-        c1 = self.act(n, h // 4, w // 4, 64)
-        F.add("maxpool", lambda: ops.maxpool2_fwd(a0, c1), 0, _nb(a0, c1))
-        if train:
-            def build_stem(B):
-                d_a0 = self.gbuf(a0)
-                d_c1 = self.gbuf(c1)
-                dz0 = self.act(*z0.shape)
-                stem_gw = torch.zeros((1, 64, 192), dtype=F32, device=self.dev)
-                self._keep.append(stem_gw)
-                stem_g = net._vec(enc.conv1.weight, net._g32)
-                B.add("maxpool", lambda: ops.maxpool2_bwd(a0, d_c1, d_a0, False), 0, _nb(a0, d_c1, d_a0))
-                B.add("bn_bwd_reduce", lambda: ops.bn_bwd_reduce(d_a0, a0, z0, bn0.mean, bn0.invstd, bn0.dbeta,
-                                                                bn0.dgamma), 0, _nb(d_a0, a0, z0))
-                self.sync_bn_grads(B, bn0)
-                B.add("bn_bwd_apply", lambda: ops.bn_bwd_apply(d_a0, a0, z0, bn0.mean, bn0.invstd, bn0.gamma,
-                                                              bn0.app_dbeta, bn0.app_dgamma, dz0, None, False,
-                                                              self.bn_scale),
-                      0, _nb(d_a0, a0, z0, dz0))
-                B.add("misc", lambda: L.zero(stem_gw))
-                B.add("conv_wgrad", lambda: ops.conv_wgrad(dz0, col, stem_gw, 1, 1), sflops, _nb(dz0, col))
-                B.add("misc", lambda: ops.stem_unpack_wgrad(stem_gw, stem_g))
-            self._bwd_builders.append(("stem", build_stem))
-
-        # ---- encoder stages (torchvision BasicBlock / Bottleneck)
-        x = c1
-        skips = []
-        for li, layer in enumerate((enc.layer1, enc.layer2, enc.layer3, enc.layer4)):
-            for bi, blk in enumerate(layer):
-                xin = x
-                self._cur_tag = "layer%d" % (li + 1)
-                x = self._res_block(x, blk)
-                self.units.append(("block", "encoder.layer%d.%d" % (li + 1, bi), (xin,), x))
-            skips.append(x)
-        c2, c3, c4, c5 = skips
-
-        # ---- centre + decoder (src/unet_models.py:373-403)
-        pool = self.act(n, c5.shape[1] // 2, c5.shape[2] // 2, c5.shape[3])
-        F.add("maxpool", lambda: ops.maxpool2_fwd(c5, pool), 0, _nb(c5, pool))
-        if train:
-            def build_pool(B):
-                d_pool, d_c5 = self.gbuf(pool), self.gbuf(c5)
-                acc = self.gmode(c5)  # dec5's skip dgrad ran first -> accumulate
-                B.add("maxpool", lambda: ops.maxpool2_bwd(c5, d_pool, d_c5, acc), 0, _nb(c5, d_pool, d_c5))
-            self._bwd_builders.append(("decoder", build_pool))
-        center = self._decoder(pool, None, net.center, pool_input=True)
-        d5 = self._decoder(center, c5, net.dec5)
-        d4 = self._decoder(d5, c4, net.dec4)
-        d3 = self._decoder(d4, c3, net.dec3)
-        d2 = self._decoder(d3, c2, net.dec2)
-        d1 = self._decoder(d2, None, net.dec1)
-        self.units += [("decoder", "center", (pool,), center), ("decoder", "dec5", (center, c5), d5),
-                       ("decoder", "dec4", (d5, c4), d4), ("decoder", "dec3", (d4, c3), d3),
-                       ("decoder", "dec2", (d3, c2), d2), ("decoder", "dec1", (d2,), d1)]
-        # dec0 = ConvRelu(32, 32)
-        conv0 = net.dec0.conv
-        w0_16 = net._packed(conv0.weight, net._w16)
-        b0 = net._vec(conv0.bias, net._p32)
-        d0 = self.act(n, h, w, conv0.out_channels)
-        f0 = 2.0 * d0.numel() * d1.shape[3] * 9
-        F.add("conv_fwd", lambda: ops.conv_fwd(d1, w0_16, 3, 1, bias=b0, relu=True, out=d0), f0, _nb(d1, d0))
-        fw, fb = net._vec(net.final.weight, net._p32), net._vec(net.final.bias, net._p32)
-        F.add("final_conv", lambda: ops.final_conv_fwd(d0, fw, fb, self.logits), 2.0 * self.logits.numel() * 32,
-              _nb(d0, self.logits))
-        self.named = dict(conv1=c1, conv2=c2, conv3=c3, conv4=c4, conv5=c5, center=center, dec5=d5, dec4=d4, dec3=d3,
-                          dec2=d2, dec1=d1, dec0=d0)
-        if train:
-            def build_head(B):
-                g_d0 = self.gbuf(d0)
-                gfw, gfb = net._vec(net.final.weight, net._g32), net._vec(net.final.bias, net._g32)
-                # final 1x1 backward also applies dec0's ReLU mask
-                B.add("final_conv", lambda: ops.final_conv_bwd(d0, fw, self.dlogits, g_d0, gfw, gfb),
-                      4.0 * self.logits.numel() * 32, _nb(d0, self.dlogits, g_d0))
-                gb0 = net._vec(conv0.bias, net._g32)
-                gw0 = net._packed(conv0.weight, net._g32)
-                B.add("channel_sum", lambda: ops.channel_sum(g_d0, gb0), 0, _nb(g_d0))
-                B.add("conv_wgrad", lambda: ops.conv_wgrad(g_d0, d1, gw0, 3, 1), f0, _nb(g_d0, d1))
-                self.dgrad_into(B, g_d0, conv0, d1, relu_mask=d1)
-            self._bwd_builders.append(("decoder", build_head))
-
-    # ------------------------------------------------------------------------------------------ VGG encoders
-    def _build_vgg(self):
-        """UNet11 / UNetVGG16 (src/unet_models.py:89-106, :296-312): five stages of conv + bias + ReLU units, each stage
-        output pooled and concatenated into the decoder; no BatchNorm.  Backward: the decoder runs first and stores the
-        skip segment's data gradient of every stage output; the pool backward adds the pooled path, applies the ReLU
-        mask and sums the bias gradient (maxpool2_bwd_skip_relu).  Units inside a stage have one consumer: their mask
-        and bias gradient ride in the next conv's dgrad epilogue."""
-        net, n, h, w = self.net, self.n, self.h, self.w
-        F = self.fwd_ops
-        enc = net.encoder
-        train = self.training
-        skips = []
-        x = None
-        for si, stage in enumerate(net._stages):
-            self._cur_tag = "conv%d" % (si + 1)
-            for ci, idx in enumerate(stage):
-                xin = x
-                x = self._vgg_input_unit(enc[idx]) if xin is None else self._vgg_unit(xin, enc[idx])
-                self.units.append(("conv", "encoder.%d" % idx, () if xin is None else (xin,), x))
-            skips.append(x)
-            x = self._vgg_pool(x)
-        c1, c2, c3, c4, c5 = skips
-        # ---- decoder (src/unet_models.py:99-105, :303-310)
-        center = self._decoder(x, None, net.center, pool_input=True)
-        d5 = self._decoder(center, c5, net.dec5)
-        d4 = self._decoder(d5, c4, net.dec4)
-        d3 = self._decoder(d4, c3, net.dec3)
-        d2 = self._decoder(d3, c2, net.dec2)
-        self.units += [("decoder", "center", (x,), center), ("decoder", "dec5", (center, c5), d5),
-                       ("decoder", "dec4", (d5, c4), d4), ("decoder", "dec3", (d4, c3), d3),
-                       ("decoder", "dec2", (d3, c2), d2)]
-        # dec1 = ConvRelu(32 + 64, 32) over cat[dec2, conv1], then the 1x1 classifier
-        conv = net.dec1.conv
-        w16 = net._packed(conv.weight, net._w16)
-        b = net._vec(conv.bias, net._p32)
-        d1 = self.act(n, h, w, conv.out_channels)
-        ca, cb = d2.shape[3], c1.shape[3]
-        f1 = 2.0 * d1.numel() * (ca + cb) * 9
-        F.add("conv_fwd", lambda: ops.conv_fwd(d2, w16, 3, 1, bias=b, relu=True, x2=c1, out=d1), f1, _nb(d2, c1, w16, d1),
-              "dec %d->%d k3 @%dx%dx%d" % (ca + cb, conv.out_channels, n, h, w))
-        fw, fb = net._vec(net.final.weight, net._p32), net._vec(net.final.bias, net._p32)
-        F.add("final_conv", lambda: ops.final_conv_fwd(d1, fw, fb, self.logits), 2.0 * self.logits.numel() * 32,
-              _nb(d1, self.logits))
-        self.units.append(("decoder", "dec1", (d2, c1), d1))
-        self.named = dict(conv1=c1, conv2=c2, conv3=c3, conv4=c4, conv5=c5, center=center, dec5=d5, dec4=d4, dec3=d3,
-                          dec2=d2, dec1=d1)
-        if train:
-            def build_head(B):
-                g_d1 = self.gbuf(d1)
-                gfw, gfb = net._vec(net.final.weight, net._g32), net._vec(net.final.bias, net._g32)
-                # the classifier's backward also applies dec1's ReLU mask
-                B.add("final_conv", lambda: ops.final_conv_bwd(d1, fw, self.dlogits, g_d1, gfw, gfb),
-                      4.0 * self.logits.numel() * 32, _nb(d1, self.dlogits, g_d1))
-                gb = net._vec(conv.bias, net._g32)
-                gw = net._packed(conv.weight, net._g32)
-                B.add("channel_sum", lambda: ops.channel_sum(g_d1, gb), 0, _nb(g_d1))
-                B.add("conv_wgrad", lambda: ops.conv_wgrad(g_d1, d2, gw, 3, 1, ci_off=0), 2.0 * d1.numel() * ca * 9,
-                      _nb(g_d1, d2), "dec %d->%d k3 @%dx%dx%d" % (ca, conv.out_channels, n, h, w))
-                B.add("conv_wgrad", lambda: ops.conv_wgrad(g_d1, c1, gw, 3, 1, ci_off=ca), 2.0 * d1.numel() * cb * 9,
-                      _nb(g_d1, c1), "dec-skip %d->%d k3 @%dx%dx%d" % (cb, conv.out_channels, n, h, w))
-                self.dgrad_into(B, g_d1, conv, d2, relu_mask=d2, ci_off=0)
-                self.dgrad_into(B, g_d1, conv, c1, relu_mask=None, ci_off=ca)
-            self._bwd_builders.append(("decoder", build_head))
-
-    def _vgg_input_unit(self, conv):
-        """encoder.0 = Conv2d(3, 64, 3, padding 1) + ReLU on the full-resolution image: im2col (27 of 32 columns) + a
-        1x1 GEMM with bias and ReLU; the weight gradient is the 1x1 wgrad, unpacked into the master slot"""
-        net, n, h, w = self.net, self.n, self.h, self.w
-        F = self.fwd_ops
-        cout = conv.out_channels
-        col = self.act(n, h, w, 32)
-        w16 = torch.zeros((1, cout, 32), dtype=BF16, device=self.dev)
-        self._keep.append(w16)
-        master = net._vec(conv.weight, net._p32)
-        b = net._vec(conv.bias, net._p32)
-        y = self.act(n, h, w, cout)
-        fl = 2.0 * n * h * w * cout * 27     # the real 27-wide reduction, as the reference counts it
-        desc = "3->%d k3 (im2col) @%dx%dx%d" % (cout, n, h, w)
-        F.add("im2col", lambda: ops.vgg_input_im2col(self.x_in, col), 0, _nb(self.x_in, col))
-        F.add("misc", lambda: ops.vgg_input_pack_weight(master, w16))
-        F.add("conv_fwd", lambda: ops.conv_fwd(col, w16, 1, 1, bias=b, relu=True, out=y), fl, _nb(col, y), desc)
-        if self.training:
-            self.bias_sum[id(y)] = net._vec(conv.bias, net._g32)
-
-            def build_input(B):
-                g = self.gbuf(y)       # complete, masked, bias gradient summed (by its consumer)
-                gw = torch.zeros((1, cout, 32), dtype=F32, device=self.dev)
-                self._keep.append(gw)
-                g_slot = net._vec(conv.weight, net._g32)
-                B.add("misc", lambda: L.zero(gw))
-                # no desc: stays on the main stream, in order with the zeroing and the unpack (like the ResNet stem)
-                B.add("conv_wgrad", lambda: ops.conv_wgrad(g, col, gw, 1, 1), fl, _nb(g, col))
-                B.add("misc", lambda: ops.vgg_input_unpack_wgrad(gw, g_slot))
-            self._bwd_builders.append((self._cur_tag, build_input))
-        return y
-
-    def _vgg_unit(self, x, conv):
-        """y = relu(conv3x3(x) + b).  x is a pool output (gradient stored plainly) or the previous unit's output (its
-        ReLU mask and bias gradient fused into this unit's dgrad epilogue)"""
+    # ------------------------------------------------------------------------------------------ decoder
+    def _conv_relu(self, x1, skip, conv, label):
+        """ConvRelu over cat[x1, skip] (src/unet_models.py:25-34): relu(conv3x3(.) + b), the concat fused into the
+        GEMM; `label`: give its launch a breakdown label"""
         net = self.net
-        F = self.fwd_ops
-        n, h, w, cin = x.shape
+        n, h, w, c1 = x1.shape
         cout = conv.out_channels
         w16 = net._packed(conv.weight, net._w16)
         b = net._vec(conv.bias, net._p32)
         y = self.act(n, h, w, cout)
-        fl = 2.0 * y.numel() * cin * 9
-        desc = "%d->%d k3 s1 @%dx%dx%d" % (cin, cout, n, h, w)
-        F.add("conv_fwd", lambda: ops.conv_fwd(x, w16, 3, 1, bias=b, relu=True, out=y), fl, _nb(x, w16, y), desc)
-        if self.training:
-            self.bias_sum[id(y)] = net._vec(conv.bias, net._g32)
-            x_is_unit = id(x) in self.bias_sum
-
-            def build_unit(B):
-                g = self.gbuf(y)
-                gw = net._packed(conv.weight, net._g32)
-                B.add("conv_wgrad", lambda: ops.conv_wgrad(g, x, gw, 3, 1), fl, _nb(g, x, gw), desc)
-                self.dgrad_into(B, g, conv, x, relu_mask=x if x_is_unit else None)
-            self._bwd_builders.append((self._cur_tag, build_unit))
+        ctot = c1 + (skip.shape[3] if skip is not None else 0)
+        self.fwd_ops.add("conv_fwd", lambda: ops.conv_fwd(x1, w16, 3, 1, bias=b, relu=True, x2=skip, out=y),
+                         2.0 * y.numel() * ctot * 9, _nb(x1, skip, w16, y),
+                         "dec %d->%d k3 @%dx%dx%d" % (ctot, cout, n, h, w) if label else "")
         return y
 
-    def _vgg_pool(self, y):
-        """2x2 max-pool of a stage output y; its backward completes grad(y) (see _build_vgg)"""
-        F = self.fwd_ops
-        n, h, w, c = y.shape
-        p = self.act(n, h // 2, w // 2, c)
-        F.add("maxpool", lambda: ops.maxpool2_fwd(y, p), 0, _nb(y, p))
-        if self.training:
-            gb = self.bias_sum[id(y)]
-
-            def build_pool(B):
-                if id(y) not in self.written:
-                    raise RuntimeError("plan error: the skip gradient of a VGG stage output must be stored first")
-                d_p, g = self.gbuf(p), self.gbuf(y)
-                self.bias_fused.add(id(y))
-                B.add("maxpool", lambda: ops.maxpool2_bwd_skip_relu(y, d_p, g, gb), 0, _nb(y, d_p, g, g))
-            self._bwd_builders.append((self._cur_tag, build_pool))
-        return p
-
-    def _vgg_segments(self):
-        """[decoder | conv5 stage | conv4 stage | rest], like bwd_segments for the ResNets"""
-        net = self.net
-        tags = self.bwd_tags
-        n = len(tags)
-        i_dec = max(i for i, t in enumerate(tags) if t == "decoder") + 1
-        i_c5 = max(i for i, t in enumerate(tags) if t == "conv5") + 1
-        i_c4 = max(i for i, t in enumerate(tags) if t == "conv4") + 1
-        off = {name: net._slots[id(p)].off for name, p, _ in net._arena_params()}
-        total = net._p32.numel()
-        o_dec = off["center.block.0.conv.weight"]
-        o_c5 = off["encoder.%d.weight" % net._stages[4][0]]
-        o_c4 = off["encoder.%d.weight" % net._stages[3][0]]
-        return [(0, i_dec, o_dec, total), (i_dec, i_c5, o_c5, o_dec), (i_c5, i_c4, o_c4, o_c5), (i_c4, n, 0, o_c4)]
-
-    def _res_block(self, x, blk):
-        """torchvision BasicBlock / Bottleneck forward + backward plan"""
-        train = self.training
-        F = self.fwd_ops
-        is_bottleneck = hasattr(blk, "conv3")
-        convs = [(blk.conv1, blk.bn1), (blk.conv2, blk.bn2)] + ([(blk.conv3, blk.bn3)] if is_bottleneck else [])
-        if not train:
-            cur = x
-            for conv, bnm in convs[:-1]:
-                cur, _, _ = self.conv_bn(cur, conv, bnm, True)
-            ident = x
-            if blk.downsample is not None:
-                ident, _, _ = self.conv_bn(x, blk.downsample[0], blk.downsample[1], False)
-            out, _, _ = self.conv_bn(cur, convs[-1][0], convs[-1][1], True, residual=ident)
-            return out
-        acts = [x]
-        units = []
-        cur = x
-        for conv, bnm in convs[:-1]:
-            y, z, bn = self.conv_bn(cur, conv, bnm, True)
-            units.append((conv, cur, y, z, bn))
-            cur = y
-        conv_l, bn_l = convs[-1]
-        _, z_l, bnl = self.conv_bn(cur, conv_l, bn_l, None)
-        out = self.act(*z_l.shape)
-        if blk.downsample is not None:
-            dconv, dbnm = blk.downsample[0], blk.downsample[1]
-            _, zd, bnd = self.conv_bn(x, dconv, dbnm, None)
-            self.bn_apply_op(z_l, bnl, out, True, zd, bnd)
-        else:
-            self.bn_apply_op(z_l, bnl, out, True, x)
-        if train:
-            last_in = cur
-
-            def build_block(B):
-                d_out = self.gbuf(out)
-                if blk.downsample is None:
-                    # identity branch: grad(x) (+)= g = d_out * (out > 0), emitted by the last BN's backward pass
-                    gx = self.gbuf(x)
-                    acc = self.gmode(x)
-                    dz_l = self.conv_unit_backward(B, d_out, out, z_l, bnl, conv_l, last_in, g_out=gx, g_out_acc=acc)
-                else:
-                    dz_l = self.conv_unit_backward(B, d_out, out, z_l, bnl, conv_l, last_in)
-                # walk back through the inner units
-                dz = dz_l
-                conv_next = conv_l
-                for conv, xin, y, z, bn in reversed(units):
-                    # y has a single consumer: its ReLU mask and its BN's backward reductions ride in the dgrad epilogue
-                    self.dgrad_into(B, dz, conv_next, y, bn_reduce=(z, bn))
-                    dz = self.conv_unit_backward(B, self.gbuf(y), None, z, bn, conv, xin, reduced=True)
-                    conv_next = conv
-                self.dgrad_into(B, dz, conv_next, x)
-                if blk.downsample is not None:
-                    dzd = self.conv_unit_backward(B, d_out, out, zd, bnd, dconv, x)
-                    self.dgrad_into(B, dzd, dconv, x)
-            self._bwd_builders.append((self._cur_tag, build_block))
-        return out
+    def _conv_relu_backward(self, B, g, conv, x1, skip, x1_relu, label, side):
+        """weight and data gradients of _conv_relu given g, the gradient of its output with the ReLU mask applied.
+        x1_relu: x1 is a ReLU output (its mask rides in the dgrad epilogue); the skip's mask is applied by its owner.
+        `side`: the weight-gradient GEMMs go to the side stream"""
+        gw = self.net._packed(conv.weight, self.net._g32)
+        n, h, w, cout = g.shape
+        c1 = x1.shape[3]
+        srcs = [(x1, 0, "dec")] if skip is None else [(x1, 0, "dec"), (skip, c1, "dec-skip")]
+        for x, ci_off, name in srcs:
+            B.add("conv_wgrad", lambda x=x, ci_off=ci_off: ops.conv_wgrad(g, x, gw, 3, 1, ci_off=ci_off),
+                  2.0 * g.numel() * x.shape[3] * 9, _nb(g, x),
+                  "%s %d->%d k3 @%dx%dx%d" % (name, x.shape[3], cout, n, h, w) if label else "", side)
+        self.dgrad_into(B, g, conv, x1, relu_mask=x1 if x1_relu else None)
+        if skip is not None:
+            self.dgrad_into(B, g, conv, skip, ci_off=c1)
 
     def _decoder(self, x1, skip, block, pool_input=False):
         """DecoderBlockV2 / DecoderBlock: relu(conv3x3(cat[x1, skip]) + b) -> relu(convT(.) + b) with the 4x4 or the 3x3
         (output_padding 1) stride-2 transposed conv   (src/unet_models.py:42-53,136-141)"""
         net = self.net
-        F = self.fwd_ops
         conv, deconv = block.block[0].conv, block.block[1]
-        n, h, w, c1 = x1.shape
-        cmid, cout = conv.out_channels, deconv.out_channels
+        mid = self._conv_relu(x1, skip, conv, label=True)
+        n, h, w, cmid = mid.shape
+        cout = deconv.out_channels
         kt = deconv.kernel_size[0]
-        w16 = net._packed(conv.weight, net._w16)
-        b1 = net._vec(conv.bias, net._p32)
         wt16 = net._packed(deconv.weight, net._w16)
         b2 = net._vec(deconv.bias, net._p32)
-        mid = self.act(n, h, w, cmid)
         out = self.act(n, 2 * h, 2 * w, cout)
-        ctot = c1 + (skip.shape[3] if skip is not None else 0)
-        if self.training:
-            self.bias_sum[id(out)] = net._vec(deconv.bias, net._g32)
-        fc = 2.0 * mid.numel() * ctot * 9
+        self.bias_sum[id(out)] = net._vec(deconv.bias, net._g32)
         ft = 2.0 * mid.numel() * cout * kt * kt
-        F.add("conv_fwd", lambda: ops.conv_fwd(x1, w16, 3, 1, bias=b1, relu=True, x2=skip, out=mid), fc,
-              _nb(x1, skip, w16, mid), "dec %d->%d k3 @%dx%dx%d" % (ctot, cmid, n, h, w))
-        F.add("convt_fwd", lambda: ops.convt_fwd(mid, wt16, bias=b2, relu=True, out=out), ft, _nb(mid, wt16, out),
-              "%d->%d @%dx%dx%d" % (cmid, cout, n, h, w))
-        if self.training:
-            def build_dec(B):
-                g_out = self.gbuf(out)   # already masked by out's ReLU (the consumer's dgrad epilogue did it)
-                g_mid = self.gbuf(mid)
-                gwt = net._packed(deconv.weight, net._g32)
-                gb2 = net._vec(deconv.bias, net._g32)
-                gw = net._packed(conv.weight, net._g32)
-                gb1 = net._vec(conv.bias, net._g32)
-                if id(out) not in self.bias_fused:   # else: summed in the epilogue of the dgrad that produced g_out
-                    B.add("channel_sum", lambda: ops.channel_sum(g_out, gb2), 0, _nb(g_out))
-                dd = "%d->%d @%dx%dx%d" % (cmid, cout, n, h, w)
-                B.add("convt_wgrad", lambda: ops.convt_wgrad(g_out, mid, gwt), ft, _nb(g_out, mid, gwt), dd)
-                B.add("convt_dgrad", lambda: ops.convt_dgrad(g_out, wt16, relu_mask=mid, out=g_mid, channel_sum=gb1), ft,
-                      _nb(g_out, wt16, mid, g_mid), dd)
-                B.add("conv_wgrad", lambda: ops.conv_wgrad(g_mid, x1, gw, 3, 1, ci_off=0),
-                      2.0 * mid.numel() * c1 * 9, _nb(g_mid, x1), "dec %d->%d k3 @%dx%dx%d" % (c1, cmid, n, h, w))
-                if skip is not None:
-                    B.add("conv_wgrad", lambda: ops.conv_wgrad(g_mid, skip, gw, 3, 1, ci_off=c1),
-                          2.0 * mid.numel() * skip.shape[3] * 9, _nb(g_mid, skip),
-                          "dec-skip %d->%d k3 @%dx%dx%d" % (skip.shape[3], cmid, n, h, w))
-                # x1 is a decoder ReLU output (mask in the epilogue) unless it is the centre's max-pool output
-                self.dgrad_into(B, g_mid, conv, x1, relu_mask=None if pool_input else x1, ci_off=0)
-                if skip is not None:
-                    self.dgrad_into(B, g_mid, conv, skip, relu_mask=None, ci_off=c1)
-            self._bwd_builders.append(("decoder", build_dec))
+        dd = "%d->%d @%dx%dx%d" % (cmid, cout, n, h, w)
+        self.fwd_ops.add("convt_fwd", lambda: ops.convt_fwd(mid, wt16, bias=b2, relu=True, out=out), ft,
+                         _nb(mid, wt16, out), dd)
+
+        def build_dec(B):
+            g_out = self.gbuf(out)   # already masked by out's ReLU (the consumer's dgrad epilogue did it)
+            g_mid = self.gbuf(mid)
+            gwt = net._packed(deconv.weight, net._g32)
+            gb2 = net._vec(deconv.bias, net._g32)
+            gb1 = net._vec(conv.bias, net._g32)
+            if id(out) not in self.bias_fused:   # else: summed in the epilogue of the dgrad that produced g_out
+                B.add("channel_sum", lambda: ops.channel_sum(g_out, gb2), 0, _nb(g_out))
+            B.add("convt_wgrad", lambda: ops.convt_wgrad(g_out, mid, gwt), ft, _nb(g_out, mid, gwt), dd, side=True)
+            B.add("convt_dgrad", lambda: ops.convt_dgrad(g_out, wt16, relu_mask=mid, out=g_mid, channel_sum=gb1), ft,
+                  _nb(g_out, wt16, mid, g_mid), dd)
+            # x1 is a decoder ReLU output unless it is the centre's max-pool output
+            self._conv_relu_backward(B, g_mid, conv, x1, skip, not pool_input, label=True, side=True)
+        self.on_backward("decoder", build_dec)
         return out
 
-    # ------------------------------------------------------------------------------------------ execution
-    def _bn_table(self):
-        if getattr(self, "_bn_tab", None) is None:
-            rows = [[b.gamma.data_ptr(), b.beta.data_ptr(), b.mod.running_mean.data_ptr(), b.mod.running_var.data_ptr(),
-                     b.scale.data_ptr(), b.shift.data_ptr(), b.c] for b in self._bns]
-            self._bn_tab = torch.tensor(rows, dtype=torch.int64, device=self.dev)
-            self._bn_maxc = max(b.c for b in self._bns)
-        return self._bn_tab
+    def _classifier(self, x1, skip, conv_relu, label, side):
+        """the last ConvRelu over cat[x1, skip] and the 1x1 classifier into self.logits, whose backward also applies the
+        ConvRelu's ReLU mask.  `label` / `side`: breakdown labels and side-stream placement of its conv launches"""
+        net = self.net
+        conv = conv_relu.conv
+        y = self._conv_relu(x1, skip, conv, label)
+        fw, fb = net._vec(net.final.weight, net._p32), net._vec(net.final.bias, net._p32)
+        self.fwd_ops.add("final_conv", lambda: ops.final_conv_fwd(y, fw, fb, self.logits),
+                         2.0 * self.logits.numel() * 32, _nb(y, self.logits))
 
+        def build_head(B):
+            g = self.gbuf(y)
+            gfw, gfb = net._vec(net.final.weight, net._g32), net._vec(net.final.bias, net._g32)
+            B.add("final_conv", lambda: ops.final_conv_bwd(y, fw, self.dlogits, g, gfw, gfb),
+                  4.0 * self.logits.numel() * 32, _nb(y, self.dlogits, g))
+            gb = net._vec(conv.bias, net._g32)
+            B.add("channel_sum", lambda: ops.channel_sum(g, gb), 0, _nb(g))
+            self._conv_relu_backward(B, g, conv, x1, skip, True, label, side)
+        self.on_backward("decoder", build_head)
+        return y
+
+    # ------------------------------------------------------------------------------------------ execution
     def _run_fwd(self):
-        if not self.training and self._bns:     # (the VGG nets have no BatchNorm)
-            tab = self._bn_table()
-            L.fcall("mcb_bn_eval_params_batched", tab.data_ptr(), len(self._bns), self._bn_maxc, BN_EPS)
+        if self._bn_tab is not None:
+            L.fcall("mcb_bn_eval_params_batched", self._bn_tab.data_ptr(), len(self._bns), max(b.c for b in self._bns),
+                    BN_EPS)
         if self.training:
             if self.sync_nvlink:
                 L.fcall("mcb_sync_step_bump", self._sync_step.data_ptr())
@@ -698,10 +438,10 @@ class Plan:
         L.zero(self.net._g32)
         if self.sync_nvlink:
             L.zero(self._dstats_loc)
-        # Weight/bias-gradient launches are leaves of the backward graph (they only add into the gradient arena): each
-        # goes to the low-priority side stream, forked right after its producer and joined at the end, so the
-        # tensor-core-bound wgrad GEMMs overlap the HBM-bound BatchNorm-backward kernels of the layers below instead of
-        # queueing behind them, and the high-priority main chain (graph_capture) is served first.
+        # Weight-gradient launches marked `side` are leaves of the backward graph (they only add into the gradient
+        # arena): each goes to the low-priority side stream, forked right after its producer and joined at the end, so
+        # the tensor-core-bound wgrad GEMMs overlap the HBM-bound BatchNorm-backward kernels of the layers below instead
+        # of queueing behind them, and the high-priority main chain (graph_capture) is served first.
         # (No buffer is recycled inside a step, so the only hazards are the recorded producer -> consumer edges.)
         main = torch.cuda.current_stream()
         if self._side is None:
@@ -721,7 +461,7 @@ class Plan:
             if hooks and li in hooks:
                 on_side(hooks[li])
             for op in layer:
-                if op.kind in _SIDE_KINDS and op.desc:
+                if op.side:
                     on_side(op)
                 else:
                     op()
@@ -733,23 +473,19 @@ class Plan:
             main.wait_event(ev)
 
     def bwd_segments(self):
-        """split points for overlapping the gradient all-reduce / the Adam update with the backward pass:
-        [decoder | layer4 | layer3 | rest].  -> [(first_layer, last_layer, arena_lo, arena_hi)], the arena range is
-        complete once the segment has run (layer3's 23 blocks reduce while layer2 / layer1 / stem still run)"""
+        """split points for overlapping the gradient all-reduce / the Adam update with the backward pass, at the
+        family's _segment_bounds (ResNets: [decoder | layer4 | layer3 | rest]).
+        -> [(first_layer, last_layer, arena_lo, arena_hi)], the arena range is complete once the segment has run
+        (layer3's 23 blocks reduce while layer2 / layer1 / stem still run)"""
         net = self.net
-        tags = self.bwd_tags
-        n = len(tags)
-        if net.plan_kind == "vgg":
-            return self._vgg_segments()
-        i_dec = max(i for i, t in enumerate(tags) if t == "decoder") + 1
-        i_l4 = max(i for i, t in enumerate(tags) if t == "layer4") + 1
-        i_l3 = max(i for i, t in enumerate(tags) if t == "layer3") + 1
         off = {name: net._slots[id(p)].off for name, p, _ in net._arena_params()}
-        total = net._p32.numel()
-        o_dec = off["center.block.0.conv.weight"]
-        o_l4 = off["encoder.layer4.0.conv1.weight"]
-        o_l3 = off["encoder.layer3.0.conv1.weight"]
-        return [(0, i_dec, o_dec, total), (i_dec, i_l4, o_l4, o_dec), (i_l4, i_l3, o_l3, o_l4), (i_l3, n, 0, o_l3)]
+        segs = []
+        first, hi = 0, net._p32.numel()
+        for tag, param in self._segment_bounds():
+            last = max(i for i, t in enumerate(self.bwd_tags) if t == tag) + 1
+            segs.append((first, last, off[param], hi))
+            first, hi = last, off[param]
+        return segs + [(first, len(self.bwd_tags), 0, hi)]
 
     def forward(self, x):
         self.x_in.copy_(x)
@@ -775,6 +511,260 @@ class Plan:
             self.graph_bwd = g
             return
         self.graph_bwd.replay()
+
+
+class ResNetPlan(Plan):
+    """UNetResNet / AlbuNet (src/unet_models.py:315-403): 7x7 stem, torchvision BasicBlock / Bottleneck stages, the
+    DecoderBlockV2 decoder, dec0 and the classifier"""
+
+    def _segment_bounds(self):
+        return [("decoder", "center.block.0.conv.weight"), ("layer4", "encoder.layer4.0.conv1.weight"),
+                ("layer3", "encoder.layer3.0.conv1.weight")]
+
+    def _build(self):
+        net, n, h, w = self.net, self.n, self.h, self.w
+        F = self.fwd_ops
+        enc = net.encoder
+
+        # ---- stem: 7x7/s2 conv as im2col + GEMM, BN, ReLU, 2x2 max-pool (src/unet_models.py:360-363)
+        col = self.act(n, h // 2, w // 2, 192)
+        stem_w16 = torch.zeros((1, 64, 192), dtype=BF16, device=self.dev)
+        self._keep.append(stem_w16)
+        stem_master = net._vec(enc.conv1.weight, net._p32)
+        F.add("stem_im2col", lambda: ops.stem_im2col(self.x_in, col), 0, _nb(self.x_in, col))
+        F.add("misc", lambda: ops.stem_pack_weight(stem_master, stem_w16))
+        sflops = 2.0 * n * (h // 2) * (w // 2) * 64 * 147
+        z0 = self.act(n, h // 2, w // 2, 64)
+        bn0 = self.bn_state(enc.bn1)
+        if self.training:
+            F.add("conv_fwd", lambda: ops.conv_fwd(col, stem_w16, 1, 1, stats=bn0.stats, out=z0), sflops, _nb(col, z0))
+            self.sync_stats(F, bn0)
+            a0 = self.act(*z0.shape)
+            self.bn_apply_op(z0, bn0, a0, True)
+        else:
+            F.add("conv_fwd", lambda: ops.conv_fwd(col, stem_w16, 1, 1, bias=bn0.shift, relu=True, scale=bn0.scale,
+                                                   out=z0), sflops, _nb(col, z0))
+            a0 = z0
+        c1 = self.act(n, h // 4, w // 4, 64)
+        F.add("maxpool", lambda: ops.maxpool2_fwd(a0, c1), 0, _nb(a0, c1))
+
+        def build_stem(B):
+            d_a0 = self.gbuf(a0)
+            d_c1 = self.gbuf(c1)
+            dz0 = self.act(*z0.shape)
+            stem_gw = torch.zeros((1, 64, 192), dtype=F32, device=self.dev)
+            self._keep.append(stem_gw)
+            stem_g = net._vec(enc.conv1.weight, net._g32)
+            B.add("maxpool", lambda: ops.maxpool2_bwd(a0, d_c1, d_a0, False), 0, _nb(a0, d_c1, d_a0))
+            B.add("bn_bwd_reduce", lambda: ops.bn_bwd_reduce(d_a0, a0, z0, bn0.mean, bn0.invstd, bn0.dbeta,
+                                                            bn0.dgamma), 0, _nb(d_a0, a0, z0))
+            self.sync_bn_grads(B, bn0)
+            B.add("bn_bwd_apply", lambda: ops.bn_bwd_apply(d_a0, a0, z0, bn0.mean, bn0.invstd, bn0.gamma,
+                                                          bn0.app_dbeta, bn0.app_dgamma, dz0, None, False,
+                                                          self.bn_scale),
+                  0, _nb(d_a0, a0, z0, dz0))
+            B.add("misc", lambda: L.zero(stem_gw))
+            # on the main stream: the unpack that follows reads stem_gw
+            B.add("conv_wgrad", lambda: ops.conv_wgrad(dz0, col, stem_gw, 1, 1), sflops, _nb(dz0, col))
+            B.add("misc", lambda: ops.stem_unpack_wgrad(stem_gw, stem_g))
+        self.on_backward("stem", build_stem)
+
+        # ---- encoder stages (torchvision BasicBlock / Bottleneck)
+        x = c1
+        skips = []
+        for li, layer in enumerate((enc.layer1, enc.layer2, enc.layer3, enc.layer4)):
+            for bi, blk in enumerate(layer):
+                xin = x
+                x = self._res_block(x, blk, "layer%d" % (li + 1))
+                self.units.append(("block", "encoder.layer%d.%d" % (li + 1, bi), (xin,), x))
+            skips.append(x)
+        c2, c3, c4, c5 = skips
+
+        # ---- centre + decoder (src/unet_models.py:373-403)
+        pool = self.act(n, c5.shape[1] // 2, c5.shape[2] // 2, c5.shape[3])
+        F.add("maxpool", lambda: ops.maxpool2_fwd(c5, pool), 0, _nb(c5, pool))
+
+        def build_pool(B):
+            d_pool, d_c5 = self.gbuf(pool), self.gbuf(c5)
+            acc = self.gmode(c5)  # dec5's skip dgrad ran first -> accumulate
+            B.add("maxpool", lambda: ops.maxpool2_bwd(c5, d_pool, d_c5, acc), 0, _nb(c5, d_pool, d_c5))
+        self.on_backward("decoder", build_pool)
+        center = self._decoder(pool, None, net.center, pool_input=True)
+        d5 = self._decoder(center, c5, net.dec5)
+        d4 = self._decoder(d5, c4, net.dec4)
+        d3 = self._decoder(d4, c3, net.dec3)
+        d2 = self._decoder(d3, c2, net.dec2)
+        d1 = self._decoder(d2, None, net.dec1)
+        self.units += [("decoder", "center", (pool,), center), ("decoder", "dec5", (center, c5), d5),
+                       ("decoder", "dec4", (d5, c4), d4), ("decoder", "dec3", (d4, c3), d3),
+                       ("decoder", "dec2", (d3, c2), d2), ("decoder", "dec1", (d2,), d1)]
+        # dec0 = ConvRelu(32, 32): unlabelled, its weight gradient on the main stream
+        self._classifier(d1, None, net.dec0, label=False, side=False)
+
+    def _res_block(self, x, blk, tag):
+        """torchvision BasicBlock / Bottleneck forward + backward plan"""
+        is_bottleneck = hasattr(blk, "conv3")
+        convs = [(blk.conv1, blk.bn1), (blk.conv2, blk.bn2)] + ([(blk.conv3, blk.bn3)] if is_bottleneck else [])
+        if not self.training:
+            cur = x
+            for conv, bnm in convs[:-1]:
+                cur, _, _ = self.conv_bn(cur, conv, bnm, True)
+            ident = x
+            if blk.downsample is not None:
+                ident, _, _ = self.conv_bn(x, blk.downsample[0], blk.downsample[1], False)
+            out, _, _ = self.conv_bn(cur, convs[-1][0], convs[-1][1], True, residual=ident)
+            return out
+        units = []
+        cur = x
+        for conv, bnm in convs[:-1]:
+            y, z, bn = self.conv_bn(cur, conv, bnm, True)
+            units.append((conv, cur, y, z, bn))
+            cur = y
+        conv_l, bn_l = convs[-1]
+        _, z_l, bnl = self.conv_bn(cur, conv_l, bn_l, None)
+        out = self.act(*z_l.shape)
+        if blk.downsample is not None:
+            dconv, dbnm = blk.downsample[0], blk.downsample[1]
+            _, zd, bnd = self.conv_bn(x, dconv, dbnm, None)
+            self.bn_apply_op(z_l, bnl, out, True, zd, bnd)
+        else:
+            self.bn_apply_op(z_l, bnl, out, True, x)
+        last_in = cur
+
+        def build_block(B):
+            d_out = self.gbuf(out)
+            if blk.downsample is None:
+                # identity branch: grad(x) (+)= g = d_out * (out > 0), emitted by the last BN's backward pass
+                gx = self.gbuf(x)
+                acc = self.gmode(x)
+                dz_l = self.conv_unit_backward(B, d_out, out, z_l, bnl, conv_l, last_in, g_out=gx, g_out_acc=acc)
+            else:
+                dz_l = self.conv_unit_backward(B, d_out, out, z_l, bnl, conv_l, last_in)
+            # walk back through the inner units
+            dz = dz_l
+            conv_next = conv_l
+            for conv, xin, y, z, bn in reversed(units):
+                # y has a single consumer: its ReLU mask and its BN's backward reductions ride in the dgrad epilogue
+                self.dgrad_into(B, dz, conv_next, y, bn_reduce=(z, bn))
+                dz = self.conv_unit_backward(B, self.gbuf(y), None, z, bn, conv, xin, reduced=True)
+                conv_next = conv
+            self.dgrad_into(B, dz, conv_next, x)
+            if blk.downsample is not None:
+                dzd = self.conv_unit_backward(B, d_out, out, zd, bnd, dconv, x)
+                self.dgrad_into(B, dzd, dconv, x)
+        self.on_backward(tag, build_block)
+        return out
+
+
+class VGGPlan(Plan):
+    """UNet11 / UNetVGG16 (src/unet_models.py:89-106, :296-312): five stages of conv + bias + ReLU units, each stage
+    output pooled and concatenated into the decoder; no BatchNorm.  Backward: the decoder runs first and stores the
+    skip segment's data gradient of every stage output; the pool backward adds the pooled path, applies the ReLU
+    mask and sums the bias gradient (maxpool2_bwd_skip_relu).  Units inside a stage have one consumer: their mask
+    and bias gradient ride in the next conv's dgrad epilogue."""
+
+    def _segment_bounds(self):
+        stages = self.net._stages
+        return [("decoder", "center.block.0.conv.weight"), ("conv5", "encoder.%d.weight" % stages[4][0]),
+                ("conv4", "encoder.%d.weight" % stages[3][0])]
+
+    def _build(self):
+        net = self.net
+        enc = net.encoder
+        skips = []
+        x = None
+        for si, stage in enumerate(net._stages):
+            tag = "conv%d" % (si + 1)
+            for idx in stage:
+                xin = x
+                x = self._input_unit(enc[idx], tag) if xin is None else self._unit(xin, enc[idx], tag)
+                self.units.append(("conv", "encoder.%d" % idx, () if xin is None else (xin,), x))
+            skips.append(x)
+            x = self._pool(x, tag)
+        c1, c2, c3, c4, c5 = skips
+        # ---- decoder (src/unet_models.py:99-105, :303-310)
+        center = self._decoder(x, None, net.center, pool_input=True)
+        d5 = self._decoder(center, c5, net.dec5)
+        d4 = self._decoder(d5, c4, net.dec4)
+        d3 = self._decoder(d4, c3, net.dec3)
+        d2 = self._decoder(d3, c2, net.dec2)
+        self.units += [("decoder", "center", (x,), center), ("decoder", "dec5", (center, c5), d5),
+                       ("decoder", "dec4", (d5, c4), d4), ("decoder", "dec3", (d4, c3), d3),
+                       ("decoder", "dec2", (d3, c2), d2)]
+        # dec1 = ConvRelu(32 + 64, 32) over cat[dec2, conv1]
+        d1 = self._classifier(d2, c1, net.dec1, label=True, side=True)
+        self.units.append(("decoder", "dec1", (d2, c1), d1))
+
+    def _input_unit(self, conv, tag):
+        """encoder.0 = Conv2d(3, 64, 3, padding 1) + ReLU on the full-resolution image: im2col (27 of 32 columns) + a
+        1x1 GEMM with bias and ReLU; the weight gradient is the 1x1 wgrad, unpacked into the master slot"""
+        net, n, h, w = self.net, self.n, self.h, self.w
+        F = self.fwd_ops
+        cout = conv.out_channels
+        col = self.act(n, h, w, 32)
+        w16 = torch.zeros((1, cout, 32), dtype=BF16, device=self.dev)
+        self._keep.append(w16)
+        master = net._vec(conv.weight, net._p32)
+        b = net._vec(conv.bias, net._p32)
+        y = self.act(n, h, w, cout)
+        fl = 2.0 * n * h * w * cout * 27     # the real 27-wide reduction, as the reference counts it
+        desc = "3->%d k3 (im2col) @%dx%dx%d" % (cout, n, h, w)
+        F.add("im2col", lambda: ops.vgg_input_im2col(self.x_in, col), 0, _nb(self.x_in, col))
+        F.add("misc", lambda: ops.vgg_input_pack_weight(master, w16))
+        F.add("conv_fwd", lambda: ops.conv_fwd(col, w16, 1, 1, bias=b, relu=True, out=y), fl, _nb(col, y), desc)
+        self.bias_sum[id(y)] = net._vec(conv.bias, net._g32)
+
+        def build_input(B):
+            g = self.gbuf(y)       # complete, masked, bias gradient summed (by its consumer)
+            gw = torch.zeros((1, cout, 32), dtype=F32, device=self.dev)
+            self._keep.append(gw)
+            g_slot = net._vec(conv.weight, net._g32)
+            B.add("misc", lambda: L.zero(gw))
+            # on the main stream, in order with the zeroing and the unpack (like the ResNet stem)
+            B.add("conv_wgrad", lambda: ops.conv_wgrad(g, col, gw, 1, 1), fl, _nb(g, col))
+            B.add("misc", lambda: ops.vgg_input_unpack_wgrad(gw, g_slot))
+        self.on_backward(tag, build_input)
+        return y
+
+    def _unit(self, x, conv, tag):
+        """y = relu(conv3x3(x) + b).  x is a pool output (gradient stored plainly) or the previous unit's output (its
+        ReLU mask and bias gradient fused into this unit's dgrad epilogue)"""
+        net = self.net
+        n, h, w, cin = x.shape
+        cout = conv.out_channels
+        w16 = net._packed(conv.weight, net._w16)
+        b = net._vec(conv.bias, net._p32)
+        y = self.act(n, h, w, cout)
+        fl = 2.0 * y.numel() * cin * 9
+        desc = _conv_desc(x, cout, 3, 1)
+        self.fwd_ops.add("conv_fwd", lambda: ops.conv_fwd(x, w16, 3, 1, bias=b, relu=True, out=y), fl, _nb(x, w16, y),
+                         desc)
+        x_is_unit = id(x) in self.bias_sum
+        self.bias_sum[id(y)] = net._vec(conv.bias, net._g32)
+
+        def build_unit(B):
+            g = self.gbuf(y)
+            gw = net._packed(conv.weight, net._g32)
+            B.add("conv_wgrad", lambda: ops.conv_wgrad(g, x, gw, 3, 1), fl, _nb(g, x, gw), desc, side=True)
+            self.dgrad_into(B, g, conv, x, relu_mask=x if x_is_unit else None)
+        self.on_backward(tag, build_unit)
+        return y
+
+    def _pool(self, y, tag):
+        """2x2 max-pool of a stage output y; its backward completes grad(y) (see the class docstring)"""
+        n, h, w, c = y.shape
+        p = self.act(n, h // 2, w // 2, c)
+        self.fwd_ops.add("maxpool", lambda: ops.maxpool2_fwd(y, p), 0, _nb(y, p))
+        gb = self.bias_sum[id(y)]
+
+        def build_pool(B):
+            if id(y) not in self.written:
+                raise RuntimeError("plan error: the skip gradient of a VGG stage output must be stored first")
+            d_p, g = self.gbuf(p), self.gbuf(y)
+            self.bias_fused.add(id(y))
+            B.add("maxpool", lambda: ops.maxpool2_bwd_skip_relu(y, d_p, g, gb), 0, _nb(y, d_p, g, g))
+        self.on_backward(tag, build_pool)
+        return p
 
 
 BN_MOMENTUM = 0.1

@@ -20,6 +20,7 @@ import torchvision
 from torch import nn
 
 from . import ops
+from .engine import ResNetPlan, VGGPlan
 
 BN_MOMENTUM = 0.1
 BN_EPS = 1e-5
@@ -68,8 +69,8 @@ class _Slot:
 class _ArenaUNet(nn.Module):
     """What every U-Net of the H100 path shares: the fp32 parameter arena whose views the nn.Parameters are, the
     gradient and bf16 operand arenas, device moves, state_dict, the cached launch plans and forward.  A subclass builds
-    the reference's module tree, then calls _init_arenas(); engine.Plan reads `plan_kind` to pick the launch plan."""
-    plan_kind = "resnet"
+    the reference's module tree, then calls _init_arenas(); `plan_class` is the engine's launch-plan builder for it."""
+    plan_class = ResNetPlan
     _arch = "UNet"           # name in error messages
     _size_multiple = 64      # H and W must be multiples of this (the reference's torch.cat fails otherwise)
 
@@ -197,8 +198,7 @@ class _ArenaUNet(nn.Module):
         key = (n, h, w, bool(training))
         pl = self._plans.get(key)
         if pl is None:
-            from .engine import Plan
-            pl = Plan(self, n, h, w, bool(training))
+            pl = self.plan_class(self, n, h, w, bool(training))
             self._plans[key] = pl
         return pl
 
@@ -272,8 +272,8 @@ class AlbuNet(UNetResNet):
 class _VGGUNet(_ArenaUNet):
     """VGG-encoder U-Nets: every conv is conv + bias + ReLU (no BatchNorm), five 2x2 max-pools, and every pooled
     stage output also feeds a decoder concat.  `_stages` lists the encoder (torchvision vgg.features) indices of each
-    stage's convs; engine.Plan builds the VGG launch plan from it."""
-    plan_kind = "vgg"
+    stage's convs; engine.VGGPlan builds the launch plan from it."""
+    plan_class = VGGPlan
     _size_multiple = 32
     _stages = ()
 

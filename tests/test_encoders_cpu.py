@@ -142,7 +142,6 @@ def test_albunet_plan_flops_equal_the_hooked_reference(plans, gold):
 
 
 def test_albunet_backward_segments_tile_the_arena(plans):
-    from mcb200.engine import _SIDE_KINDS
     net, pa, _ = plans
     segs = pa.bwd_segments()
     total = net._p32.numel()
@@ -154,7 +153,7 @@ def test_albunet_backward_segments_tile_the_arena(plans):
         lo = net._slots[id(p)].off
         hi = lo + p.numel()
         assert any(b0 <= lo and hi <= b1 for b0, b1 in zip(bounds, bounds[1:])), (lo, hi)
-    side = [o for o in _bwd_ops(pa) if o.kind in _SIDE_KINDS and o.desc]
+    side = [o for o in _bwd_ops(pa) if o.side]
     assert side and all(o.kind in ("conv_wgrad", "convt_wgrad") and o.flops > 0 for o in side)
 
 

@@ -162,7 +162,6 @@ def test_plan_op_counts_match_the_modules(plans, tag):
 
 @pytest.mark.parametrize("tag", CASES)
 def test_backward_segments_tile_the_arena(plans, tag):
-    from mcb200.engine import _SIDE_KINDS
     net, pt, _ = plans[tag]
     segs = pt.bwd_segments()
     total = net._p32.numel()
@@ -179,7 +178,7 @@ def test_backward_segments_tile_the_arena(plans, tag):
     tags = pt.bwd_tags
     assert set(tags[segs[0][0]:segs[0][1]]) == {"decoder"}
     assert set(tags[segs[1][0]:segs[1][1]]) == {"conv5"} and set(tags[segs[2][0]:segs[2][1]]) == {"conv4"}
-    side = [o for o in _bwd_ops(pt) if o.kind in _SIDE_KINDS and o.desc]
+    side = [o for o in _bwd_ops(pt) if o.side]
     assert side and all(o.kind in ("conv_wgrad", "convt_wgrad") and o.flops > 0 for o in side)
 
 

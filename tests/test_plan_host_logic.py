@@ -56,11 +56,11 @@ def test_launch_inventory_resnet101(net101, plan101):
 
 
 def test_side_stream_candidates_are_leaves(plan101):
-    """launches moved to the side stream must only write weight gradients: they are exactly the described wgrad GEMMs"""
-    from mcb200.engine import _SIDE_KINDS
-    side = [o for o in _bwd_ops(plan101) if o.kind in _SIDE_KINDS and o.desc]
-    assert len(side) == 115 + 6 - 2          # all but the stem's and dec0's (whose results are post-processed in order)
-    assert all(o.flops > 0 for o in side)
+    """launches moved to the side stream must only write weight gradients: they are weight-gradient GEMMs"""
+    side = [o for o in _bwd_ops(plan101) if o.side]
+    # all but the stem's (post-processed in order by stem_unpack_wgrad) and dec0's (kept on the main stream)
+    assert len(side) == 115 + 6 - 2
+    assert all(o.kind in ("conv_wgrad", "convt_wgrad") and o.flops > 0 for o in side)
 
 
 def test_backward_layers_run_in_reverse_forward_order(plan101):
