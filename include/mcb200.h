@@ -202,6 +202,10 @@ int mcb_bn_bwd_apply_global(const void* dy, const void* y_mask, const void* z, c
                             int g_accumulate, long pixels, long stat_count, int c, void* stream);
 /* out[c] += sum over pixels of x[.., c]  (conv bias gradients) */
 int mcb_channel_sum(const void* x, float* out, long pixels, int c, void* stream);
+/* the fixed-order sum that finishes every cross-CTA reduction of the library (csrc/detsum.cuh), over rows the caller
+ * provides: out[(i / inner) * out_stride + i % inner] += sum over r < nrows of rows[r * row_stride + i], i < n */
+int mcb_det_sum_f32(const float* rows, int nrows, long row_stride, long n, long inner, float* out, long out_stride,
+                    void* stream);
 
 /* nn.MaxPool2d(2, 2) (src/unet_models.py:356,363,392); backward routes to the first maximum like torch */
 int mcb_maxpool2_fwd(const void* x, void* y, int n, int h, int w, int c, void* stream);

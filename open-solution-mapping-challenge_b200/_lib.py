@@ -97,6 +97,7 @@ _SIGS = {
     "mcb_bn_bwd_apply": [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, cl, ci, vp],
     "mcb_bn_bwd_apply_global": [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, cl, cl, ci, vp],
     "mcb_channel_sum": [vp, vp, cl, ci, vp],
+    "mcb_det_sum_f32": [vp, ci, cl, cl, cl, vp, cl, vp],
     "mcb_maxpool2_fwd": [vp, vp, ci, ci, ci, ci, vp],
     "mcb_maxpool2_bwd": [vp, vp, vp, ci, ci, ci, ci, ci, vp],
     "mcb_final_conv_fwd": [vp, vp, vp, vp, ci, ci, ci, ci, ci, vp],

@@ -120,13 +120,13 @@ static int launch_conv(int BN, int BK, bool b_mn, ConvGemmParams& p, int m_tiles
   // per-channel sums of the CTAs' rows, in CTA order (detsum.cuh)
   const int rows = (int)grid.x;
   if (p.aux_mode == 0) {
-    conv_red_finish_kernel<<<det_finish_grid(2L * nch), kDetFinishThreads, 0, st>>>(
+    conv_red_finish_kernel<<<det_finish_grid(2L * nch, rows), kDetFinishThreads, 0, st>>>(
         0L, rows, (long)p.red_stride, 2L * nch, (long)nch, p.stats + p.n_off, (long)p.stats_c);
   } else {
-    conv_red_finish_kernel<<<det_finish_grid(nch), kDetFinishThreads, 0, st>>>(
+    conv_red_finish_kernel<<<det_finish_grid(nch, rows), kDetFinishThreads, 0, st>>>(
         0L, rows, (long)p.red_stride, (long)nch, (long)nch, p.bn_dbeta + p.n_off, 0L);
     if (p.aux_mode == 2)
-      conv_red_finish_kernel<<<det_finish_grid(nch), kDetFinishThreads, 0, st>>>(
+      conv_red_finish_kernel<<<det_finish_grid(nch, rows), kDetFinishThreads, 0, st>>>(
           (long)nch, rows, (long)p.red_stride, (long)nch, (long)nch, p.bn_dgamma + p.n_off, 0L);
   }
   MCB_LAUNCH_CHECK();
@@ -362,7 +362,7 @@ static int launch_wgrad(WgradParams& p, int cin_src, cudaStream_t st) {
   if (r || splits == 1) return r;
   // the splits that own pixel tiles, summed in split order into dW[tap][cout][ci_off + ci] (detsum.cuh)
   const int rows = (p.tiles_total + per - 1) / per;
-  wgrad_red_finish_kernel<<<det_finish_grid(p.slice), kDetFinishThreads, 0, st>>>(
+  wgrad_red_finish_kernel<<<det_finish_grid(p.slice, rows), kDetFinishThreads, 0, st>>>(
       p.ws_off, rows, p.slice, p.slice, (long)cin_src, p.dw + p.ci_off, (long)p.cin_total);
   MCB_LAUNCH_CHECK();
   return MCB_OK;

@@ -918,6 +918,20 @@ static int reduce_cfg(int c, int* threads, int* c8) {
   if (*threads < *c8) *threads = *c8;
   return MCB_OK;
 }
+__global__ void __launch_bounds__(kDetFinishThreads) det_sum_f32_kernel(const float* rows, int nrows, long row_stride,
+                                                                        long n, long inner, float* out, long out_stride) {
+  det_finish_body<float>(rows, nrows, row_stride, n, inner, out, out_stride);
+}
+extern "C" int mcb_det_sum_f32(const float* rows, int nrows, long row_stride, long n, long inner, float* out,
+                               long out_stride, void* stream) {
+  MCB_REQUIRE(rows && out, "det_sum: null pointer");
+  MCB_REQUIRE(nrows >= 1 && n >= 1 && inner >= 1 && row_stride >= n, "det_sum: %d rows, stride %ld, n %ld, inner %ld",
+              nrows, row_stride, n, inner);
+  det_sum_f32_kernel<<<det_finish_grid(n, nrows), kDetFinishThreads, 0, ST>>>(rows, nrows, row_stride, n, inner, out,
+                                                                         out_stride);
+  MCB_LAUNCH_CHECK();
+  return MCB_OK;
+}
 extern "C" int mcb_channel_sum(const void* x, float* out, long pixels, int c, void* stream) {
   MCB_REQUIRE(x && out, "channel_sum: null pointer");
   int threads, c8;
@@ -927,7 +941,7 @@ extern "C" int mcb_channel_sum(const void* x, float* out, long pixels, int c, vo
   MCB_REQUIRE((long)grid * 2 * c <= kChannelRedCap, "channel_sum: %d blocks x %d channels exceed the workspace", grid, c);
   channel_reduce_kernel<0><<<grid, threads, (size_t)threads * 8 * 2 * sizeof(float), ST>>>(
       (const uint4*)x, nullptr, nullptr, nullptr, nullptr, out, nullptr, pixels, c8);
-  channel_red_finish_kernel<<<det_finish_grid(c), kDetFinishThreads, 0, ST>>>(
+  channel_red_finish_kernel<<<det_finish_grid(c, grid), kDetFinishThreads, 0, ST>>>(
       0L, grid, 2L * c, (long)c, (long)c, out, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
@@ -942,9 +956,9 @@ extern "C" int mcb_bn_bwd_reduce(const void* dy, const void* y_mask, const void*
   MCB_REQUIRE((long)grid * 2 * c <= kChannelRedCap, "bn_bwd_reduce: %d blocks x %d channels exceed the workspace", grid, c);
   channel_reduce_kernel<1><<<grid, threads, (size_t)threads * 8 * 2 * sizeof(float), ST>>>(
       (const uint4*)dy, (const uint4*)y_mask, (const uint4*)z, mean, invstd, dbeta, dgamma, pixels, c8);
-  channel_red_finish_kernel<<<det_finish_grid(c), kDetFinishThreads, 0, ST>>>(
+  channel_red_finish_kernel<<<det_finish_grid(c, grid), kDetFinishThreads, 0, ST>>>(
       0L, grid, 2L * c, (long)c, (long)c, dbeta, 0L);
-  channel_red_finish_kernel<<<det_finish_grid(c), kDetFinishThreads, 0, ST>>>(
+  channel_red_finish_kernel<<<det_finish_grid(c, grid), kDetFinishThreads, 0, ST>>>(
       (long)c, grid, 2L * c, (long)c, (long)c, dgamma, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
@@ -1014,7 +1028,7 @@ extern "C" int mcb_maxpool2_bwd_skip_relu(const void* y, const void* dpool, void
               grid, c);
   maxpool2_bwd_skip_relu_kernel<<<grid, threads, (size_t)threads * 8 * sizeof(float), ST>>>(
       (const uint4*)y, (const uint4*)dpool, (uint4*)g, pooled, h, w, c8);
-  channel_red_finish_kernel<<<det_finish_grid(c), kDetFinishThreads, 0, ST>>>(
+  channel_red_finish_kernel<<<det_finish_grid(c, grid), kDetFinishThreads, 0, ST>>>(
       0L, grid, (long)c, (long)c, (long)c, db, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
@@ -1039,9 +1053,9 @@ extern "C" int mcb_final_conv_bwd(const void* x, const float* w, const float* dl
   MCB_REQUIRE((long)grid * n_acc <= kFinalRedCap, "final_conv_bwd: %d blocks exceed the workspace", grid);
   final_conv_bwd_kernel<<<grid, 128, (size_t)(k * c + 4 * n_acc) * sizeof(float), ST>>>(
       (const uint4*)x, w, dlogits, (uint4*)dx, dw, db, ppi, pixels, c, k);
-  final_red_finish_kernel<<<det_finish_grid(k * c), kDetFinishThreads, 0, ST>>>(
+  final_red_finish_kernel<<<det_finish_grid(k * c, grid), kDetFinishThreads, 0, ST>>>(
       0L, grid, (long)n_acc, (long)(k * c), (long)(k * c), dw, 0L);
-  final_red_finish_kernel<<<det_finish_grid(k), kDetFinishThreads, 0, ST>>>(
+  final_red_finish_kernel<<<det_finish_grid(k, grid), kDetFinishThreads, 0, ST>>>(
       (long)(k * c), grid, (long)n_acc, (long)k, (long)k, db, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;

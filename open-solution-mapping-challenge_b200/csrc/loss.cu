@@ -189,7 +189,7 @@ extern "C" int mcb_loss_partials(const mcb_loss_args* a, double* sums, void* str
   MCB_REQUIRE((long)grid * 4 <= kLossRedCap, "loss_partials: %d blocks exceed the workspace", grid);
   (sigmoid_dice(a) ? loss_partials_kernel<true> : loss_partials_kernel<false>)<<<grid, 256, 0,
       static_cast<cudaStream_t>(stream)>>>(a->logits, a->target, make_cfg(a), sums, ppi, pixels, a->mode == 0 ? 3 : 1);
-  loss_red_finish_kernel<<<det_finish_grid(4), kDetFinishThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+  loss_red_finish_kernel<<<det_finish_grid(4, grid), kDetFinishThreads, 0, static_cast<cudaStream_t>(stream)>>>(
       0L, grid, 4L, 4L, 4L, sums, 0L);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
