@@ -385,6 +385,33 @@ int mcb_size_matrix(const int* labels, const int* area, long long* out, int h, i
  * {mask, uint8(uint16(dist)), uint8(uint16(sqrt(uint16(sizes))))}, padded like the image */
 int mcb_target_channels(const uint8_t* mask, const void* dist_f16, const long long* sizes, float* out, int n, int h, int w,
                         int pad_h, int pad_w, int pad_mode, void* stream);
+/* the target tensor from augmented uint8 planes (src/loaders.py:159-165: to_pil, to_monochrome, to_tensor, cat):
+ * planes uint8 [n][h][w][c] (c = 3: mask, distances, sizes; c = 1: mask) -> fp32 [n][c][h + 2 pad_h][w + 2 pad_w],
+ * padded like the image (padding_seq of the crop-and-pad validation loaders) */
+int mcb_target_channels_u8(const uint8_t* planes, float* out, int n, int h, int w, int c, int pad_h, int pad_w,
+                           int pad_mode, void* stream);
+
+/* one sample of the training augmentation: fast_seq (src/augmentation.py:5-10) and crop_seq's RandomCropFixedSize
+ * (:34-37, :91-135), one deterministic draw applied to every array of the sample (ImgAug,
+ * src/steps/pytorch/utils.py:108-129).  Flip bits: 1 = Fliplr, 2 = Flipud. */
+typedef struct {
+  double inv[9];   /* output (x, y) -> input (column, row) map of skimage warp: np.linalg.inv of the Affine matrix */
+  int warp;        /* 0: the sample is not warped (no Affine child drawn); 1: warp through inv */
+  int pre_flip;    /* flips drawn before the Affine child */
+  int post_flip;   /* flips drawn after it (all flips when warp = 0) */
+  int top, left;   /* crop offset (0, 0 in resize mode) */
+  int reserved;
+} mcb_augment_row;
+/* the augmenters of the training loaders (src/loaders.py:140-159, 236-237, 261, 277-278, 302) for a batch:
+ * img uint8 [n][h][w][3], mask uint8 [n][h][w], dist / size uint16 [n][h][w] (both or neither: the distance loaders'
+ * Di / Si after their astype casts) -> img_out uint8 [n][out_h][out_w][3], tgt_out uint8 [n][out_h][out_w][c]
+ * (c = 3: mask, distances, sizes; c = 1 without dist / size), every pixel cropped, flipped and warped like
+ * imgaug 0.2.5's Affine over skimage.transform.warp (order 1, constant 0, fp64, clipped to each array's input range,
+ * truncated to its dtype), uint16 planes then wrapped to uint8 like to_pil (src/utils.py:284-289).
+ * rows: HOST array [n] (checked, then passed to the kernels by value); range_ws uint32 [n][8] workspace. */
+int mcb_augment_warp(const uint8_t* img, const uint8_t* mask, const uint16_t* dist, const uint16_t* size,
+                     const mcb_augment_row* rows, int n, int h, int w, int out_h, int out_w, unsigned* range_ws,
+                     uint8_t* img_out, uint8_t* tgt_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Synchronised BatchNorm over NVLink peer memory (SURVEY.md 8e collective (2)): one-shot all-reduce of a small fp32

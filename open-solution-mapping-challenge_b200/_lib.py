@@ -195,6 +195,8 @@ _SIGS5 = {
     "mcb_pil_resize_bilinear_u8": [vp, vp, vp, vp, vp, ci, vp, vp, ci, ci, ci, ci, ci, ci, ci, vp],
     "mcb_size_matrix": [vp, vp, vp, ci, ci, vp],
     "mcb_target_channels": [vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp],
+    "mcb_target_channels_u8": [vp, vp, ci, ci, ci, ci, ci, ci, ci, vp],
+    "mcb_augment_warp": [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp],
 }
 for _n, _a in _SIGS5.items():
     getattr(lib, _n).argtypes = _a

@@ -157,6 +157,15 @@ __global__ void size_matrix_kernel(const int* __restrict__ labels, const int* __
     out[q] = l > 0 ? (long long)area[l - 1] : 1ll;
   }
 }
+// source pixel (within image n of H x W) of padded target pixel q of a Ho x Wo plane
+__device__ __forceinline__ long target_src(long q, int n, int H, int W, int ph, int pw, int mode) {
+  const int Wo = W + 2 * pw;
+  const int y = q / Wo, x = q % Wo;
+  return (long)n * H * W + (long)pad_src(y - ph, H, mode) * W + pad_src(x - pw, W, mode);
+}
+// one target value: a uint8 'L' plane through to_monochrome + to_tensor (src/loaders.py:520-529) is its byte as float32
+__device__ __forceinline__ void store_target_u8(float* dst, long q, uint8_t v) { dst[q] = (float)v; }
+
 // MetadataImageSegmentationDatasetDistances.__getitem__ (src/loaders.py:141-171) without the random augmentation:
 //   M = mask image -> convert('L') -> float32;  D = distances.astype(uint16) -> uint8 (to_pil) -> float32;
 //   S = sizes.astype(uint16) -> sqrt -> uint16 -> uint8 (to_pil) -> float32;  target = cat(M, D, S)
@@ -166,18 +175,29 @@ __global__ void target_channels_kernel(const uint8_t* __restrict__ mask, const _
                                        int pw, int mode) {
   const int n = blockIdx.y;
   const int Ho = H + 2 * ph, Wo = W + 2 * pw;
-  const long plane = (long)Ho * Wo, hw = (long)H * W;
+  const long plane = (long)Ho * Wo;
   float* dst = out + (long)n * 3 * plane;
   for (long q = blockIdx.x * (long)blockDim.x + threadIdx.x; q < plane; q += (long)gridDim.x * blockDim.x) {
-    const int y = q / Wo, x = q % Wo;
-    const long p = (long)n * hw + (long)pad_src(y - ph, H, mode) * W + pad_src(x - pw, W, mode);
-    dst[q] = (float)mask[p];
+    const long p = target_src(q, n, H, W, ph, pw, mode);
+    store_target_u8(dst, q, mask[p]);
     const float df = __half2float(dist[p]);                               // numpy float16 -> uint16: truncation
     const unsigned d16 = (unsigned)(unsigned short)(long long)df;
-    dst[plane + q] = (float)(d16 & 0xFFu);
+    store_target_u8(dst + plane, q, (uint8_t)(d16 & 0xFFu));
     const unsigned s16 = (unsigned)(unsigned short)sizes[p];
     const unsigned r16 = (unsigned)(unsigned short)__fsqrt_rn((float)s16);   // np.sqrt of a uint16 array is float32
-    dst[2 * plane + q] = (float)(r16 & 0xFFu);
+    store_target_u8(dst + 2 * plane, q, (uint8_t)(r16 & 0xFFu));
+  }
+}
+// the same target from planes that already went through the casts and to_pil (csrc/augment.cu):
+// planes uint8 [n][H][W][C] -> out fp32 [n][C][Ho][Wo]
+__global__ void target_channels_u8_kernel(const uint8_t* __restrict__ planes, float* __restrict__ out, int H, int W,
+                                          int C, int ph, int pw, int mode) {
+  const int n = blockIdx.y;
+  const long plane = (long)(H + 2 * ph) * (W + 2 * pw);
+  float* dst = out + (long)n * C * plane;
+  for (long q = blockIdx.x * (long)blockDim.x + threadIdx.x; q < plane; q += (long)gridDim.x * blockDim.x) {
+    const long p = target_src(q, n, H, W, ph, pw, mode);
+    for (int c = 0; c < C; ++c) store_target_u8(dst + c * plane, q, planes[p * C + c]);
   }
 }
 
@@ -246,6 +266,18 @@ extern "C" int mcb_target_channels(const uint8_t* mask, const void* dist_f16, co
   MCB_REQUIRE(pad_h >= 0 && pad_w >= 0 && pad_h < h && pad_w < w && (pad_mode == 0 || pad_mode == 1), "target_channels: bad padding");
   target_channels_kernel<<<grid_in((long)(h + 2 * pad_h) * (w + 2 * pad_w), n, 256), 256, 0, ST>>>(
       mask, (const __half*)dist_f16, sizes, out, h, w, pad_h, pad_w, pad_mode);
+  MCB_LAUNCH_CHECK();
+  return MCB_OK;
+}
+
+extern "C" int mcb_target_channels_u8(const uint8_t* planes, float* out, int n, int h, int w, int c, int pad_h, int pad_w,
+                                      int pad_mode, void* stream) {
+  MCB_REQUIRE(planes && out, "target_channels_u8: null pointer");
+  MCB_REQUIRE(n > 0 && h > 0 && w > 0 && (c == 1 || c == 3), "target_channels_u8: bad shape");
+  MCB_REQUIRE(pad_h >= 0 && pad_w >= 0 && pad_h < h && pad_w < w && (pad_mode == 0 || pad_mode == 1),
+              "target_channels_u8: bad padding");
+  target_channels_u8_kernel<<<grid_in((long)(h + 2 * pad_h) * (w + 2 * pad_w), n, 256), 256, 0, ST>>>(
+      planes, out, h, w, c, pad_h, pad_w, pad_mode);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }

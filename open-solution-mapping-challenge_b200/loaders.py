@@ -9,6 +9,10 @@ thread pool.  Here the variants are index maps: one kernel writes the 16 views o
 device batch, and ONE kernel undoes the maps, takes the class softmax of the raw logits and reduces
 (gmean / mean / max / min) without materialising any inverse-transformed prediction (csrc/instances.cu).
 
+The training loaders of src/loaders.py:225-305 (MetadataImageSegmentationLoader[Distances]{Resize,CropPad}) are at the
+bottom: DataLoader workers only decode files, the augmentation and the tensor assembly run on the device
+(mcb200.augmentation).
+
 Assumption (skimage is not installable here, SURVEY.md 8c): `skimage.transform.rotate(image, angle,
 preserve_range=True)` at angle in {0, 90, 180, 270} on a square image is the exact quarter-turn index permutation
 (np.rot90, counter-clockwise).  Colour-shift variants (imgaug, random) are out of scope and rejected.
@@ -164,3 +168,161 @@ class TestTimeAugmentationAggregator:
                            torch.float32)
         out = aggregate_batch(pred, tta_params, img_ids, self.method).cpu().numpy()
         return {'aggregated_prediction': [a for a in out]}
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# training loaders (src/loaders.py:114-305) with the augmentation on the device
+# ---------------------------------------------------------------------------------------------------------------------
+def load_mask(filepath):
+    """the mask of src/loaders.py:145-146 (Image.open(...).convert('RGB')) as its single band: the masks are 0/1
+    grayscale PNGs, so the RGB image has three equal bands and to_monochrome gives any one of them back"""
+    from PIL import Image
+    im = Image.open(filepath, 'r')
+    if im.mode == 'L':
+        return np.array(im)
+    rgb = np.array(im.convert('RGB'))
+    if not ((rgb[..., 0] == rgb[..., 1]).all() and (rgb[..., 0] == rgb[..., 2]).all()):
+        raise ValueError("%s: mask bands differ; the device path carries one mask plane" % filepath)
+    return np.ascontiguousarray(rgb[..., 0])
+
+
+class SegmentationFiles(torch.utils.data.Dataset):
+    """what the DataLoader workers do per sample: decode the files and apply the reference's own numpy casts
+    (src/loaders.py:140-154).  Returns (image uint8 (H, W, 3)[, mask uint8 (H, W)[, distances, sizes]]), the uint16
+    distances / sizes as their int16 view (same bytes; collated and pinned like any int16 tensor)."""
+
+    def __init__(self, X, y=None, distances=False):
+        self.X, self.y, self.distances = X, y, distances
+
+    def __len__(self):
+        return len(self.X)
+
+    def __getitem__(self, index):
+        import os
+        from PIL import Image
+        Xi = np.array(Image.open(self.X[index], 'r').convert('RGB'))
+        if self.y is None:
+            return Xi
+        mask_filepath = self.y[index]
+        Mi = load_mask(mask_filepath)
+        if not self.distances:
+            return Xi, Mi
+        import joblib
+        distance_filepath = os.path.splitext(mask_filepath.replace("/masks/", "/distances/"))[0]
+        size_filepath = distance_filepath.replace("/distances/", "/sizes/")
+        Di = joblib.load(distance_filepath).astype(np.uint16)
+        Si = np.sqrt(joblib.load(size_filepath).astype(np.uint16)).astype(np.uint16)
+        return Xi, Mi, Di.view(np.int16), Si.view(np.int16)
+
+
+class DeviceBatches:
+    """iterable over a DataLoader of host batches: draws each batch's augmentation parameters, runs the device chain
+    (csrc/augment.cu -> [Pillow resize] -> normalise / pad + target) and yields [X, target] cuda float32 tensors
+    (X alone without targets).  `last_params` holds the draw of the batch last yielded."""
+
+    def __init__(self, loader, seq, rng, resize=None, pad=(0, 0)):
+        self.loader, self.seq, self.rng, self.resize, self.pad = loader, seq, rng, resize, pad
+        self.last_params = None
+
+    def __len__(self):
+        return len(self.loader)
+
+    def __iter__(self):
+        from .augmentation import batch_chain, identity_params
+        from .preparation import image_transform_batch, pil_resize_batch
+        for batch in self.loader:
+            if isinstance(batch, torch.Tensor):                     # images only (inference)
+                x = batch.to(_dev(), non_blocking=batch.is_pinned())
+                if self.resize is not None:
+                    x = pil_resize_batch(x, self.resize)
+                yield image_transform_batch(x, self.pad)
+                continue
+            images, masks = batch[0], batch[1]
+            distances, sizes = (batch[2], batch[3]) if len(batch) == 4 else (None, None)
+            n, h, w = images.shape[:3]
+            params = self.seq.draw(self.rng, n, h, w) if self.seq is not None else identity_params(n)
+            self.last_params = params
+            yield list(batch_chain(images, masks, distances, sizes, params,
+                                   crop_size=None if self.seq is None else self.seq.crop_size, resize=self.resize,
+                                   pad=self.pad))
+
+
+class _AugmentedLoader:
+    """ImageSegmentationLoaderBasic (src/loaders.py:176-222): transform(X, y, X_valid, y_valid, train_mode) ->
+    {'datagen': (flow, steps), 'validation_datagen': (flow, steps)}.  `seed` (optional) makes the augmentation draws
+    and the DataLoader's shuffling reproducible; under torch.distributed it is offset by the rank."""
+    distances = False
+    crop = False
+
+    def __init__(self, loader_params, dataset_params, seed=None):
+        self.loader_params = loader_params
+        self.dataset_params = dataset_params
+        self.seed = seed
+
+    def fit(self, *args, **kwargs):
+        return self
+
+    def fit_transform(self, *args, **kwargs):
+        return self.transform(*args, **kwargs)
+
+    def load(self, filepath):
+        return self
+
+    def save(self, filepath):
+        import joblib
+        joblib.dump({}, filepath)
+
+    def transform(self, X, y=None, X_valid=None, y_valid=None, train_mode=True):
+        if train_mode and y is not None:
+            flow, steps = self.get_datagen(X, y, True, self.loader_params['training'])
+        else:
+            flow, steps = self.get_datagen(X, None, False, self.loader_params['inference'])
+        if X_valid is not None and y_valid is not None:
+            valid_flow, valid_steps = self.get_datagen(X_valid, y_valid, False, self.loader_params['inference'])
+        else:
+            valid_flow, valid_steps = None, None
+        return {'datagen': (flow, steps), 'validation_datagen': (valid_flow, valid_steps)}
+
+    def _seed(self):
+        if self.seed is None:
+            return None
+        import torch.distributed as dist
+        rank = dist.get_rank() if dist.is_available() and dist.is_initialized() else 0
+        return int(self.seed) + rank
+
+    def get_datagen(self, X, y, train_mode, loader_params):
+        from .augmentation import crop_seq, fast_seq
+        seed = self._seed()
+        kwargs = dict(loader_params)
+        if seed is not None and kwargs.get('shuffle'):
+            kwargs['generator'] = torch.Generator().manual_seed(seed)
+        loader = torch.utils.data.DataLoader(SegmentationFiles(X, y, self.distances), **kwargs)
+        dp = self.dataset_params
+        h, w = int(dp['h']), int(dp['w'])
+        if self.crop:
+            seq = crop_seq((h, w)) if train_mode else None
+            flow = DeviceBatches(loader, seq, np.random.default_rng(seed), None,
+                                 (0, 0) if train_mode else (int(dp['h_pad']), int(dp['w_pad'])))
+        else:
+            flow = DeviceBatches(loader, fast_seq if train_mode else None, np.random.default_rng(seed), (h, w))
+        return flow, len(loader)
+
+
+class MetadataImageSegmentationLoaderDistancesCropPad(_AugmentedLoader):
+    """src/loaders.py:225-243"""
+    distances, crop = True, True
+
+
+class MetadataImageSegmentationLoaderDistancesResize(_AugmentedLoader):
+    """src/loaders.py:246-263"""
+    distances, crop = True, False
+
+
+class MetadataImageSegmentationLoaderCropPad(_AugmentedLoader):
+    """src/loaders.py:266-284"""
+    distances, crop = False, True
+
+
+class MetadataImageSegmentationLoaderResize(_AugmentedLoader):
+    """src/loaders.py:287-304"""
+    distances, crop = False, False

@@ -5,8 +5,8 @@ building distances, component-size map).
 
 Both loader modes are covered: `crop_and_pad` (PadFixed) and `resize` (transforms.Resize on the PIL image = Pillow's
 8-bit bilinear resampler, restated bit-exactly).  Out of scope: JPEG / PNG decoding, COCO polygon rasterisation
-(pycocotools), the random imgaug augmenters.  Everything here is batched device work in libmcb200.so (csrc/input.cu); no
-CPU fallback."""
+(pycocotools); the random augmenters of the training loaders are mcb200.augmentation.  Everything here is batched
+device work in libmcb200.so (csrc/input.cu); no CPU fallback."""
 import numpy as np
 import torch
 
