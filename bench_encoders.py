@@ -28,20 +28,32 @@ def plan_flops_per_tile(net, batch, size):
     return (sum(o.flops for o in pl.fwd_ops) + sum(o.flops for layer in pl.bwd_layers for o in layer)) / batch
 
 
-def vgg_fused_step(enc, x_shape, t_shape, dev):
-    """-> (net, step()) for VGG11 / VGG16: the fused train step PyTorchUNetWeighted would run for the registry entry
-    (src/models.py:22-28, 149-161) with bench.unet_config's loss and optimizer settings"""
+def vgg_step_settings(enc):
+    """-> (FusedTrainStep loss config, lr, weight decay) of bench.unet_config(enc), as PyTorchUNetWeighted derives them
+    (src/models.py:149-161)"""
     import bench
-    from mcb200.models import FusedTrainStep, _size_c
-    from mcb200.unet_models import UNet11, UNetVGG16
+    from mcb200.models import _size_c
     a = bench.unet_config(enc)["architecture_config"]
     wce, lw, dice = a["weighted_cross_entropy"], a["loss_weights"], a["dice"]
     cfg = dict(w0=float(wce["w0"]), sigma=float(wce["sigma"]), size_c=_size_c(wce["imsize"]),
                dice_weight=float(lw["dice_mask"]), ce_weight=float(lw["bce_mask"]), dice_smooth=float(dice["smooth"]))
     lr = a["optimizer_params"]["lr"]
     wd = a["regularizer_params"]["weight_decay_conv2d"] if a["regularizer_params"]["regularize"] else 0.0
-    net = UNet11(num_classes=2) if enc == "VGG11" else UNetVGG16(num_classes=2, dropout_2d=0.0, is_deconv=True)
-    net = net.to(dev)
+    return cfg, lr, wd
+
+
+def vgg_net(enc):
+    """UNet11 / UNetVGG16 as the registry entry builds them (src/models.py:22-28)"""
+    from mcb200.unet_models import UNet11, UNetVGG16
+    return UNet11(num_classes=2) if enc == "VGG11" else UNetVGG16(num_classes=2, dropout_2d=0.0, is_deconv=True)
+
+
+def vgg_fused_step(enc, x_shape, t_shape, dev):
+    """-> (net, step()) for VGG11 / VGG16: the fused train step PyTorchUNetWeighted would run for the registry entry
+    (src/models.py:22-28, 149-161) with bench.unet_config's loss and optimizer settings"""
+    from mcb200.models import FusedTrainStep
+    cfg, lr, wd = vgg_step_settings(enc)
+    net = vgg_net(enc).to(dev)
     fused = FusedTrainStep(net, x_shape, t_shape, 0, cfg)
     return net, lambda X, T: fused.step(X, T, lr=lr, weight_decay=wd)
 

@@ -84,6 +84,7 @@ class Plan:
         self._bns = []
         self._bwd_builders = []    # (tag, builder) per forward unit; run in REVERSE so store/accumulate modes follow run order
         self.units = []            # (kind, state_dict prefix, inputs, output) per forward unit, for per-unit parity tests
+        self.dec_mid = {}          # id(decoder block output) -> the block's middle ConvRelu output, for the same tests
         total_c = sum(m.num_features for m in net.modules() if isinstance(m, nn.BatchNorm2d))
         n_bn = sum(1 for m in net.modules() if isinstance(m, nn.BatchNorm2d))
         self._stats_arena = torch.zeros(2 * total_c, dtype=F32, device=self.dev)
@@ -374,6 +375,7 @@ class Plan:
         wt16 = net._packed(deconv.weight, net._w16)
         b2 = net._vec(deconv.bias, net._p32)
         out = self.act(n, 2 * h, 2 * w, cout)
+        self.dec_mid[id(out)] = mid
         self.bias_sum[id(out)] = net._vec(deconv.bias, net._g32)
         ft = 2.0 * mid.numel() * cout * kt * kt
         dd = "%d->%d @%dx%dx%d" % (cmid, cout, n, h, w)
