@@ -428,6 +428,31 @@ int mcb_sync_exchange(const float* partial, void* const* peer_recv, int rank, in
                       int count, const unsigned* step, float* out, float* out2_first, float* out2_second, int split,
                       float scale2, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * COCO segmentation evaluation (src/cocoeval.py, csrc/evaluation.cu)
+ * ---------------------------------------------------------------------------------------------------------------- */
+/* mask IoU of (detection, ground truth) pairs, pycocotools rleIou as src/cocoeval.py:196 calls it
+ * (maskUtils.iou(d, g, iscrowd)): run lists dt_cnts / gt_cnts uint32 (COCO column-major RLE counts), RLE r owning
+ * [starts[r], starts[r + 1]) (int64); gt_crowd uint8 per ground-truth RLE (union = detection area when set).
+ * Pair p (int32 pair_dt / pair_gt, bounding boxes already found to overlap by the caller) writes
+ * iou[pair_out[p]] = i / u (fp64), 0 when the masks do not intersect.  Entries of pairs not listed are the caller's
+ * (zero: pycocotools' bounding-box gate).  One thread per pair. */
+int mcb_rle_pair_iou(const uint32_t* dt_cnts, const long long* dt_starts, const uint32_t* gt_cnts,
+                     const long long* gt_starts, const uint8_t* gt_crowd, const int* pair_dt, const int* pair_gt,
+                     const long long* pair_out, double* iou, int npairs, void* stream);
+/* COCOeval.evaluateImg (src/cocoeval.py:242-320) for every (unit, area range); a unit is one (image, category) with
+ * nd[u] detections (score-ordered, already cut to maxDets[-1]) at dt_off[u] and ng[u] ground truths (file order) at
+ * gt_off[u]; its IoU table is iou[iou_off[u] + d * ng[u] + g].  dt_id int64, dt_area fp64; gt_id int64, gt_crowd uint8
+ * (iscrowd = ignore), gt_area fp64 (the JSON area); area_rng fp64 [A][2] (both bounds inclusive); thr fp64 [T]
+ * (T <= 32).  Outputs: dt_match int64 [A][T][d_total] (matched ground-truth id, 0 = none), dt_ignore uint8
+ * [A][T][d_total], gt_ignore uint8 [A][g_total] (in the stable `_ignore` order); gt_taken uint8 [A][T][g_total] is
+ * workspace, zeroed by the caller.  One warp per (unit, area range), one lane per threshold. */
+int mcb_coco_match(const double* iou, const long long* iou_off, const int* nd, const int* ng, const long long* dt_off,
+                   const long long* dt_id, const double* dt_area, const long long* gt_off, const long long* gt_id,
+                   const uint8_t* gt_crowd, const double* gt_area, const double* area_rng, const double* thr, int units,
+                   int A, int T, long long d_total, long long g_total, long long* dt_match, uint8_t* dt_ignore,
+                   uint8_t* gt_ignore, uint8_t* gt_taken, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -202,6 +202,15 @@ for _n, _a in _SIGS5.items():
     getattr(lib, _n).argtypes = _a
     getattr(lib, _n).restype = ci
 
+_SIGS6 = {
+    "mcb_rle_pair_iou": [vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, vp],
+    "mcb_coco_match": [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, C.c_longlong, C.c_longlong, vp,
+                       vp, vp, vp, vp],
+}
+for _n, _a in _SIGS6.items():
+    getattr(lib, _n).argtypes = _a
+    getattr(lib, _n).restype = ci
+
 lib.mcb_sync_step_bump.argtypes = [vp, vp]
 lib.mcb_sync_step_bump.restype = ci
 lib.mcb_sync_exchange.argtypes = [vp, vp, ci, ci, cl, cl, ci, vp, vp, vp, vp, ci, cf, vp]
