@@ -283,6 +283,10 @@ int mcb_morph_rect(const void* in, void* out, int is_i32, int is_dilation, int s
 /* add_dropped_objects (src/utils.py:333-339), per 2-D plane; workspace int32 [2*planes*h*w] */
 int mcb_add_dropped_objects(const uint8_t* original, const uint8_t* processed, uint8_t* out, int* workspace, int planes,
                             int h, int w, void* stream);
+/* skimage <= 0.17 binary_erosion (ndi.binary_erosion, border_value=True) / binary_dilation with rectangle(size, size)
+ * (src/preparation.py:170-186) on {0,1} uint8 planes; differs from mcb_morph_rect only in an even erosion's centre */
+int mcb_binary_morph_rect(const uint8_t* in, uint8_t* out, int is_dilation, int size, int planes, int h, int w,
+                          void* stream);
 /* build_score (src/postprocessing.py:228-236): scores[offsets[p] + l - 1] = mean(prob[labels == l]) * sqrt(area);
  * offsets int32 [planes] (exclusive prefix of the per-plane label counts); sums/counts/scores sized total_instances */
 int mcb_instance_scores(const int* labels, const void* prob, int prob_is_f64, const int* offsets, double* sums,
@@ -373,13 +377,23 @@ int mcb_pil_resize_bilinear_u8(const uint8_t* in, uint8_t* tmp, uint8_t* out, co
                                int ksize_h, const int* coef_v, const int* bounds_v, int ksize_v, int n, int h, int w,
                                int c, int out_h, int out_w, void* stream);
 /* update_distances + clean_distances (src/preparation.py:151-168): masks uint8 [k][h][w] (one plane per building of ONE
- * image, non-empty); dist_sum fp16 [h][w] = d_nearest + d_second (one building counts twice, none gives 0),
- * second_nearest fp64 [h][w]; distances are scipy.ndimage.distance_transform_edt(1 - mask), exact;
+ * image); dist_sum fp16 [h][w] = d_nearest + d_second (one building counts twice, none gives 0),
+ * second_nearest fp64 [h][w]; distances are scipy.ndimage.distance_transform_edt(1 - mask), exact, including an
+ * empty plane (a building eroded to nothing), for which scipy, with no background pixel, gives sqrt((y + 1)^2 + x^2);
  * workspace int32 [k][h][w] */
 int mcb_edt_two_nearest(const uint8_t* masks, int k, int h, int w, int* workspace, void* dist_sum_f16,
                         double* second_nearest, void* stream);
 /* get_size_matrix (src/preparation.py:189-195): labels int32 [h][w] (mcb_ccl_label), area int32 [labels] -> int64 [h][w] */
+/* the same over n images: image i takes the instances [image_off[i], image_off[i + 1]) of a list whose entry k is plane
+ * plane_index[k] of masks (uint8 [planes][h][w]; identity when plane_index is NULL); plane_stats (NULL, or
+ * mcb_plane_stats of masks) bounds each plane's columns; an empty plane is scipy's all-foreground transform
+ * sqrt((y + 1)^2 + x^2).  workspace int32 [k][h][w]; dist_sum fp16 / second_nearest fp64 [n][h][w] */
+int mcb_edt_two_nearest_batched(const uint8_t* masks, const int* plane_index, const int* image_off,
+                                const int* plane_stats, int k, int n, int h, int w, int* workspace, void* dist_sum_f16,
+                                double* second_nearest, void* stream);
 int mcb_size_matrix(const int* labels, const int* area, long long* out, int h, int w, void* stream);
+/* get_size_matrix of n label planes (mcb_ccl_label numbering per plane); area_ws int32 [n][h][w] workspace */
+int mcb_size_matrix_batched(const int* labels, int* area_ws, long long* out, int n, int h, int w, void* stream);
 /* the target tensor of MetadataImageSegmentationDatasetDistances (src/loaders.py:141-171), deterministic part:
  * mask uint8 [n][h][w], dist fp16 [n][h][w], sizes int64 [n][h][w] -> fp32 [n][3][h + 2 pad_h][w + 2 pad_w] =
  * {mask, uint8(uint16(dist)), uint8(uint16(sqrt(uint16(sizes))))}, padded like the image */
@@ -452,6 +466,31 @@ int mcb_coco_match(const double* iou, const long long* iou_off, const int* nd, c
                    const uint8_t* gt_crowd, const double* gt_area, const double* area_rng, const double* thr, int units,
                    int A, int T, long long d_total, long long g_total, long long* dt_match, uint8_t* dt_ignore,
                    uint8_t* gt_ignore, uint8_t* gt_taken, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * Target preparation from COCO polygons (src/preparation.py:18-198, csrc/polygon.cu)
+ * ---------------------------------------------------------------------------------------------------------------- */
+/* pycocotools maskApi.c rleFrPoly + rleDecode (cocomask.frPyObjects(polys, h, w) then decode), bit-exact.  The host
+ * scales the vertices, (int)(5 x + .5), and passes one row per edge of the closed polygons: edge_xy int32 [edges][4] =
+ * (xs, ys, xe, ye), edge_pt int64 [edges + 1] = first upsampled point of each edge (max(|dx|, |dy|) + 1 per edge,
+ * points = edge_pt[edges]), edge_plane int32 [edges] = the polygon's output plane (consecutive polygons differ).
+ * bits uint32 [planes][ceil(h*w / 32)] workspace; out uint8 [planes][h][w] row-major. */
+int mcb_rasterize_polygons(const int* edge_xy, const long long* edge_pt, const int* edge_plane, int edges,
+                           long long points, uint32_t* bits, uint8_t* out, int planes, int h, int w, void* stream);
+/* per uint8 plane: stats int32 [count][4] = (pixel count, any pixel at least `border` away from every edge
+ * (not is_on_border(m, border), src/preparation.py:197-198), first column, last column with a pixel (w, -1 if none)) */
+int mcb_plane_stats(const uint8_t* planes, int count, int h, int w, int border, int* stats, void* stream);
+/* out[g] = union of the planes index[group_off[g] .. group_off[g + 1]) of `planes`, uint8 {0,1} [groups][h][w] */
+int mcb_plane_union(const uint8_t* planes, const int* index, const int* group_off, int groups, int h, int w,
+                    uint8_t* out, void* stream);
+/* mask_overlayed = np.where(mask_c, category_nr[c], mask_overlayed) over c (src/preparation.py:50-78):
+ * cat_masks uint8 [n][categories][h][w], category_nr int32 [categories] (device) -> out uint8 [n][h][w] */
+int mcb_category_overlay(const uint8_t* cat_masks, const int* category_nr, int categories, int n, int h, int w,
+                         uint8_t* out, void* stream);
+/* the border class (src/preparation.py:83-86) in place: where second_nearest < border_width and the class is even
+ * (numpy's bool & ~uint8), the class becomes the image's max + 1 */
+int mcb_border_class(uint8_t* mask, const double* second_nearest, int n, int h, int w, double border_width,
+                     void* stream);
 
 #ifdef __cplusplus
 }

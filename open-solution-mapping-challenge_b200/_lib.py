@@ -211,6 +211,20 @@ for _n, _a in _SIGS6.items():
     getattr(lib, _n).argtypes = _a
     getattr(lib, _n).restype = ci
 
+_SIGS7 = {
+    "mcb_rasterize_polygons": [vp, vp, vp, ci, C.c_longlong, vp, vp, ci, ci, ci, vp],
+    "mcb_plane_stats": [vp, ci, ci, ci, ci, vp, vp],
+    "mcb_plane_union": [vp, vp, vp, ci, ci, ci, vp, vp],
+    "mcb_category_overlay": [vp, vp, ci, ci, ci, ci, vp, vp],
+    "mcb_border_class": [vp, vp, ci, ci, ci, C.c_double, vp],
+    "mcb_edt_two_nearest_batched": [vp, vp, vp, vp, ci, ci, ci, ci, vp, vp, vp, vp],
+    "mcb_size_matrix_batched": [vp, vp, vp, ci, ci, ci, vp],
+    "mcb_binary_morph_rect": [vp, vp, ci, ci, ci, ci, ci, vp],
+}
+for _n, _a in _SIGS7.items():
+    getattr(lib, _n).argtypes = _a
+    getattr(lib, _n).restype = ci
+
 lib.mcb_sync_step_bump.argtypes = [vp, vp]
 lib.mcb_sync_step_bump.restype = ci
 lib.mcb_sync_exchange.argtypes = [vp, vp, ci, ci, cl, cl, ci, vp, vp, vp, vp, ci, cf, vp]

@@ -91,13 +91,21 @@ __global__ void pil_resize_v_kernel(const uint8_t* __restrict__ tmp, uint8_t* __
 // ------------------------------------------------------------------------------------------ exact EDT, two nearest
 // scipy.ndimage.distance_transform_edt(1 - mask): Euclidean distance of every pixel to the nearest pixel of the
 // instance, sqrt of the exact integer squared distance in float64.
+// Batched over images: image n owns the instances [image_off[n], image_off[n + 1]) of a list whose entry k is plane
+// plane_index[k] of `masks` (identity when plane_index is null; one image of K instances when image_off is null).
+// cols (nullable) holds per plane the first and last column with a pixel at cols[4 p + 2], cols[4 p + 3]
+// (mcb_plane_stats); both passes skip the columns outside, which hold no pixel and so never give the minimum.
+// An empty plane gives what scipy returns for an input without background: sqrt((y + 1)^2 + x^2).
 // Pass 1 (columns): g[k][y][x] = vertical distance to the nearest instance pixel of column x (kInfCol if none).
 constexpr int kInfCol = 1 << 20;
-__global__ void edt_columns_kernel(const uint8_t* __restrict__ masks, int* __restrict__ g, int K, int H, int W) {
+__device__ __forceinline__ int edt_plane(const int* plane_index, int k) { return plane_index ? plane_index[k] : k; }
+__global__ void edt_columns_kernel(const uint8_t* __restrict__ masks, const int* __restrict__ plane_index,
+                                   const int* __restrict__ cols, int* __restrict__ g, int H, int W, int k0) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x;
-  const int k = blockIdx.y;
-  if (x >= W || k >= K) return;
-  const uint8_t* m = masks + (long)k * H * W;
+  const int k = k0 + blockIdx.y;
+  const int p = edt_plane(plane_index, k);
+  if (x >= W || (cols && (x < cols[4 * p + 2] || x > cols[4 * p + 3]))) return;
+  const uint8_t* m = masks + (long)p * H * W;
   int* gk = g + (long)k * H * W;
   int d = kInfCol;
   for (int y = 0; y < H; ++y) {
@@ -110,40 +118,48 @@ __global__ void edt_columns_kernel(const uint8_t* __restrict__ masks, int* __res
     gk[(long)y * W + x] = min(gk[(long)y * W + x], d);
   }
 }
-// Pass 2 (rows) fused with the reduction over instances: one CTA per image row; for each instance the row of g is
-// staged in shared memory and every thread takes min over x' of (x - x')^2 + g^2 (exact int64), keeping the two
+// Pass 2 (rows) fused with the reduction over instances: one CTA per (image row, image); for each instance the row of
+// g is staged in shared memory and every thread takes min over x' of (x - x')^2 + g^2 (exact int64), keeping the two
 // smallest squared distances over instances.  clean_distances (src/preparation.py:159-168): sum of the two nearest
 // distances as float16, the second nearest as float64; one instance -> it counts twice; none -> zeros.
-__global__ void edt_rows_two_nearest_kernel(const int* __restrict__ g, __half* __restrict__ dist_sum,
-                                            double* __restrict__ second, int K, int H, int W) {
+__global__ void edt_rows_two_nearest_kernel(const int* __restrict__ g, const int* __restrict__ plane_index,
+                                            const int* __restrict__ image_off, const int* __restrict__ cols,
+                                            __half* __restrict__ dist_sum, double* __restrict__ second, int K, int H,
+                                            int W) {
   extern __shared__ int s_g[];
   const int y = blockIdx.x;
+  const int n = blockIdx.y;
+  const int k0 = image_off ? image_off[n] : 0, k1 = image_off ? image_off[n + 1] : K;
+  const long out_base = (long)n * H * W + (long)y * W;
   const int x = threadIdx.x;   // blockDim.x >= W handled by a strided loop below
   for (int xb = 0; xb < W; xb += blockDim.x) {
     const int xx = xb + x;
     long long b1 = -1, b2 = -1;   // two smallest squared distances (-1 = none yet)
-    for (int k = 0; k < K; ++k) {
+    for (int k = k0; k < k1; ++k) {
+      const int p = edt_plane(plane_index, k);
+      const int c0 = cols ? cols[4 * p + 2] : 0, c1 = cols ? cols[4 * p + 3] : W - 1;
       __syncthreads();
-      for (int i = threadIdx.x; i < W; i += blockDim.x) s_g[i] = g[((long)k * H + y) * W + i];
+      for (int i = c0 + threadIdx.x; i <= c1; i += blockDim.x) s_g[i] = g[((long)k * H + y) * W + i];
       __syncthreads();
       if (xx < W) {
         long long best = (long long)1 << 60;
-        for (int xp = 0; xp < W; ++xp) {
+        for (int xp = c0; xp <= c1; ++xp) {
           const long long gv = s_g[xp];
           if (gv >= kInfCol) continue;
           const long long dx = xx - xp;
           best = min(best, dx * dx + gv * gv);
         }
+        if (best == ((long long)1 << 60)) best = (long long)(y + 1) * (y + 1) + (long long)xx * xx;
         if (b1 < 0 || best < b1) { b2 = b1; b1 = best; }
         else if (b2 < 0 || best < b2) { b2 = best; }
       }
     }
     if (xx < W) {
       double d1 = 0.0, d2 = 0.0;
-      if (K == 1) { d1 = d2 = sqrt((double)b1); }
-      else if (K >= 2) { d1 = sqrt((double)b1); d2 = sqrt((double)b2); }
-      dist_sum[(long)y * W + xx] = __double2half(d1 + d2);
-      second[(long)y * W + xx] = d2;
+      if (k1 - k0 == 1) { d1 = d2 = sqrt((double)b1); }
+      else if (k1 - k0 >= 2) { d1 = sqrt((double)b1); d2 = sqrt((double)b2); }
+      dist_sum[out_base + xx] = __double2half(d1 + d2);
+      second[out_base + xx] = d2;
     }
   }
 }
@@ -236,20 +252,40 @@ extern "C" int mcb_pil_resize_bilinear_u8(const uint8_t* in, uint8_t* tmp, uint8
   return MCB_OK;
 }
 
+static int edt_launch(const uint8_t* masks, const int* plane_index, const int* image_off, const int* cols, int k,
+                      int n, int h, int w, int* workspace, void* dist_sum_f16, double* second_nearest, void* stream) {
+  MCB_REQUIRE(h < kInfCol && w < kInfCol, "edt: image too large");
+  constexpr int kMaxGridY = 65535;   // instances and images go on gridDim.y, in slices
+  for (int k0 = 0; k0 < k; k0 += kMaxGridY) {
+    edt_columns_kernel<<<dim3((w + 127) / 128, std::min(kMaxGridY, k - k0)), 128, 0, ST>>>(masks, plane_index, cols,
+                                                                                         workspace, h, w, k0);
+    MCB_LAUNCH_CHECK();
+  }
+  const int threads = std::min(1024, ((w + 31) / 32) * 32);
+  const long hw = (long)h * w;
+  for (int n0 = 0; n0 < n; n0 += kMaxGridY) {   // n > 1 only with image_off
+    edt_rows_two_nearest_kernel<<<dim3(h, std::min(kMaxGridY, n - n0)), threads, (size_t)w * sizeof(int), ST>>>(
+        workspace, plane_index, image_off ? image_off + n0 : nullptr, cols, (__half*)dist_sum_f16 + n0 * hw,
+        second_nearest + n0 * hw, k, h, w);
+    MCB_LAUNCH_CHECK();
+  }
+  return MCB_OK;
+}
+
 extern "C" int mcb_edt_two_nearest(const uint8_t* masks, int k, int h, int w, int* workspace, void* dist_sum_f16,
                                    double* second_nearest, void* stream) {
   MCB_REQUIRE(dist_sum_f16 && second_nearest && k >= 0 && h > 0 && w > 0, "edt: bad argument");
   MCB_REQUIRE(k == 0 || (masks && workspace), "edt: null pointer");
-  MCB_REQUIRE(h < kInfCol && w < kInfCol, "edt: image too large");
-  if (k > 0) {
-    edt_columns_kernel<<<dim3((w + 127) / 128, k), 128, 0, ST>>>(masks, workspace, k, h, w);
-    MCB_LAUNCH_CHECK();
-  }
-  const int threads = std::min(1024, ((w + 31) / 32) * 32);
-  edt_rows_two_nearest_kernel<<<h, threads, (size_t)w * sizeof(int), ST>>>(workspace, (__half*)dist_sum_f16,
-                                                                         second_nearest, k, h, w);
-  MCB_LAUNCH_CHECK();
-  return MCB_OK;
+  return edt_launch(masks, nullptr, nullptr, nullptr, k, 1, h, w, workspace, dist_sum_f16, second_nearest, stream);
+}
+
+extern "C" int mcb_edt_two_nearest_batched(const uint8_t* masks, const int* plane_index, const int* image_off,
+                                           const int* plane_stats, int k, int n, int h, int w, int* workspace,
+                                           void* dist_sum_f16, double* second_nearest, void* stream) {
+  MCB_REQUIRE(dist_sum_f16 && second_nearest && image_off && k >= 0 && n > 0 && h > 0 && w > 0, "edt: bad argument");
+  MCB_REQUIRE(k == 0 || (masks && workspace), "edt: null pointer");
+  return edt_launch(masks, plane_index, image_off, plane_stats, k, n, h, w, workspace, dist_sum_f16, second_nearest,
+                    stream);
 }
 
 extern "C" int mcb_size_matrix(const int* labels, const int* area, long long* out, int h, int w, void* stream) {

@@ -408,6 +408,30 @@ extern "C" int mcb_morph_rect(const void* in, void* out, int is_i32, int is_dila
   return MCB_OK;
 }
 
+// skimage <= 0.17 binary_erosion / binary_dilation with rectangle(k, k) (src/preparation.py:170-186), i.e.
+// ndi.binary_erosion(structure, border_value=True) / ndi.binary_dilation(structure), on {0,1} uint8 planes.  Dilation
+// takes the same window as the grey dilation above; scipy centres an even binary erosion at index k/2, so its window
+// is [-k/2, k/2 - 1] where the grey erosion's is [-k/2 + 1, k/2].  Out-of-range taps are ignored in both (border_value
+// True for the erosion, 0 for the dilation).
+extern "C" int mcb_binary_morph_rect(const uint8_t* in, uint8_t* out, int is_dilation, int size, int planes, int h, int w,
+                                     void* stream) {
+  MCB_REQUIRE(in && out && in != out, "binary_morph: null or aliased pointer");
+  MCB_REQUIRE(size >= 1 && size <= 31, "binary_morph: size %d", size);
+  constexpr int kMaxGridY = 65535;   // planes go on gridDim.y, in slices
+  const long hw = (long)h * w;
+  for (int p0 = 0; p0 < planes; p0 += kMaxGridY) {
+    const int cnt = std::min(kMaxGridY, planes - p0);
+    if (is_dilation || size % 2 == 1) {
+      if (int r = mcb_morph_rect(in + p0 * hw, out + p0 * hw, 0, is_dilation, size, cnt, h, w, stream)) return r;
+      continue;
+    }
+    morph_rect_kernel<uint8_t, false><<<plane_grid(hw, cnt, 256), 256, 0, ST>>>(in + p0 * hw, out + p0 * hw, h, w,
+                                                                               -size / 2, size / 2 - 1);
+    MCB_LAUNCH_CHECK();
+  }
+  return MCB_OK;
+}
+
 extern "C" int mcb_add_dropped_objects(const uint8_t* original, const uint8_t* processed, uint8_t* out, int* workspace,
                                        int planes, int h, int w, void* stream) {
   MCB_REQUIRE(original && processed && out && workspace, "add_dropped: null pointer");

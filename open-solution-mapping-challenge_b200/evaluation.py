@@ -54,6 +54,49 @@ def segmentation_counts(segm, h, w):
     return np.asarray(cnts, dtype=np.int64), (int(segm['size'][0]), int(segm['size'][1]))
 
 
+GT_RLE_CHUNK = 4096   # polygon annotations rasterised per device batch
+
+
+def ground_truth_rle(gt):
+    """a copy of a COCO ground truth (dict or JSON path) whose polygon segmentations are replaced by the uncompressed
+    RLE {'size': [h, w], 'counts': [...]} of COCO.annToRLE, merge(frPyObjects(polygons, h, w)): the union of the
+    annotation's polygons, rasterised on the device exactly as pycocotools does (mcb200.preparation).  The result
+    feeds DeviceCOCOEvaluator / coco_evaluation without pycocotools."""
+    import copy
+    from .preparation import polygons_csr, rasterize_polygons, segmentation_polygons
+    from .postprocessing import _dev
+    if not isinstance(gt, dict):
+        with open(gt) as f:
+            gt = json.load(f)
+    out = copy.deepcopy(gt)
+    size = {im["id"]: (int(im["height"]), int(im["width"])) for im in out.get("images", [])}
+    by_size = {}
+    for a in out.get("annotations", []):
+        if isinstance(a.get("segmentation"), list):
+            by_size.setdefault(size[a["image_id"]], []).append(a)
+    for (h, w), anns in by_size.items():
+        for c0 in range(0, len(anns), GT_RLE_CHUNK):
+            chunk = anns[c0:c0 + GT_RLE_CHUNK]
+            polys, group = [], []
+            for j, a in enumerate(chunk):
+                segm = segmentation_polygons(a["segmentation"])
+                polys.extend(segm)
+                group.extend([j] * len(segm))
+            dev = _dev()
+            planes = rasterize_polygons(*polygons_csr(polys), h, w)
+            union = torch.empty((len(chunk), h, w), dtype=torch.uint8, device=dev)
+            goff = np.concatenate([[0], np.cumsum(np.bincount(group, minlength=len(chunk)))]).astype(np.int32)
+            index = torch.arange(max(len(polys), 1), dtype=torch.int32, device=dev)
+            goff_d = torch.from_numpy(goff).to(dev)
+            L.fcall("mcb_plane_union", planes.data_ptr() if len(polys) else index.data_ptr(), index.data_ptr(),
+                    goff_d.data_ptr(), len(chunk), h, w, union.data_ptr())
+            labels = union.to(torch.int32)
+            cnts, starts, _, _ = rle_encode_instances(labels, torch.ones(len(chunk), dtype=torch.int32, device=dev))
+            for j, a in enumerate(chunk):
+                a["segmentation"] = {"size": [h, w], "counts": cnts[starts[j]:starts[j + 1]].astype(np.int64).tolist()}
+    return out
+
+
 def _rle_area(cnts):
     return int(np.asarray(cnts, dtype=np.int64)[1::2].sum())
 
