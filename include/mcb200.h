@@ -334,10 +334,11 @@ int mcb_tta_aggregate(const float* pred, int from_logits, const int* var_start, 
 /* Instance emission (src/utils.py:61-127; src/postprocessing.py:284-352).  An instance is (plane, label); its slot is
  * offsets[plane] + label - 1 with offsets the exclusive prefix of counts (labels per plane, from mcb_ccl_label).
  * geometry: geo int32 [total][5] = {area, rmin, rmax, cmin, cmax} (caller initialises {0, INT_MAX, -1, INT_MAX, -1});
- * with prob (fp32|fp64 planes aligned with labels): psum fp64 [total] (zeroed) and pmax int32 [total] (order-preserving
- * integer image of the fp32 maximum, initialised to that of -inf) */
+ * with prob (fp32|fp64 planes aligned with labels): psum fp64 [total] (zeroed) and pmax int64 [total] (order-preserving
+ * integer image of the fp64 maximum -- bits b >= 0 stay, b < 0 become b ^ 0x7FFFFFFFFFFFFFFF -- initialised to that of
+ * -inf; an fp32 input widens exactly, so the maximum is exact in either precision) */
 int mcb_instance_geometry(const int* labels, const void* prob, int prob_is_f64, const int* offsets, const int* counts,
-                          int* geo, double* psum, int* pmax, int planes, int h, int w, void* stream);
+                          int* geo, double* psum, long long* pmax, int planes, int h, int w, void* stream);
 /* COCO run-length encoding of every instance mask (pycocotools rleEncode on the Fortran-ordered mask,
  * src/utils.py:118-120).  One task per (instance, bounding-box column), listed in (instance, column) order by the caller
  * (task_slot, task_x: int32 [ntasks]).  Pass write=0 fills task_n[t] = number of value changes of the column-major scan

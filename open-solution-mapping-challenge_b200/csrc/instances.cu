@@ -17,8 +17,9 @@ namespace mcb {
 // ------------------------------------------------------------------------------------------ categorize_image
 // numpy argmax: index of the FIRST maximum; a NaN compares as the maximum (first NaN wins).
 template <typename T>
-__global__ void argmax_channels_kernel(const T* __restrict__ prob, long long* __restrict__ out, int C, long hw) {
-  const int img = blockIdx.y;
+__global__ void argmax_channels_kernel(const T* __restrict__ prob, long long* __restrict__ out, int C, long hw,
+                                       int img0) {
+  const int img = img0 + blockIdx.y;
   const T* p = prob + (long)img * C * hw;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < hw; i += (long)gridDim.x * blockDim.x) {
     T best = p[i];
@@ -50,8 +51,8 @@ __device__ __forceinline__ void rot90_src(int k, int i, int j, int H, int W, int
 
 // x [n][c][h][w] -> out [nv][c][ho][wo], (ho, wo) = (h, w) or (w, h) for odd k (square images keep their shape)
 __global__ void tta_transform_kernel(const float* __restrict__ x, float* __restrict__ out, const int* __restrict__ img_of,
-                                     const int* __restrict__ code, int C, int H, int W) {
-  const int v = blockIdx.y;
+                                     const int* __restrict__ code, int C, int H, int W, int v0) {
+  const int v = v0 + blockIdx.y;
   const int cd = code[v];
   const int k = cd & 3, flip = (cd >> 2) & 3;
   const int Ho = (k & 1) ? W : H, Wo = (k & 1) ? H : W;
@@ -78,8 +79,8 @@ __global__ void tta_transform_kernel(const float* __restrict__ x, float* __restr
 constexpr int kTtaMaxC = 8;
 __global__ void tta_aggregate_kernel(const float* __restrict__ pred, int from_logits, const int* __restrict__ var_start,
                                      const int* __restrict__ var_index, const int* __restrict__ code,
-                                     float* __restrict__ out, int C, int H, int W, int method) {
-  const int img = blockIdx.y;
+                                     float* __restrict__ out, int C, int H, int W, int method, int img0) {
+  const int img = img0 + blockIdx.y;
   const int vb = var_start[img], ve = var_start[img + 1];
   const long hw = (long)H * W;
   for (long q = blockIdx.x * (long)blockDim.x + threadIdx.x; q < hw; q += (long)gridDim.x * blockDim.x) {
@@ -129,20 +130,21 @@ __global__ void tta_aggregate_kernel(const float* __restrict__ pred, int from_lo
 // One pass over the label planes: per instance (slot = offsets[plane] + label - 1) the pixel count, the tight
 // bounding box and the probability sum / maximum (FeatureExtractor: area, mean_prob, max_prob, get_bbox).  Threads walk
 // contiguous row segments and flush once per label change.  geo: int32 [total][5] = {area, rmin, rmax, cmin, cmax}
-// (initialised by the caller to {0, INT_MAX, -1, INT_MAX, -1}); psum fp64 [total]; pmax fp32-as-ordered-int [total].
-__device__ __forceinline__ int float_to_ordered(float f) {
-  const int i = __float_as_int(f);
-  return i >= 0 ? i : i ^ 0x7FFFFFFF;
+// (initialised by the caller to {0, INT_MAX, -1, INT_MAX, -1}); psum fp64 [total]; pmax int64 [total], the
+// order-preserving integer image of the fp64 maximum.  The maximum is kept in fp64 for both input types: the reference
+// takes it over skimage's float64 resize, and an fp32 input widens exactly, so one path serves both.
+__device__ __forceinline__ long long double_to_ordered(double d) {
+  const long long i = __double_as_longlong(d);
+  return i >= 0 ? i : i ^ 0x7FFFFFFFFFFFFFFFLL;
 }
-__device__ __forceinline__ float ordered_to_float(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7FFFFFFF); }
 
 template <typename T>
 __global__ void __launch_bounds__(256) instance_geometry_kernel(const int* __restrict__ labels, const T* __restrict__ prob,
                                                                 const int* __restrict__ offsets,
                                                                 const int* __restrict__ counts, int* __restrict__ geo,
-                                                                double* __restrict__ psum, int* __restrict__ pmax,
-                                                                int H, int W, int seg) {
-  const int plane = blockIdx.y;
+                                                                double* __restrict__ psum, long long* __restrict__ pmax,
+                                                                int H, int W, int seg, int plane0) {
+  const int plane = plane0 + blockIdx.y;
   const int off = offsets[plane], K = counts[plane];
   const long hw = (long)H * W;
   const int* L = labels + (long)plane * hw;
@@ -154,7 +156,7 @@ __global__ void __launch_bounds__(256) instance_geometry_kernel(const int* __res
     const int c0 = (int)(sidx % segs_per_row) * seg, c1 = min(W, c0 + seg);
     int cur = 0, cnt = 0, cs = 0;
     double sum = 0.0;
-    float mx = -INFINITY;
+    double mx = -INFINITY;
     auto flush = [&](int cend) {
       if (cur > 0 && cur <= K) {
         int* g = geo + (long)(off + cur - 1) * 5;
@@ -163,7 +165,7 @@ __global__ void __launch_bounds__(256) instance_geometry_kernel(const int* __res
         atomicMax(g + 2, r);
         atomicMin(g + 3, cs);
         atomicMax(g + 4, cend);
-        if (P) { atomicAdd(psum + off + cur - 1, sum); atomicMax(pmax + off + cur - 1, float_to_ordered(mx)); }
+        if (P) { atomicAdd(psum + off + cur - 1, sum); atomicMax(pmax + off + cur - 1, double_to_ordered(mx)); }
       }
     };
     for (int c = c0; c < c1; ++c) {
@@ -174,7 +176,7 @@ __global__ void __launch_bounds__(256) instance_geometry_kernel(const int* __res
       }
       if (l > 0) {
         ++cnt;
-        if (P) { const float pv = (float)__ldg(P + (long)r * W + c); sum += (double)__ldg(P + (long)r * W + c); mx = fmaxf(mx, pv); }
+        if (P) { const double pv = (double)__ldg(P + (long)r * W + c); sum += pv; mx = fmax(mx, pv); }
       }
     }
     flush(c1 - 1);
@@ -287,8 +289,8 @@ __global__ void __launch_bounds__(256) pair_intersection_kernel(const int* __res
 __global__ void __launch_bounds__(256) contour_length_kernel(const int* __restrict__ labels,
                                                              const int* __restrict__ offsets,
                                                              const int* __restrict__ counts, int* __restrict__ clen,
-                                                             int H, int W) {
-  const int plane = blockIdx.y;
+                                                             int H, int W, int plane0) {
+  const int plane = plane0 + blockIdx.y;
   const int off = offsets[plane], K = counts[plane];
   const long hw = (long)H * W;
   const int* L = labels + (long)plane * hw;
@@ -307,6 +309,9 @@ __global__ void __launch_bounds__(256) contour_length_kernel(const int* __restri
 using namespace mcb;
 #define ST static_cast<cudaStream_t>(stream)
 
+// grids put planes / images / variants on y; launches over more than kMaxGridY of them go in slices
+// (gridDim.y <= 65535), each kernel adding its slice's first index to blockIdx.y
+constexpr int kMaxGridY = 65535;
 static dim3 grid2(long items, int planes, int threads) {
   const int per_plane =
       (int)std::max(1L, std::min((items + threads - 1) / threads, (long)num_sms() * 8L / std::max(planes, 1) + 1));
@@ -317,17 +322,23 @@ extern "C" int mcb_argmax_channels(const void* prob, int prob_is_f64, long long*
                                    void* stream) {
   MCB_REQUIRE(prob && out && n > 0 && c > 0 && h > 0 && w > 0, "argmax: bad argument");
   const long hw = (long)h * w;
-  if (prob_is_f64) argmax_channels_kernel<double><<<grid2(hw, n, 256), 256, 0, ST>>>((const double*)prob, out, c, hw);
-  else argmax_channels_kernel<float><<<grid2(hw, n, 256), 256, 0, ST>>>((const float*)prob, out, c, hw);
-  MCB_LAUNCH_CHECK();
+  for (int i0 = 0; i0 < n; i0 += kMaxGridY) {
+    const dim3 grid = grid2(hw, std::min(kMaxGridY, n - i0), 256);
+    if (prob_is_f64) argmax_channels_kernel<double><<<grid, 256, 0, ST>>>((const double*)prob, out, c, hw, i0);
+    else argmax_channels_kernel<float><<<grid, 256, 0, ST>>>((const float*)prob, out, c, hw, i0);
+    MCB_LAUNCH_CHECK();
+  }
   return MCB_OK;
 }
 
 extern "C" int mcb_tta_transform(const float* x, float* out, const int* img_of, const int* code, int nv, int c, int h,
                                  int w, void* stream) {
   MCB_REQUIRE(x && out && img_of && code && nv > 0 && c > 0, "tta_transform: bad argument");
-  tta_transform_kernel<<<grid2((long)c * h * w, nv, 256), 256, 0, ST>>>(x, out, img_of, code, c, h, w);
-  MCB_LAUNCH_CHECK();
+  for (int v0 = 0; v0 < nv; v0 += kMaxGridY) {
+    tta_transform_kernel<<<grid2((long)c * h * w, std::min(kMaxGridY, nv - v0), 256), 256, 0, ST>>>(x, out, img_of, code,
+                                                                                                  c, h, w, v0);
+    MCB_LAUNCH_CHECK();
+  }
   return MCB_OK;
 }
 
@@ -336,25 +347,31 @@ extern "C" int mcb_tta_aggregate(const float* pred, int from_logits, const int* 
   MCB_REQUIRE(pred && var_start && var_index && code && out && n > 0, "tta_aggregate: null pointer");
   MCB_REQUIRE(c >= 1 && c <= kTtaMaxC, "tta_aggregate: %d classes (max %d)", c, kTtaMaxC);
   MCB_REQUIRE(method >= 0 && method <= 3, "tta_aggregate: method %d", method);
-  tta_aggregate_kernel<<<grid2((long)h * w, n, 256), 256, 0, ST>>>(pred, from_logits, var_start, var_index, code, out, c,
-                                                                  h, w, method);
-  MCB_LAUNCH_CHECK();
+  for (int i0 = 0; i0 < n; i0 += kMaxGridY) {
+    tta_aggregate_kernel<<<grid2((long)h * w, std::min(kMaxGridY, n - i0), 256), 256, 0, ST>>>(
+        pred, from_logits, var_start, var_index, code, out, c, h, w, method, i0);
+    MCB_LAUNCH_CHECK();
+  }
   return MCB_OK;
 }
 
 extern "C" int mcb_instance_geometry(const int* labels, const void* prob, int prob_is_f64, const int* offsets,
-                                     const int* counts, int* geo, double* psum, int* pmax, int planes, int h, int w,
-                                     void* stream) {
+                                     const int* counts, int* geo, double* psum, long long* pmax, int planes, int h,
+                                     int w, void* stream) {
   MCB_REQUIRE(labels && offsets && counts && geo, "instance_geometry: null pointer");
   MCB_REQUIRE(!prob || (psum && pmax), "instance_geometry: prob needs psum and pmax");
   const int seg = 32;
   const long nseg = (long)h * ((w + seg - 1) / seg);
-  dim3 grid = grid2(nseg, planes, 256);
-  if (prob && prob_is_f64)
-    instance_geometry_kernel<double><<<grid, 256, 0, ST>>>(labels, (const double*)prob, offsets, counts, geo, psum, pmax, h, w, seg);
-  else
-    instance_geometry_kernel<float><<<grid, 256, 0, ST>>>(labels, (const float*)prob, offsets, counts, geo, psum, pmax, h, w, seg);
-  MCB_LAUNCH_CHECK();
+  for (int p0 = 0; p0 < planes; p0 += kMaxGridY) {
+    const dim3 grid = grid2(nseg, std::min(kMaxGridY, planes - p0), 256);
+    if (prob && prob_is_f64)
+      instance_geometry_kernel<double><<<grid, 256, 0, ST>>>(labels, (const double*)prob, offsets, counts, geo, psum,
+                                                             pmax, h, w, seg, p0);
+    else
+      instance_geometry_kernel<float><<<grid, 256, 0, ST>>>(labels, (const float*)prob, offsets, counts, geo, psum, pmax,
+                                                            h, w, seg, p0);
+    MCB_LAUNCH_CHECK();
+  }
   return MCB_OK;
 }
 
@@ -398,7 +415,10 @@ extern "C" int mcb_pair_intersections(const int* labels_a, const int* labels_b, 
 extern "C" int mcb_contour_length(const int* labels, const int* offsets, const int* counts, int* clen, int planes, int h,
                                   int w, void* stream) {
   MCB_REQUIRE(labels && offsets && counts && clen, "contour_length: null pointer");
-  contour_length_kernel<<<grid2((long)h * w, planes, 256), 256, 0, ST>>>(labels, offsets, counts, clen, h, w);
-  MCB_LAUNCH_CHECK();
+  for (int p0 = 0; p0 < planes; p0 += kMaxGridY) {
+    contour_length_kernel<<<grid2((long)h * w, std::min(kMaxGridY, planes - p0), 256), 256, 0, ST>>>(labels, offsets,
+                                                                                                   counts, clen, h, w, p0);
+    MCB_LAUNCH_CHECK();
+  }
   return MCB_OK;
 }

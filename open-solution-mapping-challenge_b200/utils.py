@@ -20,6 +20,7 @@ from . import _lib as L
 from .postprocessing import _dev, _to_dev
 
 _INT_MAX = 2 ** 31 - 1
+_ORDERED_FLIP = 0x7FFFFFFFFFFFFFFF       # float64 bits b < 0 <-> order-preserving int64 b ^ _ORDERED_FLIP
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -35,8 +36,9 @@ def _offsets(counts):
 
 def instance_geometry(labels, counts, probs=None):
     """labels (P, H, W) int32 cuda, counts (P,) int32 cuda (labels per plane), probs (P, H, W) float32|float64 or None
-    -> dict of host arrays per instance slot: area, rmin, rmax, cmin, cmax [, psum (float64), pmax (float32)],
-    plus 'offsets', 'counts', 'plane' (slot -> plane)."""
+    -> dict of host arrays per instance slot: area, rmin, rmax, cmin, cmax [, psum (float64), pmax (float64)],
+    plus 'offsets', 'counts', 'plane' (slot -> plane).  pmax is the exact maximum in the probabilities' own precision
+    (float32 values widen exactly), -inf for an empty instance."""
     assert labels.is_cuda and labels.dtype == torch.int32 and labels.is_contiguous() and labels.dim() == 3
     p, h, w = labels.shape
     counts = counts.to(torch.int32).contiguous()
@@ -51,9 +53,9 @@ def instance_geometry(labels, counts, probs=None):
     if probs is not None:
         assert probs.shape == labels.shape and probs.is_cuda and probs.is_contiguous()
         psum = torch.zeros(max(total, 1), dtype=torch.float64, device=labels.device)
-        # order-preserving integer image of float32 -inf
-        pmax = torch.full((max(total, 1),), int(np.array(-np.inf, np.float32).view(np.int32)) ^ 0x7FFFFFFF,
-                          dtype=torch.int32, device=labels.device)
+        # order-preserving integer image of float64 -inf
+        pmax = torch.full((max(total, 1),), int(np.array(-np.inf, np.float64).view(np.int64)) ^ _ORDERED_FLIP,
+                          dtype=torch.int64, device=labels.device)
     if total > 0:
         L.fcall("mcb_instance_geometry", labels.data_ptr(), None if probs is None else probs.data_ptr(),
                 int(probs is not None and probs.dtype == torch.float64), offs_d.data_ptr(), counts.data_ptr(),
@@ -66,7 +68,7 @@ def instance_geometry(labels, counts, probs=None):
     if probs is not None:
         out["psum"] = psum[:total].cpu().numpy()
         pm = pmax[:total].cpu().numpy()
-        out["pmax"] = np.where(pm >= 0, pm, pm ^ 0x7FFFFFFF).astype(np.int32).view(np.float32)
+        out["pmax"] = np.where(pm >= 0, pm, pm ^ _ORDERED_FLIP).astype(np.int64).view(np.float64)
     return out
 
 

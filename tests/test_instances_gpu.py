@@ -122,9 +122,9 @@ def test_nms_and_features(mcb, cuda):
             assert len(lg) == len(lw)
             for a, b in zip(lg, lw):
                 for k in ("threshold", "area", "bbox_area", "min_dist_to_border", "max_dist_to_border",
-                          "contour_length"):
+                          "contour_length", "max_prob"):
                     assert a[k] == b[k], (k, a[k], b[k])
-                for k in ("mean_prob", "max_prob", "bbox_ar", "bbox_fill"):
+                for k in ("mean_prob", "bbox_ar", "bbox_fill"):
                     assert abs(a[k] - b[k]) <= 1e-9 * max(1.0, abs(b[k])), (k, a[k], b[k])
 
 
