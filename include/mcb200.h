@@ -324,6 +324,14 @@ int mcb_argmax_channels(const void* prob, int prob_is_f64, long long* out, int n
  * 2 left-right).  x fp32 [n][c][h][w], out fp32 [nv][c][h][w] (h == w when k is odd) */
 int mcb_tta_transform(const float* x, float* out, const int* img_of, const int* code, int nv, int c, int h, int w,
                       void* stream);
+/* The variant rows of the TTA loaders before their pad / resize: test_time_augmentation_transform
+ * (src/loaders.py:477-487) with its colour-shift branch, color_seq (src/augmentation.py:12-31), on the decoded tiles.
+ * images uint8 [n][h][w][3] RGB -> out uint8 [nv][h][w][3], row v from tile src[v]; code[v] = geometry (bits 0-3, as
+ * mcb_tta_transform) | colour branch << 4 (0 none; 1-3 Add to H, S or V through cv2's RGB2HSV / HSV2RGB; 4-6 Add to
+ * R, G or B) | value << 8 (0-255; clipped at 255 after the add).  Bit-exact to cv2 4.x's vector body on every pixel
+ * (h == w when k is odd) */
+int mcb_tta_variants_u8(const uint8_t* images, uint8_t* out, const int* src, const int* code, int nv, int h, int w,
+                        void* stream);
 /* TestTimeAugmentationAggregator.transform + test_time_augmentation_inverse_transform (src/loaders.py:437-497) in one
  * pass: out[i] = agg over the variants v of image i of flip(rot90(pred[v], -k)); pred fp32 [nv][c][h][w] holds class
  * probabilities, or logits when from_logits (the class softmax of src/models.py:88-92 is then taken in registers).

@@ -170,6 +170,7 @@ lib.mcb_instance_scores_strided.restype = ci
 _SIGS4 = {
     "mcb_argmax_channels": [vp, ci, vp, ci, ci, ci, ci, vp],
     "mcb_tta_transform": [vp, vp, vp, vp, ci, ci, ci, ci, vp],
+    "mcb_tta_variants_u8": [vp, vp, vp, vp, ci, ci, ci, vp],
     "mcb_tta_aggregate": [vp, ci, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp],
     "mcb_instance_geometry": [vp, vp, ci, vp, vp, vp, vp, vp, ci, ci, ci, vp],
     "mcb_rle_walk": [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, vp],

@@ -49,12 +49,20 @@ __device__ __forceinline__ void rot90_src(int k, int i, int j, int H, int W, int
   }
 }
 
+// source pixel (si, sj) of output pixel (i, j) of the variant with geometry code `cd` (bits 0-3) of an (H, W) image
+__device__ __forceinline__ void tta_src(int cd, int i, int j, int H, int W, int& si, int& sj) {
+  const int k = cd & 3, flip = (cd >> 2) & 3;
+  rot90_src(k, i, j, H, W, si, sj);          // into the flipped image (H, W)
+  if (flip == 1) si = H - 1 - si;
+  else if (flip == 2) sj = W - 1 - sj;
+}
+
 // x [n][c][h][w] -> out [nv][c][ho][wo], (ho, wo) = (h, w) or (w, h) for odd k (square images keep their shape)
 __global__ void tta_transform_kernel(const float* __restrict__ x, float* __restrict__ out, const int* __restrict__ img_of,
                                      const int* __restrict__ code, int C, int H, int W, int v0) {
   const int v = v0 + blockIdx.y;
   const int cd = code[v];
-  const int k = cd & 3, flip = (cd >> 2) & 3;
+  const int k = cd & 3;
   const int Ho = (k & 1) ? W : H, Wo = (k & 1) ? H : W;
   const float* src = x + (long)img_of[v] * C * H * W;
   float* dst = out + (long)v * C * H * W;
@@ -64,10 +72,79 @@ __global__ void tta_transform_kernel(const float* __restrict__ x, float* __restr
     const int r = q % ((long)Ho * Wo);
     const int i = r / Wo, j = r % Wo;
     int si, sj;
-    rot90_src(k, i, j, H, W, si, sj);          // into the flipped image (H, W)
-    if (flip == 1) si = H - 1 - si;
-    else if (flip == 2) sj = W - 1 - sj;
+    tta_src(cd, i, j, H, W, si, sj);
     dst[q] = src[((long)c * H + si) * W + sj];
+  }
+}
+
+// color_seq (src/augmentation.py:12-31, imgaug 0.2.5) on one uint8 RGB pixel.  branch 1-3: cv2 RGB2HSV (H in 0..179),
+// Add `value` to channel branch-1 clipped at 255 (H too: imgaug clips at the dtype's maximum, not at 180), cv2 HSV2RGB;
+// branch 4-6: Add `value` to R, G or B clipped at 255.
+// RGB2HSV is cv2's integer path (12-bit fixed-point reciprocal tables; the rint of the division is taken here in integer
+// arithmetic, which has no ties for these operands).  HSV2RGB is the map of cv2's AVX2 vector body (OpenCV 4.x
+// HSV2RGB_b), derived by an exhaustive probe over all 2^24 inputs: fp32, the two `1 - s·t` terms fused (one rounding),
+// every other product and difference rounded on its own, the result ×255 truncated.  The explicit __f*_rn intrinsics
+// keep nvcc from contracting any other pair into an FMA.  cv2's scalar tail (the last columns of a row that do not fill
+// a vector) rounds instead of truncating; DESIGN.md §4.5.
+__device__ __forceinline__ void color_shift_px(int branch, int value, int& r, int& g, int& b) {
+  if (branch >= 4) {
+    if (branch == 4) r = min(255, r + value);
+    else if (branch == 5) g = min(255, g + value);
+    else b = min(255, b + value);
+    return;
+  }
+  const int v = max(r, max(g, b));
+  const int diff = v - min(r, min(g, b));
+  const int sdiv = v ? ((255 << 13) + v) / (2 * v) : 0;                 // rint((255 << 12) / v)
+  const int hdiv = diff ? ((180 << 13) + 6 * diff) / (12 * diff) : 0;   // rint((180 << 12) / (6 diff))
+  const int num = v == r ? g - b : (v == g ? b - r + 2 * diff : r - g + 4 * diff);
+  int hh = (num * hdiv + 2048) >> 12, ss = (diff * sdiv + 2048) >> 12, vi = v;
+  if (hh < 0) hh += 180;
+  if (branch == 1) hh = min(255, hh + value);
+  else if (branch == 2) ss = min(255, ss + value);
+  else vi = min(255, vi + value);
+  const float h = __fmul_rn((float)hh, 6.f / 180.f);
+  const float s = __fmul_rn((float)ss, 1.f / 255.f);
+  const float vv = __fmul_rn((float)vi, 1.f / 255.f);
+  const float pre = truncf(h);
+  const float f = __fsub_rn(h, pre);
+  const float t1 = __fmul_rn(vv, __fsub_rn(1.f, s));
+  const float t2 = __fmul_rn(vv, __fmaf_rn(-s, f, 1.f));
+  const float t3 = __fmul_rn(vv, __fmaf_rn(-s, __fsub_rn(1.f, f), 1.f));
+  const int sector = (int)pre - 6 * (int)truncf(__fmul_rn(pre, 1.f / 6.f));   // H up to 255 wraps: 200 = 20 (mod 180)
+  // cv2's sector table {1,3,0} {1,0,2} {3,0,1} {0,2,1} {0,1,3} {2,1,0}: (b, g, r) picks from (vv, t1, t2, t3)
+  const float fb = sector < 2 ? t1 : (sector == 2 ? t3 : (sector <= 4 ? vv : t2));
+  const float fg = sector == 0 ? t3 : (sector <= 2 ? vv : (sector == 3 ? t2 : t1));
+  const float fr = (sector == 0 || sector == 5) ? vv : (sector == 1 ? t2 : (sector == 4 ? t3 : t1));
+  b = min(255, (int)__fmul_rn(fb, 255.f));
+  g = min(255, (int)__fmul_rn(fg, 255.f));
+  r = min(255, (int)__fmul_rn(fr, 255.f));
+}
+
+// The variant rows of the TTA loaders (MetadataImageSegmentationTTA.__getitem__ + test_time_augmentation_transform,
+// src/loaders.py:94-111,477-487) on the decoded tiles: img uint8 [n][h][w][3] -> out uint8 [nv][h][w][3], row v from
+// tile src[v].  code[v] = geometry (bits 0-3, as tta_transform_kernel) | colour branch << 4 | value << 8.  Colour is
+// per pixel, so applying it at the source pixel equals the reference's colour-then-rotate order.  One thread per output
+// pixel: 3 B in, 3 B out.
+__global__ void tta_variants_u8_kernel(const uint8_t* __restrict__ img, uint8_t* __restrict__ out,
+                                       const int* __restrict__ src, const int* __restrict__ code, int H, int W, int v0) {
+  const int v = v0 + blockIdx.y;
+  const int cd = code[v];
+  const int branch = (cd >> 4) & 7, value = (cd >> 8) & 255;
+  const int Wo = (cd & 1) ? H : W;
+  const long hw = (long)H * W;
+  const uint8_t* s = img + (long)src[v] * hw * 3;
+  uint8_t* d = out + (long)v * hw * 3;
+  for (long q = blockIdx.x * (long)blockDim.x + threadIdx.x; q < hw; q += (long)gridDim.x * blockDim.x) {
+    const int i = q / Wo, j = q % Wo;
+    int si, sj;
+    tta_src(cd, i, j, H, W, si, sj);
+    const uint8_t* p = s + ((long)si * W + sj) * 3;
+    int r = p[0], g = p[1], b = p[2];
+    if (branch) color_shift_px(branch, value, r, g, b);
+    d[q * 3] = (uint8_t)r;
+    d[q * 3 + 1] = (uint8_t)g;
+    d[q * 3 + 2] = (uint8_t)b;
   }
 }
 
@@ -337,6 +414,17 @@ extern "C" int mcb_tta_transform(const float* x, float* out, const int* img_of, 
   for (int v0 = 0; v0 < nv; v0 += kMaxGridY) {
     tta_transform_kernel<<<grid2((long)c * h * w, std::min(kMaxGridY, nv - v0), 256), 256, 0, ST>>>(x, out, img_of, code,
                                                                                                   c, h, w, v0);
+    MCB_LAUNCH_CHECK();
+  }
+  return MCB_OK;
+}
+
+extern "C" int mcb_tta_variants_u8(const uint8_t* images, uint8_t* out, const int* src, const int* code, int nv, int h,
+                                   int w, void* stream) {
+  MCB_REQUIRE(images && out && src && code && nv > 0 && h > 0 && w > 0, "tta_variants_u8: bad argument");
+  for (int v0 = 0; v0 < nv; v0 += kMaxGridY) {
+    tta_variants_u8_kernel<<<grid2((long)h * w, std::min(kMaxGridY, nv - v0), 256), 256, 0, ST>>>(images, out, src, code,
+                                                                                                h, w, v0);
     MCB_LAUNCH_CHECK();
   }
   return MCB_OK;
