@@ -68,6 +68,16 @@ class _BN:
                  "idx", "off", "app_dgamma", "app_dbeta", "g32_dgamma", "g32_dbeta")
 
 
+class _ConvPart:
+    """one conv + BatchNorm of a ResNet block in a training plan, for per-unit tests: the state_dict prefixes of the
+    conv and its BatchNorm, the conv's input x and output z, the BatchNorm output y (None for the block's last conv and
+    its downsample, whose BatchNorms the residual pass applies), the _BN state and the backward's dz buffer"""
+    __slots__ = ("conv", "bn", "x", "z", "y", "state", "dz")
+
+    def __init__(self, conv, bn, x, z, y, state):
+        self.conv, self.bn, self.x, self.z, self.y, self.state, self.dz = conv, bn, x, z, y, state, None
+
+
 class Plan:
     """What every launch plan shares: activation and gradient buffers, the BatchNorm units, the decoder blocks and the
     classifier tail, backward registration, the arena segments and execution.  A subclass per encoder family builds
@@ -85,6 +95,9 @@ class Plan:
         self._bwd_builders = []    # (tag, builder) per forward unit; run in REVERSE so store/accumulate modes follow run order
         self.units = []            # (kind, state_dict prefix, inputs, output) per forward unit, for per-unit parity tests
         self.dec_mid = {}          # id(decoder block output) -> the block's middle ConvRelu output, for the same tests
+        self.block_parts = {}      # training ResNet plans: id(block output) -> [_ConvPart], conv1 .. [downsample]
+        self.stem_parts = {}       # training ResNet plans: the stem's col, z0, a0, c1, bn0 and dz0
+        self.classifier_in = None  # the last ConvRelu's output, which the 1x1 classifier reads
         total_c = sum(m.num_features for m in net.modules() if isinstance(m, nn.BatchNorm2d))
         n_bn = sum(1 for m in net.modules() if isinstance(m, nn.BatchNorm2d))
         self._stats_arena = torch.zeros(2 * total_c, dtype=F32, device=self.dev)
@@ -404,6 +417,7 @@ class Plan:
         net = self.net
         conv = conv_relu.conv
         y = self._conv_relu(x1, skip, conv, label)
+        self.classifier_in = y
         fw, fb = net._vec(net.final.weight, net._p32), net._vec(net.final.bias, net._p32)
         self.fwd_ops.add("final_conv", lambda: ops.final_conv_fwd(y, fw, fb, self.logits),
                          2.0 * self.logits.numel() * 32, _nb(y, self.logits))
@@ -549,11 +563,14 @@ class ResNetPlan(Plan):
             a0 = z0
         c1 = self.act(n, h // 4, w // 4, 64)
         F.add("maxpool", lambda: ops.maxpool2_fwd(a0, c1), 0, _nb(a0, c1))
+        if self.training:
+            self.stem_parts.update(col=col, z0=z0, a0=a0, c1=c1, bn0=bn0)
 
         def build_stem(B):
             d_a0 = self.gbuf(a0)
             d_c1 = self.gbuf(c1)
             dz0 = self.act(*z0.shape)
+            self.stem_parts["dz0"] = dz0
             stem_gw = torch.zeros((1, 64, 192), dtype=F32, device=self.dev)
             self._keep.append(stem_gw)
             stem_g = net._vec(enc.conv1.weight, net._g32)
@@ -577,8 +594,9 @@ class ResNetPlan(Plan):
         for li, layer in enumerate((enc.layer1, enc.layer2, enc.layer3, enc.layer4)):
             for bi, blk in enumerate(layer):
                 xin = x
-                x = self._res_block(x, blk, "layer%d" % (li + 1))
-                self.units.append(("block", "encoder.layer%d.%d" % (li + 1, bi), (xin,), x))
+                prefix = "encoder.layer%d.%d" % (li + 1, bi)
+                x = self._res_block(x, blk, "layer%d" % (li + 1), prefix)
+                self.units.append(("block", prefix, (xin,), x))
             skips.append(x)
         c2, c3, c4, c5 = skips
 
@@ -603,10 +621,11 @@ class ResNetPlan(Plan):
         # dec0 = ConvRelu(32, 32): unlabelled, its weight gradient on the main stream
         self._classifier(d1, None, net.dec0, label=False, side=False)
 
-    def _res_block(self, x, blk, tag):
-        """torchvision BasicBlock / Bottleneck forward + backward plan"""
+    def _res_block(self, x, blk, tag, prefix):
+        """torchvision BasicBlock / Bottleneck forward + backward plan; `prefix`: the block's state_dict prefix"""
         is_bottleneck = hasattr(blk, "conv3")
         convs = [(blk.conv1, blk.bn1), (blk.conv2, blk.bn2)] + ([(blk.conv3, blk.bn3)] if is_bottleneck else [])
+        names = [("%s.conv%d" % (prefix, i), "%s.bn%d" % (prefix, i)) for i in range(1, len(convs) + 1)]
         if not self.training:
             cur = x
             for conv, bnm in convs[:-1]:
@@ -617,21 +636,26 @@ class ResNetPlan(Plan):
             out, _, _ = self.conv_bn(cur, convs[-1][0], convs[-1][1], True, residual=ident)
             return out
         units = []
+        parts = []
         cur = x
-        for conv, bnm in convs[:-1]:
+        for (conv, bnm), (cname, bname) in zip(convs[:-1], names):
             y, z, bn = self.conv_bn(cur, conv, bnm, True)
             units.append((conv, cur, y, z, bn))
+            parts.append(_ConvPart(cname, bname, cur, z, y, bn))
             cur = y
         conv_l, bn_l = convs[-1]
         _, z_l, bnl = self.conv_bn(cur, conv_l, bn_l, None)
+        parts.append(_ConvPart(names[-1][0], names[-1][1], cur, z_l, None, bnl))
         out = self.act(*z_l.shape)
         if blk.downsample is not None:
             dconv, dbnm = blk.downsample[0], blk.downsample[1]
             _, zd, bnd = self.conv_bn(x, dconv, dbnm, None)
+            parts.append(_ConvPart(prefix + ".downsample.0", prefix + ".downsample.1", x, zd, None, bnd))
             self.bn_apply_op(z_l, bnl, out, True, zd, bnd)
         else:
             self.bn_apply_op(z_l, bnl, out, True, x)
         last_in = cur
+        self.block_parts[id(out)] = parts
 
         def build_block(B):
             d_out = self.gbuf(out)
@@ -642,17 +666,20 @@ class ResNetPlan(Plan):
                 dz_l = self.conv_unit_backward(B, d_out, out, z_l, bnl, conv_l, last_in, g_out=gx, g_out_acc=acc)
             else:
                 dz_l = self.conv_unit_backward(B, d_out, out, z_l, bnl, conv_l, last_in)
+            parts[len(units)].dz = dz_l
             # walk back through the inner units
             dz = dz_l
             conv_next = conv_l
-            for conv, xin, y, z, bn in reversed(units):
+            for i, (conv, xin, y, z, bn) in reversed(list(enumerate(units))):
                 # y has a single consumer: its ReLU mask and its BN's backward reductions ride in the dgrad epilogue
                 self.dgrad_into(B, dz, conv_next, y, bn_reduce=(z, bn))
                 dz = self.conv_unit_backward(B, self.gbuf(y), None, z, bn, conv, xin, reduced=True)
+                parts[i].dz = dz
                 conv_next = conv
             self.dgrad_into(B, dz, conv_next, x)
             if blk.downsample is not None:
                 dzd = self.conv_unit_backward(B, d_out, out, zd, bnd, dconv, x)
+                parts[-1].dz = dzd
                 self.dgrad_into(B, dzd, dconv, x)
         self.on_backward(tag, build_block)
         return out
