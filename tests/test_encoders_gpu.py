@@ -22,7 +22,8 @@ import torch
 from oracle import synthetic
 from oracle import unet_oracle as O
 from oracle.make_golden_cases import LOGIT_STRIDE
-from oracle.make_golden_encoders import DEVIATION_JSON, ENCODER_CASES, ENCODER_GRAD_HEAD, SEED, STEP_HEAD, golden_path
+from oracle.make_golden_encoders import DEVIATION_JSON, ENCODER_CASES, ENCODER_GRAD_HEAD, SEED, STEP_HEAD
+from oracle.step_checks import gold, host_nchw, rel_l2
 
 pytestmark = pytest.mark.gpu
 LOGIT_TOL = 1e-3   # BASELINE.json north_star
@@ -32,11 +33,6 @@ CASES = [c[0] for c in ENCODER_CASES]
 
 def _case(tag):
     return next(c for c in ENCODER_CASES if c[0] == tag)
-
-
-def _gold(tag):
-    with np.load(golden_path(tag)) as g:
-        return {k: g[k] for k in g.files}
 
 
 def _logit_bound(emulated):
@@ -49,17 +45,12 @@ def _seeded(depth):
         return O.make_reference_like_state_dict(depth, seed=SEED)
 
 
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-300))
-
-
 @pytest.mark.parametrize("tag", CASES)
 def test_logits_loss_and_gradients_against_reference(mcb, cuda, tag):
     from mcb200 import models
     from mcb200.unet_models import AlbuNet
     _, enc, depth, n, s = _case(tag)
-    g = _gold(tag)
+    g = gold(tag)
     emu = json.load(open(DEVIATION_JSON))[tag]
     st = LOGIT_STRIDE
     x, t = synthetic.train_batch(n, s, seed=SEED)
@@ -90,7 +81,7 @@ def test_logits_loss_and_gradients_against_reference(mcb, cuda, tag):
     for k, e in sorted(emu["grads"].items()):
         got = params[k].grad.detach().cpu().contiguous().reshape(-1)[:ENCODER_GRAD_HEAD]
         assert bool(torch.isfinite(got).all()), k
-        rel = _rel(got, torch.from_numpy(g["grad_" + k]))
+        rel = rel_l2(got, torch.from_numpy(g["grad_" + k]))
         print("    grad %-34s rel %.3e (emulated %.3e)" % (k, rel, e["rel"]))
         if e["rel"] <= REPRODUCIBLE_REL:
             assert rel <= 1.15 * e["rel"] + 0.01, (k, rel, e["rel"])
@@ -98,10 +89,6 @@ def test_logits_loss_and_gradients_against_reference(mcb, cuda, tag):
         else:
             assert rel < 1.0, (k, rel, e["rel"])     # still the reference's gradient, not noise
     assert bounded >= 6     # dec2, dec1, dec0 and the classifier
-
-
-def _nchw(t):
-    return t.permute(0, 3, 1, 2).float().cpu()
 
 
 def test_every_unit_against_bf16_emulated_oracle(mcb, cuda):
@@ -127,19 +114,19 @@ def test_every_unit_against_bf16_emulated_oracle(mcb, cuda):
         for k in keys:
             leaves[k].requires_grad_(True)
         orc = O.UNetOracle(leaves, depth, update_running_stats=False, emulate_bf16=True)
-        xin = [_nchw(a) for a in ins]
+        xin = [host_nchw(a) for a in ins]
         if kind == "block":
             li = int(prefix.split("layer")[1][0])
             y = orc._block(xin[0], prefix, 2 if (prefix in first_of_layer and li > 1) else 1, True)
         else:
             y = orc._decoder(torch.cat(xin, 1) if len(xin) > 1 else xin[0], prefix)
-        assert _rel(_nchw(out), y.detach()) < 1.5e-2, (prefix, "forward")
-        g_out = _nchw(plan.grad[id(out)])
+        assert rel_l2(host_nchw(out), y.detach()) < 1.5e-2, (prefix, "forward")
+        g_out = host_nchw(plan.grad[id(out)])
         if kind == "decoder":
             g_out = g_out * (y.detach() > 0)   # decoder gradients are stored already masked by the unit's ReLU
         grads = torch.autograd.grad(y, [leaves[k] for k in keys], g_out)
         for k, gr in zip(keys, grads):
-            assert _rel(params[k].grad.detach(), gr) < 8e-2, (prefix, k)
+            assert rel_l2(params[k].grad.detach(), gr) < 8e-2, (prefix, k)
             checked += 1
     assert len(plan.units) == 16 + 6 and checked > 2 * len(plan.units)
 
@@ -149,7 +136,7 @@ def test_fused_fit_loop_step_against_reference(mcb, cuda):
     import bench
     from mcb200.models import PyTorchUNetWeighted
     tag, enc, depth, n, s = ENCODER_CASES[0]
-    g = _gold(tag)
+    g = gold(tag)
     sd = _seeded(depth)
     with torch.random.fork_rng():
         model = PyTorchUNetWeighted(**bench.unet_config(enc))
@@ -180,7 +167,7 @@ def test_fused_fit_loop_step_against_reference(mcb, cuda):
         ref = torch.from_numpy(g["step_" + k])
         assert torch.allclose(got[k].cpu().reshape(-1)[:STEP_HEAD], ref, rtol=2e-2, atol=1e-3), k
     for k in ("encoder.layer4.2.bn2.running_mean", "encoder.layer4.2.bn2.running_var"):
-        rel = _rel(got[k].reshape(-1)[:STEP_HEAD], torch.from_numpy(g["step_" + k]))
+        rel = rel_l2(got[k].reshape(-1)[:STEP_HEAD], torch.from_numpy(g["step_" + k]))
         print("    step %-34s rel %.2e" % (k, rel))
         assert rel < 1.0, (k, rel)
     assert all(bool(torch.isfinite(v).all()) for v in got.values() if v.is_floating_point())
@@ -223,7 +210,7 @@ def test_save_load_transform_round_trip(mcb, cuda, tmp_path):
         m.save(path)
         saved = torch.load(path)
         m2 = PyTorchUNetWeighted(**bench.unet_config("AlbuNet"))
-    g = _gold(ENCODER_CASES[0][0])
+    g = gold(ENCODER_CASES[0][0])
     assert sorted(saved) == sorted("module." + str(k) for k in g["init_keys"])
     m2.load(path)
     ref = m._net().state_dict()

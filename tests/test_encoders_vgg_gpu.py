@@ -30,8 +30,9 @@ import torch
 from oracle import synthetic
 from oracle import vgg_oracle as V
 from oracle.make_golden_cases import LOGIT_STRIDE
-from oracle.make_golden_encoders import ENCODER_GRAD_HEAD, SEED, STEP_HEAD, golden_path
+from oracle.make_golden_encoders import ENCODER_GRAD_HEAD, SEED, STEP_HEAD
 from oracle.make_golden_vgg import DEVIATION_JSON, VGG_CASES
+from oracle.step_checks import gold, host_nchw, rel_l2
 
 pytestmark = pytest.mark.gpu
 LOGIT_TOL = 1e-3
@@ -45,11 +46,6 @@ LR, WD = 5e-4, 1e-4
 
 def _case(tag):
     return next(c for c in VGG_CASES if c[0] == tag)
-
-
-def _gold(tag):
-    with np.load(golden_path(tag)) as g:
-        return {k: g[k] for k in g.files}
 
 
 def _net(enc):
@@ -68,16 +64,11 @@ def _logit_bound(emulated):
     return LOGIT_TOL if emulated <= 0.5 * LOGIT_TOL else max(LOGIT_TOL, 2.0 * emulated)
 
 
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-300))
-
-
 @pytest.mark.parametrize("tag", CASES)
 def test_logits_loss_and_gradients_against_reference(mcb, cuda, tag):
     from mcb200 import models
     _, enc, n, s = _case(tag)
-    g = _gold(tag)
+    g = gold(tag)
     emu = json.load(open(DEVIATION_JSON))[tag]
     st = LOGIT_STRIDE
     x, t = synthetic.train_batch(n, s, seed=SEED)
@@ -107,7 +98,7 @@ def test_logits_loss_and_gradients_against_reference(mcb, cuda, tag):
     for k, e in sorted(emu["grads"].items()):
         got = params[k].grad.detach().cpu().contiguous().reshape(-1)[:ENCODER_GRAD_HEAD]
         assert bool(torch.isfinite(got).all()), k
-        rel = _rel(got, torch.from_numpy(g["grad_" + k]))
+        rel = rel_l2(got, torch.from_numpy(g["grad_" + k]))
         print("    grad %-30s rel %.3e (emulated %.3e)" % (k, rel, e["rel"]))
         if (tag, k) in GRAD_EXCEPTIONS:
             assert rel <= 2.0 * e["rel"] + 0.01, (k, rel, e["rel"])
@@ -118,10 +109,6 @@ def test_logits_loss_and_gradients_against_reference(mcb, cuda, tag):
             assert rel < 1.0, (k, rel, e["rel"])     # still the reference's gradient, not noise
     # the input conv, the middle encoder conv, dec4's transposed conv, dec3 .. classifier (one exception at UNetVGG16)
     assert bounded == 10 - sum(1 for c, _ in GRAD_EXCEPTIONS if c == tag), bounded
-
-
-def _nchw(t):
-    return t.permute(0, 3, 1, 2).float().cpu()
 
 
 @pytest.mark.parametrize("tag", CASES)
@@ -147,23 +134,23 @@ def test_every_unit_against_bf16_emulated_oracle(mcb, cuda, tag):
         orc = V.VGGUNetOracle(leaves, enc, emulate_bf16=True)
         if kind == "conv":
             # the input conv reads the image, rounded to bf16 by the im2col
-            xin = _nchw(ins[0]) if ins else plan.x_in.cpu().to(torch.bfloat16).float()
+            xin = host_nchw(ins[0]) if ins else plan.x_in.cpu().to(torch.bfloat16).float()
             y = orc._conv_relu(xin, prefix)
         elif prefix == "dec1":
-            y = orc._conv_relu(torch.cat([_nchw(a) for a in ins], 1), "dec1.conv")
+            y = orc._conv_relu(torch.cat([host_nchw(a) for a in ins], 1), "dec1.conv")
         else:
-            y = orc._decoder(torch.cat([_nchw(a) for a in ins], 1) if len(ins) > 1 else _nchw(ins[0]), prefix)
-        fwd = _rel(_nchw(out), y.detach())
+            y = orc._decoder(torch.cat([host_nchw(a) for a in ins], 1) if len(ins) > 1 else host_nchw(ins[0]), prefix)
+        fwd = rel_l2(host_nchw(out), y.detach())
         assert fwd < 1.5e-2, (prefix, "forward", fwd)
         # every stored output gradient is complete and already masked by the unit's own ReLU (dgrad epilogue, pool-skip
         # kernel or classifier backward); autograd through the oracle's ReLU masks it again, a no-op but at the
         # elements where the two forwards round to different sides of zero
-        g_out = _nchw(plan.grad[id(out)])
+        g_out = host_nchw(plan.grad[id(out)])
         unmasked = float(((g_out != 0) & (y.detach() == 0)).float().mean())
         assert unmasked < 1e-3, (prefix, "ReLU mask", unmasked)
         grads = torch.autograd.grad(y, [leaves[k] for k in keys], g_out)
         for k, gr in zip(keys, grads):
-            rel = _rel(params[k].grad.detach(), gr)
+            rel = rel_l2(params[k].grad.detach(), gr)
             worst[k] = rel
             assert rel < 2e-2, (prefix, k, rel)
             checked += 1
@@ -182,7 +169,7 @@ def _fused(net, n, s):
 def test_fused_train_step_against_reference_fit_loop(mcb, cuda, tag):
     """one FusedTrainStep (forward -> loss -> backward -> in-graph Adam) against the reference's _fit_loop"""
     _, enc, n, s = _case(tag)
-    g = _gold(tag)
+    g = gold(tag)
     sd = _seeded(enc)
     net = _net(enc)
     net.load_state_dict(sd)

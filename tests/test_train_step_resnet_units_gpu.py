@@ -43,51 +43,21 @@ and the data gradients 0.96 .. 0.996 (the bf16 rounding of the output itself), B
 statistics 0.005, dbeta / dgamma 0.006, weight gradients 0.30 (dec0), bias and classifier sums 0.005, max-pool exact.
 The largest |mean| / std of a pre-BN channel is 4.99 (ResNet101's layer1.0 downsample; ResNet34: 4.02, layer1.0.bn1),
 and the worst relative invstd error is 2^-19.5 (ResNet34: 2^-20.1): the one-pass variance is well inside its bound."""
-import gc
-import time
-
 import pytest
 import torch
 import torch.nn.functional as F
 
-import bench
-import bench_data
-from oracle import unet_oracle as O
+from oracle.step_checks import N, RESNET_DEPTH, SEED, STATS, BenchStep, batch, free_device_memory, seeded_sd
+from oracle.step_checks import rng_and_peak_memory  # noqa: F401  (fixture)
 from oracle.unit_checks import (CHUNK, SAMPLE, WGRAD_ACC, Bounds, check_conv_half, f64, grad_view, nchw,
                                 wgrad64)
 
 pytestmark = pytest.mark.gpu
 
-DEPTH = {"ResNet101": 101, "ResNet34": 34}
-N, S = 32, 320            # bench.py's train batch and net input
-SEED = 1234
 REL = 2.0 ** -8           # bf16 rounding of a stored output (and its share of what the reference rounds away)
 TERMS = 2.0 ** -20        # fp32 rounding of the BN apply's affine terms
 INVSTD_REL = 2.0 ** -12
 MEAN_ACC = 2.0 ** -16
-
-
-@pytest.fixture(autouse=True)
-def _rng_and_peak_memory(cuda):
-    """leave torch's generators as the other tests expect them; report the device and the peak memory of each test"""
-    with torch.random.fork_rng(devices=[cuda]):
-        torch.cuda.reset_peak_memory_stats(cuda)
-        t0 = time.time()
-        yield
-    print("\n[%s] peak device memory %.1f GiB, %.0f s" % (torch.cuda.get_device_name(cuda),
-                                                           torch.cuda.max_memory_allocated(cuda) / 2 ** 30,
-                                                           time.time() - t0))
-
-
-def free_device_memory():
-    gc.collect()               # launch plans hold their closures in reference cycles
-    torch.cuda.synchronize()
-    torch.cuda.empty_cache()
-
-
-def batch(seed):
-    x, t = bench_data.train_batch(N, S, seed=seed)
-    return torch.from_numpy(x), torch.from_numpy(t)
 
 
 class Step:
@@ -95,28 +65,23 @@ class Step:
     and fp32 parameters (float64 on the device, by parameter name) and running statistics"""
 
     def __init__(self, enc, cuda):
-        from mcb200.models import PyTorchUNetWeighted
         from mcb200 import engine
         self.momentum, self.eps = engine.BN_MOMENTUM, engine.BN_EPS
-        with torch.random.fork_rng(devices=[]):
-            sd = O.make_reference_like_state_dict(DEPTH[enc], seed=SEED)
-        model = PyTorchUNetWeighted(**bench.unet_config(enc))
-        model.model.load_state_dict(sd)
-        model._to_device()
-        net = model._net()
+        run = BenchStep(enc, seeded_sd(enc), cuda)
+        net = run.net
         X, T = (t.to(cuda) for t in batch(SEED))
-        model._fit_loop([X, T])
+        run.step(X, T)
         X, T = (t.to(cuda) for t in batch(SEED + 1))
         torch.cuda.synchronize()
         w16, p32 = net._w16.clone(), net._p32.clone()
-        self.stats_pre = {k: f64(b) for k, b in net.named_buffers() if k.endswith(("running_mean", "running_var"))}
-        model._fit_loop([X, T])
+        self.stats_pre = {k: f64(b) for k, b in net.named_buffers() if k.endswith(STATS)}
+        run.step(X, T)
         torch.cuda.synchronize()
-        assert model._fused.graphs is not None and model._opt_state.t == 2, "the second step must be a graph replay"
+        assert run.fused.graphs is not None and run.fused.opt.t == 2, "the second step must be a graph replay"
         self.w = {name: f64(net._view(w16, net._slots[id(p)])) for name, p, _ in net._arena_params()}
         self.p = {name: f64(net._view(p32, net._slots[id(p)])) for name, p, _ in net._arena_params()}
         del w16, p32, X, T
-        self.model, self.net, self.plan = model, net, model._fused.plan
+        self.run, self.net, self.plan = run, net, run.fused.plan
 
     def mod(self, name):
         return self.net.get_submodule(name)
@@ -273,7 +238,7 @@ def routed(x, g):
     return F.max_unpool2d(g, where, 2, 2, output_size=x.shape[2:])
 
 
-@pytest.mark.parametrize("enc", list(DEPTH))
+@pytest.mark.parametrize("enc", list(RESNET_DEPTH))
 def test_every_unit_against_float64(mcb, cuda, enc):
     st = Step(enc, cuda)
     net, plan = st.net, st.plan

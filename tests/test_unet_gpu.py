@@ -11,15 +11,11 @@ import torch
 
 from oracle import synthetic
 from oracle import unet_oracle as O
+from oracle.step_checks import host_nchw, rel_l2
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 LOGIT_TOL = 1e-3  # BASELINE.json north_star: "within 1e-3 max-abs on logits"
-
-
-def rel(a, b):
-    a, b = a.detach().float().cpu(), b.detach().float().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-20))
 
 
 @pytest.fixture(scope="module")
@@ -67,11 +63,7 @@ def test_train_logits_and_loss_match_reference_golden(setup34, cuda):
             # at 2x64x64 the deep layers see 2..32 samples per BatchNorm channel: their gradients are chaotic under any
             # bf16 storage (see DESIGN.md section 3); the decoder tail is well conditioned and must match tightly
             if k.startswith(("final", "dec0", "dec1")):
-                assert rel(got, ref) < 2e-2, (k, rel(got, ref))
-
-
-def _nchw(t):
-    return t.permute(0, 3, 1, 2).float().cpu()
+                assert rel_l2(got, ref) < 2e-2, (k, rel_l2(got, ref))
 
 
 @pytest.mark.parametrize("depth,n,s", [(34, 4, 128), (101, 2, 128)])
@@ -100,17 +92,17 @@ def test_every_unit_against_bf16_emulated_oracle(mcb, cuda, depth, n, s):
             return sd[k].is_floating_point() and not k.endswith(("running_mean", "running_var"))
         leaves = {k: sd[k].clone().requires_grad_(is_param(k)) for k in keys}
         orc = O.UNetOracle(leaves, depth, update_running_stats=False, emulate_bf16=True)
-        xin = [_nchw(a).requires_grad_(True) for a in ins]
+        xin = [host_nchw(a).requires_grad_(True) for a in ins]
         if kind == "block":
             li = int(prefix.split("layer")[1][0])
             stride = 2 if (prefix in first_of_layer and li > 1) else 1
             y = orc._block(xin[0], prefix, stride, True)
         else:
             y = orc._decoder(torch.cat(xin, 1) if len(xin) > 1 else xin[0], prefix)
-        got = _nchw(out)
-        assert rel(got, y) < 1.5e-2, (prefix, "forward", rel(got, y))
+        got = host_nchw(out)
+        assert rel_l2(got, y) < 1.5e-2, (prefix, "forward", rel_l2(got, y))
         # backward of this unit from the CUDA path's own output gradient
-        g_out = _nchw(plan.grad[id(out)])
+        g_out = host_nchw(plan.grad[id(out)])
         if kind == "decoder":
             g_out = g_out * (y.detach() > 0)  # decoder gradients are stored already masked by the unit's ReLU
             yy = y
@@ -131,14 +123,14 @@ def test_every_unit_against_bf16_emulated_oracle(mcb, cuda, depth, n, s):
                 single_consumer = (kind == "block" and prefix not in first_of_layer) or (kind == "decoder" and nm == "x0")
                 if not single_consumer or id(a) not in plan.grad:
                     continue  # skip tensors also receive gradient from other consumers
-                gg = _nchw(plan.grad[id(a)])
+                gg = host_nchw(plan.grad[id(a)])
                 if kind == "decoder" and prefix != "center":
                     gr = gr * (xin[0].detach() > 0)  # stored masked by the producer's ReLU
                 tol = 4e-2
             else:
                 gg = params[nm].grad.detach().cpu()
                 tol = 8e-2  # bf16 operands, fp32 accumulation; deep layers see only a few dozen samples per channel here
-            r = rel(gg, gr)
+            r = rel_l2(gg, gr)
             assert r < tol, (prefix, nm, r)
             checked += 1
     assert checked > 5 * len(plan.units) // 2
@@ -146,8 +138,8 @@ def test_every_unit_against_bf16_emulated_oracle(mcb, cuda, depth, n, s):
     sd_o = {k: v.clone() for k, v in sd.items()}
     ref_logits = O.UNetOracle(sd_o, depth, update_running_stats=True, emulate_bf16=True).forward(X, training=True)
     assert float((logits.detach().cpu() - ref_logits).abs().max()) < LOGIT_TOL
-    assert rel(net.encoder.bn1.running_mean, sd_o["encoder.bn1.running_mean"]) < 1e-2
-    assert rel(net.encoder.bn1.running_var, sd_o["encoder.bn1.running_var"]) < 1e-2
+    assert rel_l2(net.encoder.bn1.running_mean, sd_o["encoder.bn1.running_mean"]) < 1e-2
+    assert rel_l2(net.encoder.bn1.running_var, sd_o["encoder.bn1.running_var"]) < 1e-2
 
 
 def test_state_dict_roundtrip_and_module_prefix(setup34, cuda, tmp_path):
