@@ -69,9 +69,11 @@ class _BN:
 
 
 class _ConvPart:
-    """one conv + BatchNorm of a ResNet block in a training plan, for per-unit tests: the state_dict prefixes of the
-    conv and its BatchNorm, the conv's input x and output z, the BatchNorm output y (None for the block's last conv and
-    its downsample, whose BatchNorms the residual pass applies), the _BN state and the backward's dz buffer"""
+    """one conv + BatchNorm of a ResNet block, for per-unit tests: the state_dict prefixes of the conv and its
+    BatchNorm, the conv's input x and output z, the BatchNorm output y, the _BN state and the backward's dz buffer.
+    Training: y is None for the block's last conv and its downsample, whose BatchNorms the residual pass applies.
+    Inference: the BatchNorm (and the residual, the ReLU) is folded into the conv epilogue, so y is z, the stored
+    output, and dz stays None"""
     __slots__ = ("conv", "bn", "x", "z", "y", "state", "dz")
 
     def __init__(self, conv, bn, x, z, y, state):
@@ -95,8 +97,9 @@ class Plan:
         self._bwd_builders = []    # (tag, builder) per forward unit; run in REVERSE so store/accumulate modes follow run order
         self.units = []            # (kind, state_dict prefix, inputs, output) per forward unit, for per-unit parity tests
         self.dec_mid = {}          # id(decoder block output) -> the block's middle ConvRelu output, for the same tests
-        self.block_parts = {}      # training ResNet plans: id(block output) -> [_ConvPart], conv1 .. [downsample]
-        self.stem_parts = {}       # training ResNet plans: the stem's col, z0, a0, c1, bn0 and dz0
+        self.block_parts = {}      # ResNet plans: id(block output) -> [_ConvPart], conv1 .. [downsample]
+        self.stem_parts = {}       # ResNet plans: the stem's col, z0, a0, c1, bn0 (and dz0 when training; z0 is a0
+        #                            when not: the inference stem folds its BatchNorm and ReLU into the GEMM)
         self.classifier_in = None  # the last ConvRelu's output, which the 1x1 classifier reads
         total_c = sum(m.num_features for m in net.modules() if isinstance(m, nn.BatchNorm2d))
         n_bn = sum(1 for m in net.modules() if isinstance(m, nn.BatchNorm2d))
@@ -563,8 +566,7 @@ class ResNetPlan(Plan):
             a0 = z0
         c1 = self.act(n, h // 4, w // 4, 64)
         F.add("maxpool", lambda: ops.maxpool2_fwd(a0, c1), 0, _nb(a0, c1))
-        if self.training:
-            self.stem_parts.update(col=col, z0=z0, a0=a0, c1=c1, bn0=bn0)
+        self.stem_parts.update(col=col, z0=z0, a0=a0, c1=c1, bn0=bn0)
 
         def build_stem(B):
             d_a0 = self.gbuf(a0)
@@ -627,13 +629,21 @@ class ResNetPlan(Plan):
         convs = [(blk.conv1, blk.bn1), (blk.conv2, blk.bn2)] + ([(blk.conv3, blk.bn3)] if is_bottleneck else [])
         names = [("%s.conv%d" % (prefix, i), "%s.bn%d" % (prefix, i)) for i in range(1, len(convs) + 1)]
         if not self.training:
+            # every conv's output is its folded BatchNorm's output: the parts record it as both z and y
+            parts = []
             cur = x
-            for conv, bnm in convs[:-1]:
-                cur, _, _ = self.conv_bn(cur, conv, bnm, True)
+            for (conv, bnm), (cname, bname) in zip(convs[:-1], names):
+                y, _, bn = self.conv_bn(cur, conv, bnm, True)
+                parts.append(_ConvPart(cname, bname, cur, y, y, bn))
+                cur = y
             ident = x
+            down = None
             if blk.downsample is not None:
-                ident, _, _ = self.conv_bn(x, blk.downsample[0], blk.downsample[1], False)
-            out, _, _ = self.conv_bn(cur, convs[-1][0], convs[-1][1], True, residual=ident)
+                ident, _, bnd = self.conv_bn(x, blk.downsample[0], blk.downsample[1], False)
+                down = _ConvPart(prefix + ".downsample.0", prefix + ".downsample.1", x, ident, ident, bnd)
+            out, _, bnl = self.conv_bn(cur, convs[-1][0], convs[-1][1], True, residual=ident)
+            parts.append(_ConvPart(names[-1][0], names[-1][1], cur, out, out, bnl))
+            self.block_parts[id(out)] = parts + ([down] if down is not None else [])
             return out
         units = []
         parts = []

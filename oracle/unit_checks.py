@@ -1,13 +1,15 @@
-"""Float64 references of single plan units on the train step's own buffers, shared by the batch-32 unit tests
-(tests/test_train_step_vgg_scale_gpu.py, tests/test_train_step_resnet_units_gpu.py).
+"""Float64 references of single plan units on a plan's own buffers, shared by the unit tests of the batch-32 train step
+(tests/test_train_step_vgg_scale_gpu.py, tests/test_train_step_resnet_units_gpu.py) and of the batch-64 inference
+forward (tests/test_infer_forward_units_gpu.py).
 
 Activations and gradients are the plan's NHWC bf16 buffers; every reference is evaluated in float64 on their device.
 Bounds are element-wise, |got - ref| <= rel |ref| + acc A + extra, with A the same operation on absolute values."""
 import torch
 import torch.nn.functional as F
 
-SAMPLE = (0, 10, 21, 31)  # images of the element-wise forward and data-gradient checks (the reductions take all 32)
-CHUNK = 8                 # images per float64 weight-gradient evaluation (their sums are added in float64)
+SAMPLE = (0, 10, 21, 31)  # images of the train step's element-wise forward and data-gradient checks (the reductions
+#                           take all 32)
+CHUNK = 8                 # images per float64 evaluation over a whole batch (sums over the chunks added in float64)
 # accumulation allowance of the weight gradients.  Their reductions run over all 3.3 M pixels of the batch, and the
 # split-K GEMM caps its splits at one wave of CTAs, so one fp32 accumulator chain adds up to k = 12800 pixel tiles x 4
 # MMA steps (VGG's dec1: 4 splits).  The a-priori bound of such a chain, k 2^-24 A, is 2^-8.4 A, and the rounding
@@ -86,11 +88,27 @@ def check_bias(bd, what, got, g):
     bd.check(what[0], what[1], got, ref, absref)
 
 
-def check_conv_half(bd, net, w16, b32, prefix, wkey, bkey, x, y, g, bias_from, transposed=False):
-    """one conv (or stride-2 transposed conv) + bias + ReLU: x the NCHW bf16 input, y and g the NHWC stored output and
-    output gradient; w16 / b32 the pre-step bf16 weight and fp32 bias (float64 on the device)"""
-    w, b = w16[wkey], b32[bkey]
-    xs = f64(x[list(SAMPLE)])
+def conv_kw(conv):
+    return dict(stride=conv.stride, padding=conv.padding)
+
+
+def conv_ref(x, w, conv):
+    """float64 conv2d of x with w as the nn.Conv2d `conv` runs it, and the same on absolute values"""
+    kw = conv_kw(conv)
+    return F.conv2d(x, w, **kw), F.conv2d(x.abs(), w.abs(), **kw)
+
+
+def bn_affine(p, bn_name, mean, invstd):
+    """float64 per-channel (scale, shift) of BatchNorm `bn_name` normalising with (mean, invstd); p: its fp32 gamma and
+    beta (float64 on the device), by parameter name.  Training passes the batch statistics, inference the running ones"""
+    sc = p[bn_name + ".weight"] * invstd
+    return sc, p[bn_name + ".bias"] - mean * sc
+
+
+def check_conv_forward(bd, prefix, x, y, w, b, transposed=False, images=SAMPLE):
+    """forward of one conv (or stride-2 transposed conv) + bias + ReLU on `images`: x the NCHW bf16 input, y the NHWC
+    stored output, w / b the bf16 weight and fp32 bias (float64 on the device).  |got - ref| <= 2^-8 |ref| + 2^-16 A"""
+    xs = f64(x[list(images)])
     if transposed:
         op = dict(stride=2, padding=1, output_padding=1 if w.shape[-1] == 3 else 0)
         ref = F.conv_transpose2d(xs, w, b, **op)
@@ -98,8 +116,16 @@ def check_conv_half(bd, net, w16, b32, prefix, wkey, bkey, x, y, g, bias_from, t
     else:
         ref = F.conv2d(xs, w, b, padding=1)
         absref = F.conv2d(xs.abs(), w.abs(), b.abs(), padding=1)
-    bd.check("forward", prefix, nchw(y)[list(SAMPLE)], ref.clamp_min(0), absref, rel=2.0 ** -8)
-    del xs, ref, absref
+    del xs
+    bd.check("forward", prefix, nchw(y)[list(images)], ref.clamp_min(0), absref, rel=2.0 ** -8)
+    del ref, absref
+
+
+def check_conv_half(bd, net, w16, b32, prefix, wkey, bkey, x, y, g, bias_from, transposed=False):
+    """one conv (or stride-2 transposed conv) + bias + ReLU: x the NCHW bf16 input, y and g the NHWC stored output and
+    output gradient; w16 / b32 the pre-step bf16 weight and fp32 bias (float64 on the device)"""
+    w = w16[wkey]
+    check_conv_forward(bd, prefix, x, y, w, b32[bkey], transposed)
     bd.zero_where_off(prefix + " ReLU mask", g, y)
     if transposed:     # d conv_transpose2d(x, W) / dW = conv2d weight gradient of the conv from the output back to x
         ref, absref = wgrad64(nchw(g), x, w.shape, stride=2, padding=1)

@@ -49,8 +49,8 @@ import torch.nn.functional as F
 
 from oracle.step_checks import N, RESNET_DEPTH, SEED, STATS, BenchStep, batch, free_device_memory, seeded_sd
 from oracle.step_checks import rng_and_peak_memory  # noqa: F401  (fixture)
-from oracle.unit_checks import (CHUNK, SAMPLE, WGRAD_ACC, Bounds, check_conv_half, f64, grad_view, nchw,
-                                wgrad64)
+from oracle.unit_checks import (CHUNK, SAMPLE, WGRAD_ACC, Bounds, bn_affine, check_conv_half, conv_kw, conv_ref, f64,
+                                grad_view, nchw, wgrad64)
 
 pytestmark = pytest.mark.gpu
 
@@ -85,15 +85,6 @@ class Step:
 
     def mod(self, name):
         return self.net.get_submodule(name)
-
-
-def conv_kw(conv):
-    return dict(stride=conv.stride, padding=conv.padding)
-
-
-def conv_ref(x, w, conv):
-    kw = conv_kw(conv)
-    return F.conv2d(x, w, **kw), F.conv2d(x.abs(), w.abs(), **kw)
 
 
 def dgrad_ref(shape, w, dz, conv):
@@ -138,10 +129,9 @@ def check_bn_forward(bd, st, report, bn_name, z, state):
     bd.check("running var", bn_name, bnm.running_var, rv_ref, 0.0, rel=INVSTD_REL)
 
 
-def bn_affine(st, bn_name, state):
+def step_affine(st, bn_name, state):
     """float64 (scale, shift) of a BatchNorm from the kernel's own mean / invstd and the pre-step gamma / beta"""
-    sc = st.p[bn_name + ".weight"] * f64(state.invstd)
-    return sc, st.p[bn_name + ".bias"] - f64(state.mean) * sc
+    return bn_affine(st.p, bn_name, f64(state.mean), f64(state.invstd))
 
 
 def check_bn_backward(bd, st, part, dy, ymask):
@@ -186,7 +176,7 @@ def check_conv_bn(bd, st, report, part, dy, ymask, x_nchw=None):
 
 def check_apply(bd, st, what, kind, y, z, bn_name, state, residual=None):
     """y = relu(bn(z) [+ residual]) over the whole batch; residual = ("x", x) or ("bn", z_d, bn name, state)"""
-    sc, sh = bn_affine(st, bn_name, state)
+    sc, sh = step_affine(st, bn_name, state)
     zz = f64(z)
     ref = zz * sc + sh
     terms = (zz * sc).abs() + (f64(state.mean) * sc).abs() + st.p[bn_name + ".bias"].abs()
@@ -196,7 +186,7 @@ def check_apply(bd, st, what, kind, y, z, bn_name, state, residual=None):
         ref, terms = ref + r, terms + r.abs()
         del r
     elif residual is not None:
-        rsc, rsh = bn_affine(st, residual[2], residual[3])
+        rsc, rsh = step_affine(st, residual[2], residual[3])
         r = f64(residual[1])
         ref = ref + r * rsc + rsh
         terms = terms + (r * rsc).abs() + (f64(residual[3].mean) * rsc).abs() + st.p[residual[2] + ".bias"].abs()
