@@ -501,6 +501,33 @@ int mcb_category_overlay(const uint8_t* cat_masks, const int* category_nr, int c
 int mcb_border_class(uint8_t* mask, const double* second_nearest, int n, int h, int w, double border_width,
                      void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * JPEG decode (csrc/jpeg.cu; the host side that parses the files and lays out these tables is mcb200.jpeg)
+ * Sequential Huffman JPEG, 8-bit, one scan, 1 or 3 components each sampled at 1 or 1/2 of the largest factor, bit-exact
+ * to libjpeg-turbo (islow IDCT, fancy upsampling).  All int32 tables are device memory:
+ *   images [n][36]   = ncomp, mcux, hmax, vmax, first segment, segment count, then per component (10 words): h, v, blocks_w, blocks_h, first block of
+ *                      the component in `coef` / `planes`, downsampled width, downsampled height, DC table slot, AC
+ *                      table slot (image * 8 + class * 4 + id), 0.  Blocks and segments of an image are consecutive,
+ *                      images in order.
+ *   segments [s][5]  = image, byte offset in `data`, byte count, first MCU, MCU count (an image, or one restart
+ *                      interval; bytes unstuffed, restart markers removed)
+ *   huff [slot][804] = 512 lookahead entries (length << 8 | symbol for codes of at most 9 bits, else 0), maxcode[18]
+ *                      by length (index 17 a sentinel), value offset[18] by length, symbols[256]
+ *   qt [n][3][64]    = quantisation tables in natural order, per component
+ *   tables [4][256]  = jdcolor.c's Cr->R, Cb->B, Cr->G, Cb->G tables
+ * ---------------------------------------------------------------------------------------------------------------- */
+/* entropy decode, one thread per segment, one CTA per image: coef int16 [blocks][64] (natural order, padding blocks of the MCUs included);
+ * status int32 [n] is zeroed, then set non-zero for an image whose data ends inside a segment (1), holds a code no table
+ * has (2) or runs a coefficient index past 63 (3).  No segment is read past its byte count. */
+int mcb_jpeg_entropy_decode(const uint8_t* data, const int* segments, int nseg, const int* images, const int* huff,
+                            int n, int16_t* coef, int* status, void* stream);
+/* dequantisation + libjpeg's jpeg_idct_islow per block -> planes uint8 [blocks][8][8] */
+int mcb_jpeg_idct(const int16_t* coef, const int* qt, const int* images, int n, int n_blocks, uint8_t* planes,
+                  void* stream);
+/* libjpeg-turbo's fancy upsampling + ycc_rgb_convert (grayscale replicated) -> out uint8 [n][h][w][3] */
+int mcb_jpeg_upsample_rgb(const uint8_t* planes, const int* images, const int* tables, int n, int h, int w,
+                          uint8_t* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

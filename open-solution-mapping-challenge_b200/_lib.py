@@ -226,6 +226,15 @@ for _n, _a in _SIGS7.items():
     getattr(lib, _n).argtypes = _a
     getattr(lib, _n).restype = ci
 
+_SIGS8 = {
+    "mcb_jpeg_entropy_decode": [vp, vp, ci, vp, vp, ci, vp, vp, vp],
+    "mcb_jpeg_idct": [vp, vp, vp, ci, ci, vp, vp],
+    "mcb_jpeg_upsample_rgb": [vp, vp, vp, ci, ci, ci, vp, vp],
+}
+for _n, _a in _SIGS8.items():
+    getattr(lib, _n).argtypes = _a
+    getattr(lib, _n).restype = ci
+
 lib.mcb_sync_step_bump.argtypes = [vp, vp]
 lib.mcb_sync_step_bump.restype = ci
 lib.mcb_sync_exchange.argtypes = [vp, vp, ci, ci, cl, cl, ci, vp, vp, vp, vp, ci, cf, vp]
