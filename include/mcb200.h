@@ -521,6 +521,24 @@ int mcb_border_class(uint8_t* mask, const double* second_nearest, int n, int h, 
  * has (2) or runs a coefficient index past 63 (3).  No segment is read past its byte count. */
 int mcb_jpeg_entropy_decode(const uint8_t* data, const int* segments, int nseg, const int* images, const int* huff,
                             int n, int16_t* coef, int* status, void* stream);
+/* bits per subsequence of the parallel entropy decode (a compile-time constant of the library) */
+int mcb_jpeg_subsequence_bits(void);
+/* entropy decode with the same inputs and the same coef and status as mcb_jpeg_entropy_decode, parallel inside each
+ * segment: a segment of B bytes is cut into S = mcb_jpeg_subsequence_bits()-bit subsequences, decoded speculatively,
+ * resolved in order (a guess that proves wrong is decoded again, so a stream that never resynchronises costs about
+ * one serial decode) and written out; a segment given one subsequence is decoded whole by one thread.  Three launches,
+ * no memset, no allocation, no host synchronisation; capturable into a CUDA graph.  A segment must be shorter than
+ * 2^28 bytes, and one image may have at most 65535 * 128 subsequences.
+ *   sub_first int32 [nseg + 1]  first subsequence of each segment, numbered across the batch (prefix sum of the counts);
+ *                               a segment's count is 1 or ceil(8 * B / S) (mcb200.jpeg splits segments of more than 16)
+ *   max_image_subs              the most subsequences of any one image (sizes the grid)
+ *   workspace int32 [16 + 16 * sub_first[nseg]]  caller-owned; words 0..3 count the speculated entry states that held,
+ *                               were corrected, the longest run of consecutive corrections and the exact re-decodes
+ *                               of a segment's error or last block; the rest is per-subsequence state
+ * coef is fully written (every block zeroed first); status as mcb_jpeg_entropy_decode. */
+int mcb_jpeg_entropy_decode_parallel(const uint8_t* data, const int* segments, int nseg, const int* images,
+                                     const int* huff, int n, const int* sub_first, int max_image_subs, int* workspace,
+                                     int16_t* coef, int* status, void* stream);
 /* dequantisation + libjpeg's jpeg_idct_islow per block -> planes uint8 [blocks][8][8] */
 int mcb_jpeg_idct(const int16_t* coef, const int* qt, const int* images, int n, int n_blocks, uint8_t* planes,
                   void* stream);

@@ -228,6 +228,8 @@ for _n, _a in _SIGS7.items():
 
 _SIGS8 = {
     "mcb_jpeg_entropy_decode": [vp, vp, ci, vp, vp, ci, vp, vp, vp],
+    "mcb_jpeg_entropy_decode_parallel": [vp, vp, ci, vp, vp, ci, vp, ci, vp, vp, vp, vp],
+    "mcb_jpeg_subsequence_bits": [],
     "mcb_jpeg_idct": [vp, vp, vp, ci, ci, vp, vp],
     "mcb_jpeg_upsample_rgb": [vp, vp, vp, ci, ci, ci, vp, vp],
 }

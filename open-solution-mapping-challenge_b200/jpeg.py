@@ -3,9 +3,9 @@
 The host parses the markers (SOI, APPn, DQT, DHT, SOF0/SOF1, DRI, SOS, EOI), checks every length and index, removes
 the byte stuffing, splits the entropy-coded data at its restart markers into independent segments and builds the
 canonical Huffman lookup tables.  `decode_jpeg_batch` packs a batch into one byte buffer plus per-image and per-segment
-tables and runs the three kernels of csrc/jpeg.cu: entropy decode (one thread per segment), libjpeg's islow IDCT, and
-libjpeg-turbo's fancy upsampling + YCbCr -> RGB.  The result is what `np.array(Image.open(f).convert('RGB'))` returns,
-bit for bit.
+tables and runs the three stages of csrc/jpeg.cu: entropy decode (parallel inside each long segment: speculate,
+resolve, emit), libjpeg's islow IDCT, and libjpeg-turbo's fancy upsampling + YCbCr -> RGB.  The result is what
+`np.array(Image.open(f).convert('RGB'))` returns, bit for bit.
 
 Supported: sequential Huffman JPEG (SOF0 / SOF1) with 8-bit samples, one scan holding every component, grayscale or
 YCbCr (JFIF or Adobe transform 1), each component sampled at 1 or 1/2 of the largest factor in either direction (4:4:4,
@@ -378,9 +378,68 @@ def pack_batch(records):
                 qt=qt, n_blocks=block, height=h, width=w)
 
 
+# A segment of at most this many subsequences is decoded whole by one thread, as the serial kernel does: the parallel
+# path's critical path is about four subsequence decodes long even when every guess holds (warm-up, speculation, the
+# exact last subsequence, emission), and a short periodic stream (a flat tile) can hold every guess at a wrong phase.
+SPLIT_MIN_SUBSEQUENCES = 16
+
+
+def subsequence_table(pk, bits):
+    """subsequences of `bits` unstuffed bits per segment of a packed batch (a segment of at most
+    SPLIT_MIN_SUBSEQUENCES of them is one) -> (sub_first int32 (nseg + 1,): first subsequence of each segment, the most
+    subsequences of one image)"""
+    nbytes = pk["segments"][:, 2].astype(np.int64)
+    if len(nbytes) and nbytes.max() >= 2 ** 28:
+        raise ValueError("JPEG entropy segment of %d bytes: the device decode takes less than 2^28" % nbytes.max())
+    counts = -(-nbytes * 8 // bits)
+    counts[counts <= SPLIT_MIN_SUBSEQUENCES] = 1
+    sub_first = np.concatenate([[0], np.cumsum(counts)])
+    if sub_first[-1] >= 2 ** 31 // 16:
+        raise ValueError("JPEG batch too large: %d subsequences" % sub_first[-1])
+    im = pk["images"]
+    per_image = sub_first[im[:, 4] + im[:, 5]] - sub_first[im[:, 4]]
+    return sub_first.astype(np.int32), int(per_image.max())
+
+
+class DeviceBatch:
+    """a packed batch on the device: the tables csrc/jpeg.cu reads, uploaded from pinned memory on the current stream"""
+
+    def __init__(self, pk, dev):
+        import torch
+        from . import _lib as L
+
+        def up(a):
+            return torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(dev, non_blocking=True)
+        self.n, self.n_blocks, self.nseg = len(pk["images"]), pk["n_blocks"], len(pk["segments"])
+        sub_first, self.max_image_subs = subsequence_table(pk, L.lib.mcb_jpeg_subsequence_bits())
+        self.data, self.segs, self.images, self.huff, self.qt, self.sub_first = (
+            up(a) for a in (pk["data"], pk["segments"], pk["images"], pk["huff"], pk["qt"], sub_first))
+        self.workspace = torch.empty(16 + 16 * int(sub_first[-1]), dtype=torch.int32, device=dev)
+        self.coef = torch.empty((self.n_blocks, 64), dtype=torch.int16, device=dev)
+        self.status = torch.empty(self.n, dtype=torch.int32, device=dev)
+
+    def entropy_decode(self):
+        """the parallel entropy decode into self.coef / self.status (three launches on the current stream)"""
+        from . import _lib as L
+        L.fcall("mcb_jpeg_entropy_decode_parallel", self.data.data_ptr(), self.segs.data_ptr(), self.nseg,
+                self.images.data_ptr(), self.huff.data_ptr(), self.n, self.sub_first.data_ptr(), self.max_image_subs,
+                self.workspace.data_ptr(), self.coef.data_ptr(), self.status.data_ptr())
+
+    def entropy_decode_serial(self):
+        """the one-thread-per-segment entropy decode into self.coef / self.status, as a reference"""
+        from . import _lib as L
+        L.fcall("mcb_jpeg_entropy_decode", self.data.data_ptr(), self.segs.data_ptr(), self.nseg,
+                self.images.data_ptr(), self.huff.data_ptr(), self.n, self.coef.data_ptr(), self.status.data_ptr())
+
+    def counters(self):
+        """speculation counters of the last parallel decode: entry states that held, were corrected, the longest run of
+        consecutive corrections, exact re-decodes of a segment's error or last block (synchronises)"""
+        return self.workspace[:4].cpu().numpy()
+
+
 def decode_records(records, device=None):
     """JpegRecords of one size -> (rgb uint8 cuda (n, H, W, 3), coefficients int16 cuda (blocks, 64), IDCT planes uint8
-    cuda (blocks, 8, 8), status int32 numpy (n,)), blocks in pack_batch's order.  Three launches on the current stream,
+    cuda (blocks, 8, 8), status int32 numpy (n,)), blocks in pack_batch's order.  Five launches on the current stream,
     then one read of the status words; an image with a non-zero status has undefined pixels, the others are exact."""
     import torch
     from . import _lib as L
@@ -388,18 +447,13 @@ def decode_records(records, device=None):
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     n, hgt, wid = len(records), pk["height"], pk["width"]
 
-    def up(a):
-        return torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(dev, non_blocking=True)
-
     with torch.cuda.device(dev):
-        data, segs, images, huff, qt, tables = (up(a) for a in (pk["data"], pk["segments"], pk["images"], pk["huff"],
-                                                                 pk["qt"], ycc_tables()))
-        coef = torch.empty((pk["n_blocks"], 64), dtype=torch.int16, device=dev)
+        b = DeviceBatch(pk, dev)
+        tables = torch.from_numpy(ycc_tables()).pin_memory().to(dev, non_blocking=True)
+        coef, status, qt, images = b.coef, b.status, b.qt, b.images
         planes = torch.empty((pk["n_blocks"], 8, 8), dtype=torch.uint8, device=dev)
-        status = torch.empty(n, dtype=torch.int32, device=dev)
         out = torch.empty((n, hgt, wid, 3), dtype=torch.uint8, device=dev)
-        L.fcall("mcb_jpeg_entropy_decode", data.data_ptr(), segs.data_ptr(), len(pk["segments"]), images.data_ptr(),
-                huff.data_ptr(), n, coef.data_ptr(), status.data_ptr())
+        b.entropy_decode()
         L.fcall("mcb_jpeg_idct", coef.data_ptr(), qt.data_ptr(), images.data_ptr(), n, pk["n_blocks"],
                 planes.data_ptr())
         L.fcall("mcb_jpeg_upsample_rgb", planes.data_ptr(), images.data_ptr(), tables.data_ptr(), n, hgt, wid,

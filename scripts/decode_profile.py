@@ -3,10 +3,14 @@
 
   python scripts/decode_profile.py [--reps 100] [--out FILE]
 
-Records, in one run on one card, for seeded 300x300 JPEG tiles at quality 75 and 95, 4:2:0 and 4:4:4 sampling:
-  device_ms   device time of one batch of 20 and of 64 tiles through the three kernels of csrc/jpeg.cu, each stage
-              separately (entropy decode, IDCT, upsample + colour) and all three, CUDA events around launches queued
-              behind a device-side wait (host launch time kept out), median over --reps after warm-up
+Records, in one run on one card, for seeded 300x300 JPEG tiles at quality 75 and 95, 4:2:0 and 4:4:4 sampling, and
+flat 4:2:0 tiles (quality "flat"):
+  device_ms   device time of one batch of 20 and of 64 tiles through the stages of csrc/jpeg.cu, each stage
+              separately (parallel entropy decode, IDCT, upsample + colour) and all three, and the one-thread-per-
+              segment entropy decode (`entropy_serial`) beside the parallel one (`entropy_speedup`); CUDA events around
+              launches queued behind a device-side wait (host launch time kept out), median over --reps after warm-up;
+              `speculation` = the parallel decode's counters (guesses held, corrected, longest correction run, exact
+              re-decodes of a segment's end)
   worker_ms   host time per file of the device path's worker share (mcb200.jpeg.read_jpeg: read, parse, unstuff, Huffman
               tables), median
   pillow_ms   host time per file of np.array(Image.open(f).convert('RGB')), the loaders' decode, median
@@ -44,6 +48,8 @@ def power_limit_w():
 
 def _tiles(n, quality, sampling):
     from oracle import jpeg_oracle as O
+    if quality is None:                      # flat tiles: every block "DC diff 0 + EOB" after the first
+        return [O.encode_pil(np.full((300, 300, 3), 40 + 3 * i, np.uint8), 75, sampling) for i in range(n)]
     return [O.encode_pil(O.content(300, 300, seed=1000 + i), quality, sampling) for i in range(n)]
 
 
@@ -52,24 +58,22 @@ def device_ms(blobs, reps):
     from mcb200 import _lib as L
     from mcb200 import jpeg as J
     recs = [J.load(b) for b in blobs]
-    out, coef, planes, st = J.decode_records(recs)          # also warms the module up
+    out, _, planes, st = J.decode_records(recs)             # also warms the module up
     assert not st.any()
     pk = J.pack_batch(recs)
     dev = out.device
-    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)   # noqa: E731
-    data, segs, images, huff, qt, tables = (up(a) for a in (pk["data"], pk["segments"], pk["images"], pk["huff"],
-                                                             pk["qt"], J.ycc_tables()))
-    status = torch.empty(len(recs), dtype=torch.int32, device=dev)
+    batch = J.DeviceBatch(pk, dev)
+    tables = torch.from_numpy(J.ycc_tables()).to(dev)
     n, h, w, nb = len(recs), pk["height"], pk["width"], pk["n_blocks"]
     stages = {
-        "entropy": lambda: L.fcall("mcb_jpeg_entropy_decode", data.data_ptr(), segs.data_ptr(), len(pk["segments"]),
-                                   images.data_ptr(), huff.data_ptr(), n, coef.data_ptr(), status.data_ptr()),
-        "idct": lambda: L.fcall("mcb_jpeg_idct", coef.data_ptr(), qt.data_ptr(), images.data_ptr(), n, nb,
-                                planes.data_ptr()),
-        "upsample_rgb": lambda: L.fcall("mcb_jpeg_upsample_rgb", planes.data_ptr(), images.data_ptr(),
+        "entropy": batch.entropy_decode,
+        "idct": lambda: L.fcall("mcb_jpeg_idct", batch.coef.data_ptr(), batch.qt.data_ptr(), batch.images.data_ptr(),
+                                n, nb, planes.data_ptr()),
+        "upsample_rgb": lambda: L.fcall("mcb_jpeg_upsample_rgb", planes.data_ptr(), batch.images.data_ptr(),
                                         tables.data_ptr(), n, h, w, out.data_ptr()),
     }
     stages["all"] = lambda: [f() for k, f in list(stages.items())[:3]]
+    stages["entropy_serial"] = batch.entropy_decode_serial
     res = {}
     for name, fn in stages.items():
         times = []
@@ -83,7 +87,10 @@ def device_ms(blobs, reps):
             if i >= 10:
                 times.append(a.elapsed_time(b))
         res[name] = round(float(np.median(times)), 4)
-    assert not status.cpu().numpy().any()
+    assert not batch.status.cpu().numpy().any()
+    batch.entropy_decode()
+    res["speculation"] = [int(x) for x in batch.counters()]
+    res["entropy_speedup"] = round(res["entropy_serial"] / res["entropy"], 2)
     return res
 
 
@@ -165,16 +172,16 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("decode_profile.py needs a CUDA device")
     res = {"card": torch.cuda.get_device_name(0), "power_limit_w": power_limit_w(), "tile": "300x300", "cases": []}
-    for quality in (75, 95):
-        for sampling in ("420", "444"):
-            blobs = _tiles(64, quality, sampling)
-            worker, pillow = host_ms(blobs, args.reps)
-            case = {"quality": quality, "sampling": sampling, "bytes_per_file": int(np.mean([len(b) for b in blobs])),
-                    "worker_ms_per_file": worker, "pillow_ms_per_file": pillow}
-            for n in (20, 64):
-                case["device_ms_batch%d" % n] = device_ms(blobs[:n], args.reps)
-                case["loader_ms_per_batch%d" % n] = loader_ms(blobs, n)
-            res["cases"].append(case)
+    for quality, sampling in ((75, "420"), (75, "444"), (95, "420"), (95, "444"), (None, "420")):
+        blobs = _tiles(64, quality, sampling)
+        worker, pillow = host_ms(blobs, args.reps)
+        case = {"quality": quality or "flat", "sampling": sampling,
+                "bytes_per_file": int(np.mean([len(b) for b in blobs])),
+                "worker_ms_per_file": worker, "pillow_ms_per_file": pillow}
+        for n in (20, 64):
+            case["device_ms_batch%d" % n] = device_ms(blobs[:n], args.reps)
+            case["loader_ms_per_batch%d" % n] = loader_ms(blobs, n)
+        res["cases"].append(case)
     line = json.dumps(res)
     print(line)
     if args.out:
