@@ -1,10 +1,12 @@
-"""TEST INFRASTRUCTURE -- the harness of the batch-32 train-step tests (tests/test_train_step_scale_gpu.py,
-tests/test_train_step_vgg_scale_gpu.py, tests/test_train_step_resnet_units_gpu.py), and the helpers the golden-fixture
-encoder tests share.  Never imported by the product path.
+"""TEST INFRASTRUCTURE -- the harness of the train-step tests at the benchmarks' sizes
+(tests/test_train_step_scale_gpu.py, tests/test_train_step_vgg_scale_gpu.py, tests/test_train_step_resnet_units_gpu.py
+at batch 32 and 320x320, tests/test_train_step_config5_gpu.py at BASELINE.json config 5's batch 16 and 512x512), and
+the helpers the golden-fixture encoder tests share.  Never imported by the product path.
 
-BenchStep is the train step the benchmarks time, for every encoder family they run at batch N and SxS: the ResNets
-through PyTorchUNetWeighted._fit_loop as bench.py builds it, VGG11 and VGG16 through FusedTrainStep as bench_encoders.py
-builds them.  Its serial_steps is the only code of the tests that reaches into FusedTrainStep's private state.
+BenchStep is the train step the benchmarks time, for every encoder family they run, at batch n and sxs (N and S, the
+default, are bench.py's): the ResNets through PyTorchUNetWeighted._fit_loop as bench.py builds it, VGG11 and VGG16
+through FusedTrainStep as bench_encoders.py builds them.  Its serial_steps is the only code of the tests that reaches
+into FusedTrainStep's private state.
 
 What the tests compare across runs is kept on the host: snapshot / snapshot_mismatches compare two train steps bit for
 bit, and name a difference by the parameter it falls in, in backward order.
@@ -28,7 +30,10 @@ from oracle.unit_checks import nchw
 
 N, S = 32, 320            # bench.py's and bench_encoders.py's train batch and net input
 SEED = 1234
-RESNET_DEPTH = {"ResNet101": 101, "ResNet34": 34}
+RESNET_DEPTH = {"ResNet101": 101, "ResNet34": 34}     # the ResNets trained at batch N and SxS
+CONFIG5 = "ResNet152"                                  # BASELINE.json config 5: bench.py --encoder 152 --batch 16
+N5, S5 = 16, 512                                       # --size 512
+DEPTH = dict(RESNET_DEPTH, **{CONFIG5: 152})           # every ResNet encoder the harness builds
 VGG = ("VGG11", "VGG16")
 STATS = ("running_mean", "running_var")
 
@@ -68,17 +73,17 @@ def seeded_sd(enc):
     with torch.random.fork_rng(devices=[]):
         if enc in VGG:
             return V.make_reference_like_state_dict(enc, seed=SEED)
-        return O.make_reference_like_state_dict(RESNET_DEPTH[enc], seed=SEED)
+        return O.make_reference_like_state_dict(DEPTH[enc], seed=SEED)
 
 
 class BenchStep:
-    """the train step the benchmarks time for `enc`, on a net loaded with sd, at batch N and SxS.  fused is that
+    """the train step the benchmarks time for `enc`, on a net loaded with sd, at batch n and sxs.  fused is that
     FusedTrainStep (for the ResNets the one PyTorchUNetWeighted._fit_loop caches for this shape); adam is what the step
     hands it: (lr, betas, eps, weight_decay)"""
 
-    def __init__(self, enc, sd, dev):
+    def __init__(self, enc, sd, dev, n=N, s=S):
         from mcb200.models import FusedTrainStep, PyTorchUNetWeighted
-        shape = (N, 3, S, S)
+        shape = (n, 3, s, s)
         if enc in VGG:
             cfg, lr, wd = bench_encoders.vgg_step_settings(enc)
             self.adam = (lr, (0.9, 0.999), 1e-8, wd)        # FusedTrainStep.step's defaults, as the benchmark calls it
@@ -130,8 +135,8 @@ def free_device_memory():
     torch.cuda.empty_cache()
 
 
-def batch(seed, n=N):
-    x, t = bench_data.train_batch(n, S, seed=seed)
+def batch(seed, n=N, s=S):
+    x, t = bench_data.train_batch(n, s, seed=seed)
     return torch.from_numpy(x), torch.from_numpy(t)
 
 
@@ -198,6 +203,63 @@ def snapshot_mismatches(layout, a, b):
     if stats:
         out.append("running statistics: %d differ, first in backward order %s" % (len(stats), stats[-1]))
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the composed step: the captured step against program order (A), Adam against the step's own gradients (B)
+# ---------------------------------------------------------------------------------------------------------------------
+def check_captured_equals_serial(enc, cuda, n=N, s=S):
+    """three distinct batches through the captured step (eager, then graph replays) and through the same launches in
+    program order (BenchStep.serial_steps) on a fresh net: every snapshot bitwise equal.  One plan alive at a time"""
+    sd = seeded_sd(enc)
+    batches = [tuple(t.to(cuda) for t in batch(SEED + i, n, s)) for i in range(3)]
+
+    run = BenchStep(enc, sd, cuda, n, s)
+    layout = arena_layout(run.net)
+    graphed = []
+    for i, (X, T) in enumerate(batches):
+        graphed.append(snapshot(run, run.step(X, T)))
+        assert run.fused.graphs is not None and run.fused.opt.t == i + 1
+    del run
+    free_device_memory()
+
+    run = BenchStep(enc, sd, cuda, n, s)
+    for i, loss in enumerate(run.serial_steps(batches)):
+        serial = snapshot(run, loss)
+        bad = snapshot_mismatches(layout, graphed[i], serial)
+        print("%s step %d: loss %.7f, captured == serial: %s" % (enc, i + 1, float(serial["loss"]), not bad))
+        assert not bad, "%s step %d (%s): %s" % (enc, i + 1, "eager" if i == 0 else "graph replay", "; ".join(bad))
+    assert run.fused.opt.t == 3
+    assert len({float(g["loss"]) for g in graphed}) == 3, "distinct batches must give distinct losses"
+    del run, graphed
+    free_device_memory()
+
+
+def check_adam_of_own_gradients(enc, cuda, n=N, s=S):
+    """three steps (eager, then graph replays): each step's fp32 weights and Adam moments exactly whole-arena Adam of
+    that step's own final gradients, and the bf16 operand copy exactly the new fp32 weights"""
+    from mcb200 import ops
+    run = BenchStep(enc, seeded_sd(enc), cuda, n, s)
+    net, opt = run.net, run.fused.opt
+    layout = arena_layout(net)
+    lr, betas, eps, wd = run.adam
+    for i in range(3):
+        X, T = (t.to(cuda) for t in batch(SEED + 10 + i, n, s))
+        p, m, v = net._p32.clone(), opt.m.clone(), opt.v.clone()
+        run.step(X, T)
+        assert opt.t == i + 1
+        assert bool(net._g32.any()) and not same_bits(p, net._p32), "the step must compute gradients and move weights"
+        w16 = torch.zeros_like(net._w16)
+        ops.adam_step(p, net._g32, m, v, w16, opt.t, lr, betas, eps, wd, 1.0)
+        bad = ["%s: first differing tensor %s" % (k, d) for k, d in
+               (("p32", arena_mismatch(layout, net._p32, p)), ("m", arena_mismatch(layout, opt.m, m)),
+                ("v", arena_mismatch(layout, opt.v, v)), ("w16", arena_mismatch(layout, net._w16, w16)),
+                ("w16 against bf16(p32)", arena_mismatch(layout, net._w16, net._p32.to(torch.bfloat16)))) if d]
+        print("%s step %d: fused Adam == whole-arena Adam of the step's gradients: %s" % (enc, i + 1, not bad))
+        assert not bad, "%s step %d (%s): %s" % (enc, i + 1, "eager" if i == 0 else "graph replay", "; ".join(bad))
+        del p, m, v, w16
+    del run, net, opt
+    free_device_memory()
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -1,14 +1,14 @@
-"""Float64 references of single plan units on a plan's own buffers, shared by the unit tests of the batch-32 train step
-(tests/test_train_step_vgg_scale_gpu.py, tests/test_train_step_resnet_units_gpu.py) and of the batch-64 inference
-forward (tests/test_infer_forward_units_gpu.py).
+"""Float64 references of single plan units on a plan's own buffers, shared by the unit tests of the train step
+(tests/test_train_step_vgg_scale_gpu.py, oracle/resnet_step_units.py) and of the batch-64 inference forward
+(tests/test_infer_forward_units_gpu.py).
 
 Activations and gradients are the plan's NHWC bf16 buffers; every reference is evaluated in float64 on their device.
 Bounds are element-wise, |got - ref| <= rel |ref| + acc A + extra, with A the same operation on absolute values."""
 import torch
 import torch.nn.functional as F
 
-SAMPLE = (0, 10, 21, 31)  # images of the train step's element-wise forward and data-gradient checks (the reductions
-#                           take all 32)
+SAMPLE = (0, 10, 21, 31)  # images of the batch-32 train step's element-wise forward and data-gradient checks (the
+#                           reductions take all 32); the first and the last image hold the batch's edge tiles
 CHUNK = 8                 # images per float64 evaluation over a whole batch (sums over the chunks added in float64)
 # accumulation allowance of the weight gradients.  Their reductions run over all 3.3 M pixels of the batch, and the
 # split-K GEMM caps its splits at one wave of CTAs, so one fp32 accumulator chain adds up to k = 12800 pixel tiles x 4
@@ -121,11 +121,12 @@ def check_conv_forward(bd, prefix, x, y, w, b, transposed=False, images=SAMPLE):
     del ref, absref
 
 
-def check_conv_half(bd, net, w16, b32, prefix, wkey, bkey, x, y, g, bias_from, transposed=False):
+def check_conv_half(bd, net, w16, b32, prefix, wkey, bkey, x, y, g, bias_from, transposed=False, images=SAMPLE):
     """one conv (or stride-2 transposed conv) + bias + ReLU: x the NCHW bf16 input, y and g the NHWC stored output and
-    output gradient; w16 / b32 the pre-step bf16 weight and fp32 bias (float64 on the device)"""
+    output gradient; w16 / b32 the pre-step bf16 weight and fp32 bias (float64 on the device).  The forward is checked
+    on `images`, the weight and bias gradients over the whole batch"""
     w = w16[wkey]
-    check_conv_forward(bd, prefix, x, y, w, b32[bkey], transposed)
+    check_conv_forward(bd, prefix, x, y, w, b32[bkey], transposed, images)
     bd.zero_where_off(prefix + " ReLU mask", g, y)
     if transposed:     # d conv_transpose2d(x, W) / dW = conv2d weight gradient of the conv from the output back to x
         ref, absref = wgrad64(nchw(g), x, w.shape, stride=2, padding=1)

@@ -36,9 +36,9 @@ import torch
 import bench
 import bench_data
 from oracle import unet_oracle as O
-from oracle.step_checks import (N, S, SEED, BenchStep, arena_layout, arena_mismatch, batch, deviation,
-                                free_device_memory, host, reference_step, running_stats, same_bits, seeded_sd, snapshot,
-                                snapshot_mismatches, step_outputs)
+from oracle.step_checks import (N, S, SEED, BenchStep, arena_layout, arena_mismatch, batch, check_adam_of_own_gradients,
+                                check_captured_equals_serial, deviation, free_device_memory, host, reference_step,
+                                running_stats, same_bits, seeded_sd, step_outputs)
 from oracle.step_checks import no_tf32, rng_and_peak_memory  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
@@ -65,28 +65,7 @@ def conditioned_sd():
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("enc", ["ResNet101", "ResNet34", "VGG11", "VGG16"])
 def test_captured_step_equals_serial_launch_order(mcb, cuda, enc):
-    sd = seeded_sd(enc)
-    batches = [tuple(t.to(cuda) for t in batch(SEED + i)) for i in range(3)]
-
-    run = BenchStep(enc, sd, cuda)
-    layout = arena_layout(run.net)
-    graphed = []
-    for i, (X, T) in enumerate(batches):
-        graphed.append(snapshot(run, run.step(X, T)))
-        assert run.fused.graphs is not None and run.fused.opt.t == i + 1
-    del run
-    free_device_memory()
-
-    run = BenchStep(enc, sd, cuda)
-    for i, loss in enumerate(run.serial_steps(batches)):
-        serial = snapshot(run, loss)
-        bad = snapshot_mismatches(layout, graphed[i], serial)
-        print("%s step %d: loss %.7f, captured == serial: %s" % (enc, i + 1, float(serial["loss"]), not bad))
-        assert not bad, "%s step %d (%s): %s" % (enc, i + 1, "eager" if i == 0 else "graph replay", "; ".join(bad))
-    assert run.fused.opt.t == 3
-    assert len({float(g["loss"]) for g in graphed}) == 3, "distinct batches must give distinct losses"
-    del run, graphed
-    free_device_memory()
+    check_captured_equals_serial(enc, cuda)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -94,28 +73,7 @@ def test_captured_step_equals_serial_launch_order(mcb, cuda, enc):
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("enc", ["ResNet101", "VGG11", "VGG16"])
 def test_fused_adam_is_adam_of_the_steps_own_gradients(mcb, cuda, enc):
-    from mcb200 import ops
-    run = BenchStep(enc, seeded_sd(enc), cuda)
-    net, opt = run.net, run.fused.opt
-    layout = arena_layout(net)
-    lr, betas, eps, wd = run.adam
-    for i in range(3):
-        X, T = (t.to(cuda) for t in batch(SEED + 10 + i))
-        p, m, v = net._p32.clone(), opt.m.clone(), opt.v.clone()
-        run.step(X, T)
-        assert opt.t == i + 1
-        assert bool(net._g32.any()) and not same_bits(p, net._p32), "the step must compute gradients and move weights"
-        w16 = torch.zeros_like(net._w16)
-        ops.adam_step(p, net._g32, m, v, w16, opt.t, lr, betas, eps, wd, 1.0)
-        bad = ["%s: first differing tensor %s" % (k, d) for k, d in
-               (("p32", arena_mismatch(layout, net._p32, p)), ("m", arena_mismatch(layout, opt.m, m)),
-                ("v", arena_mismatch(layout, opt.v, v)), ("w16", arena_mismatch(layout, net._w16, w16)),
-                ("w16 against bf16(p32)", arena_mismatch(layout, net._w16, net._p32.to(torch.bfloat16)))) if d]
-        print("%s step %d: fused Adam == whole-arena Adam of the step's gradients: %s" % (enc, i + 1, not bad))
-        assert not bad, "%s step %d (%s): %s" % (enc, i + 1, "eager" if i == 0 else "graph replay", "; ".join(bad))
-        del p, m, v, w16
-    del run, net, opt
-    free_device_memory()
+    check_adam_of_own_gradients(enc, cuda)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
