@@ -41,6 +41,7 @@ static void pick_tile(int Wv, int Hv, int N, int max_rows, int row_mult, int* pb
 // them the fp32 summation order: rewriting one can change a rounding, a split count and so the results' last bits.
 constexpr int kSmemBudget = 227 * 1024;               // dynamic shared memory of one CTA (the sm_90 maximum)
 constexpr int kMaxStagesHalo = 9, kMaxStages = 6;     // operand ring depth, haloed / per-tap path
+constexpr int kTwoStagingMinStages = 3;               // two epilogue staging buffers while the ring keeps this many stages
 constexpr int kHaloMinChannels = 128;                 // haloed tile from this many channels per tap
 constexpr int kBn256MinWaveX10 = 6;                   // 256-wide N tiles down to 0.6 of a wave
 constexpr int kWgradWavesX10 = 10;                    // weight-gradient grid: one wave
@@ -92,13 +93,14 @@ static int launch_conv(int BN, int BK, bool b_mn, ConvGemmParams& p, int m_tiles
   const int a_bytes = halo ? ((kHaloW * kHaloH * BK * 2 + 1023) / 1024) * 1024 : 128 * BK * 2;
   const int b_bytes = BN * BK * 2;
   const int stage = halo ? b_bytes : a_bytes + b_bytes;
-  const int out_bufs = BN <= 64 ? 4 : (BN == 128 ? 2 : 1);
-  const int out_bytes = out_bufs * 128 * BN * 2;
-  const int aux_bytes = p.aux_mode != 0 ? 2 * 128 * (BN >= 64 ? 64 : 32) * 2 : 0;  // one aux chunk per MMA warpgroup
-  const int fixed = out_bytes + aux_bytes + kStatBytes + 1024 /*align*/ + 1536 /*barriers, row table*/ +
-                    (halo ? 2 * a_bytes : 0);
+  const int out_buf_bytes = 128 * BN * 2;  // one bf16 staging buffer
+  const int aux_bytes = p.aux_mode != 0 ? 2 * 128 * (BN >= 64 ? 64 : 32) * 2 : 0;  // the epilogue's ring of two aux chunks
+  const int base = aux_bytes + kStatBytes + 1024 /*align*/ + 1536 /*barriers, row table*/ + (halo ? 2 * a_bytes : 0);
+  const int out_bufs = (kSmemBudget - base - 2 * out_buf_bytes) / stage >= kTwoStagingMinStages ? 2 : 1;
+  const int fixed = base + out_bufs * out_buf_bytes;
   const int stages = std::max(2, std::min(halo ? kMaxStagesHalo : kMaxStages, (kSmemBudget - fixed) / stage));
   p.stages = stages;
+  p.out_bufs = out_bufs;
   p.m_tiles = m_tiles; p.n_tiles = n_tiles; p.phases = phases;
   const size_t smem = (size_t)stages * stage + fixed;
   const long total = (long)m_tiles * n_tiles * phases;

@@ -12,8 +12,8 @@
 //       dW_t[co, ci] += sum over pixels: dY[pixel + offA_t, co] * X[pixel + offB_t, ci]
 //       both operands MN-major (the pixel axis is GEMM-K), split-K over pixel tiles, deterministic split sum.
 //
-// Warp roles (384 threads): warpgroup 0 = TMA producer (one warp issues, the register file goes to the others),
-// warpgroups 1 and 2 = MMA + epilogue, rows 0..63 and 64..127 of the 128-row tile.
+// Warp roles: warpgroup 0 = TMA producer (one warp issues, the register file goes to the others), warpgroups 1 and 2 =
+// MMA, rows 0..63 and 64..127 of the 128-row tile; conv_gemm_kernel adds warpgroup 3 = epilogue.
 #pragma once
 #include "tc.cuh"
 #include "detsum.cuh"
@@ -53,6 +53,7 @@ struct ConvGemmParams {
   int tiles_x, tiles_y;
   int m_tiles, n_tiles, phases;  // persistent tile space: phases x m_tiles x n_tiles
   int stages;
+  int out_bufs;  // bf16 staging buffers between pass 1 and the epilogue warpgroup: 1 or 2
   int n_off;  // first N (weight row / column) coordinate of this launch (concat source slice for dgrad)
   // epilogue:  v = acc * scale[c] + bias[c] + residual[pix][c];  v = relu(v);  v = mask ? v : 0
   const float* scale;              // per-channel multiplier (inference-mode BatchNorm folded into the epilogue), or null
@@ -115,9 +116,17 @@ __device__ __forceinline__ uint8_t* align_up_1024(uint8_t* p) {
 
 // -------------------------------------------------------------------------------------------------
 // Persistent, warp-specialised: one CTA per SM walks tiles t = blockIdx.x, += gridDim.x (n fastest, so CTAs that run
-// together share the A pixel tile in L2).  The TMA ring (full/empty mbarriers) runs continuously across tiles, so the
-// producer loads the operands of tile i+1 while the MMA warpgroups run the epilogue of tile i.
-constexpr int kConvThreads = 384;  // warpgroup 0 TMA producer, warpgroups 1, 2 MMA + epilogue
+// together share the A pixel tile in L2).  The TMA ring (full/empty mbarriers) runs continuously across tiles, and so
+// do the MMA warpgroups: after a tile's main loop they only write the accumulators through scale / bias / residual /
+// ReLU to a bf16 staging buffer (pass 1), signal staged[b] and start the next tile's main loop.  The epilogue
+// warpgroup runs the second pass over the staged tile (BatchNorm statistics, ReLU / BatchNorm-backward masks and
+// their channel sums), issues the TMA stores and signals drained[b] once they have read the buffer.  With two staging
+// buffers pass 1 of tile i+1 never waits for the epilogue of tile i; with one it waits for the drain of tile i, which
+// had the whole main loop of tile i+1 to finish.
+constexpr int kConvThreads = 512;  // warpgroup 0 TMA producer, warpgroups 1, 2 MMA + pass 1, warpgroup 3 epilogue
+// 128 x 24 + 128 x 120 + 256 x 184 = 64 K registers: BN = 256's 128 fp32 accumulators in the MMA warpgroups, pass 2's
+// per-thread state in the epilogue warpgroup, neither spilling (ptxas -v)
+constexpr int kConvProducerRegs = 24, kConvEpilogueRegs = 120, kConvMmaRegs = 184;
 
 // HALO (3x3, stride 1): the pixel tile is 8 wide x 16 tall in one image and ONE haloed TMA box (BK channels, 10, 18, 1)
 // per channel chunk serves all nine taps: tap (dy, dx) is the same shared-memory tile read through a descriptor whose
@@ -126,10 +135,10 @@ constexpr int kConvThreads = 384;  // warpgroup 0 TMA producer, warpgroups 1, 2 
 // the same bytes TMA wrote).  A and B then travel in separate mbarrier rings: 1 A load + 9 B loads per channel chunk.
 constexpr int kHaloW = 10, kHaloH = 18;  // (8 + 2) x (16 + 2)
 
-// per-channel reduction scratch: per MMA warpgroup 4 warps x (up to) 8 channel groups x 16 floats
-constexpr int kStatBytes = 2 * 4 * 8 * 16 * 4;
+// per-channel reduction scratch of the epilogue warpgroup: 4 warps x (up to) 8 channel groups x 16 floats
+constexpr int kStatBytes = 4 * 8 * 16 * 4;
 
-__device__ __forceinline__ void mma_wg_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+__device__ __forceinline__ void epi_wg_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 
 template <int BN, int BK, bool B_MN, bool HALO>
 __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
@@ -151,26 +160,26 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
   constexpr int OUT_ROW_BYTES = OUT_CW * 2;
   constexpr int OUT_CHUNK_BYTES = 128 * OUT_ROW_BYTES;
   constexpr int OUT_CHUNKS = BN / OUT_CW;
-  // small tiles finish faster than a TMA store drains: rotate several staging buffers so the epilogue of tile i+1 never
-  // waits for the store of tile i
-  constexpr int OUT_BUFS = (BN <= 64) ? 4 : (BN == 128 ? 2 : 1);
-  constexpr int OUT_BYTES = OUT_BUFS * OUT_CHUNKS * OUT_CHUNK_BYTES;
+  constexpr int OUT_TILE_BYTES = OUT_CHUNKS * OUT_CHUNK_BYTES;   // one staging buffer
   constexpr int ACC = BN / 2;  // fp32 accumulators per thread (64 x BN per warpgroup)
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_up_1024(smem_raw);
   const int stages = p.stages;
+  const int out_bufs = p.out_bufs;   // staging buffers: 1 or 2 (launch_conv)
   const int aux_mode = p.aux_mode;
   uint8_t* a_ring = smem + (size_t)stages * STAGE_BYTES;               // HALO only: 2 haloed A tiles
   uint8_t* out_stage = a_ring + A_RING_BYTES;                          // 1024-aligned (all pieces are)
-  uint8_t* aux_stage = out_stage + OUT_BYTES;                          // aux modes: one chunk per MMA warpgroup
+  uint8_t* aux_stage = out_stage + (size_t)out_bufs * OUT_TILE_BYTES;  // aux modes: a ring of two chunks
   float* stat_scratch = reinterpret_cast<float*>(aux_stage + (aux_mode != 0 ? 2 * OUT_CHUNK_BYTES : 0));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stat_scratch) + kStatBytes);
   uint64_t* empty_bar = full_bar + stages;
   uint64_t* a_full_bar = empty_bar + stages;      // [2] (HALO)
   uint64_t* a_empty_bar = a_full_bar + 2;         // [2] (HALO)
-  uint64_t* aux_full_bar = a_empty_bar + 2;       // [2] one per MMA warpgroup
-  int* row_pix = reinterpret_cast<int*>(aux_full_bar + 2);  // [128] pixel index in the full-resolution tensor, -1 = invalid
+  uint64_t* aux_full_bar = a_empty_bar + 2;       // [2] aux ring
+  uint64_t* staged_bar = aux_full_bar + 2;        // [2] per staging buffer: pass 1 done (one arrival per MMA warp)
+  uint64_t* drained_bar = staged_bar + 2;         // [2] per staging buffer: its TMA stores have read it
+  int* row_ok = reinterpret_cast<int*>(drained_bar + 2);  // [128] ragged tiles: the row is an output pixel
 
   // the shuffle makes the warp index provably warp-uniform, so the role loops below compile onto the uniform datapath
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
@@ -187,8 +196,11 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
     tc::mbar_init(&a_full_bar[1], 1);
     tc::mbar_init(&a_empty_bar[0], 2);
     tc::mbar_init(&a_empty_bar[1], 2);
-    tc::mbar_init(&aux_full_bar[0], 1);
-    tc::mbar_init(&aux_full_bar[1], 1);
+    for (int b = 0; b < 2; ++b) {
+      tc::mbar_init(&aux_full_bar[b], 1);
+      tc::mbar_init(&staged_bar[b], 8);
+      tc::mbar_init(&drained_bar[b], 1);
+    }
     tc::fence_barrier_init();
     tc::prefetch_tmap(&p.tmB);
     tc::prefetch_tmap(&p.tmA[0]);
@@ -196,7 +208,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
   __syncthreads();
 
   if (warp < 4) {
-    tc::regs_dealloc<kProducerRegs>();
+    tc::regs_dealloc<kConvProducerRegs>();
     if (warp != 0) return;
     // ===================================================== TMA producer (whole warp walks the loop, one elected lane issues)
     const uint32_t a_bytes = (uint32_t)p.rows * A_ROW_BYTES;
@@ -271,57 +283,220 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
     return;
   }
 
-  // ===================================================== MMA + epilogue (warpgroups 1, 2)
-  tc::regs_alloc<kMmaRegs>();
-  const int wg = (warp >> 2) - 1;              // rows 64 * wg .. 64 * wg + 63 of the tile
-  const int wtid = threadIdx.x & 127;          // thread index inside the warpgroup
-  const int ww = wtid >> 5;                    // warp inside the warpgroup
-  const int bar_id = 2 + wg;
-  const int r_lo = wg * 64 + ww * 16 + (lane >> 2);  // accumulator rows r_lo and r_lo + 8 (tc::wgmma_bf16 layout)
-  constexpr int CH = (OUT_CHUNKS + 1) / 2;   // chunks per warpgroup in the second pass (warpgroup 1 may own fewer)
-  constexpr int CGc = OUT_CW / 8;            // 8-channel groups per chunk
-  constexpr int RGc = 128 / CGc;             // row groups
-  constexpr int ROWSc = 128 / RGc;           // rows per thread in the reduction
-  float* my_scratch = stat_scratch + wg * (4 * CGc * 16);
-  const int my_chunks = (OUT_CHUNKS - wg + 1) / 2;   // warpgroup wg owns chunks wg, wg + 2, ...
-  // per-channel reductions are kept in registers (threads wtid < OUT_CW, one channel per chunk) across all tiles of
-  // this CTA that share an N tile, and flushed with one atomic per channel when the N tile changes / at the end
-  float racc1[CH], racc2[CH];
+  if (warp >= 12) {
+    // ===================================================== epilogue (warpgroup 3): pass 2 and the TMA stores
+    tc::regs_dealloc<kConvEpilogueRegs>();
+    const int wtid = threadIdx.x & 127;
+    const int ww = wtid >> 5;
+    constexpr int CGc = OUT_CW / 8;            // 8-channel groups per chunk
+    constexpr int RGc = 128 / CGc;             // row groups
+    constexpr int ROWSc = 128 / RGc;           // rows per thread in the reduction
+    // aux 1 with bn_dbeta set: per-channel sum of the masked gradient (bias gradient of the producing layer)
+    const bool do_red = (p.stats != nullptr || aux_mode == 2 || (aux_mode == 1 && p.bn_dbeta != nullptr));
+    const bool pass2 = do_red || aux_mode != 0;
+    // per-channel reductions are kept in registers (threads wtid < OUT_CW, one channel per chunk) across all tiles of
+    // this CTA that share an N tile, and added to this CTA's row when the N tile changes / at the end
+    float racc1[OUT_CHUNKS], racc2[OUT_CHUNKS];
 #pragma unroll
-  for (int j = 0; j < CH; ++j) racc1[j] = racc2[j] = 0.f;
-  int racc_nt = -1;
-  // aux 1 with bn_dbeta set: per-channel sum of the masked gradient (bias gradient of the producing layer)
-  const bool do_red = (p.stats != nullptr || aux_mode == 2 || (aux_mode == 1 && p.bn_dbeta != nullptr));
-  uint8_t* abuf = aux_stage + (size_t)wg * OUT_CHUNK_BYTES;
-  uint32_t aux_n = 0;
-  auto issue_aux = [&](int t2, int chunk2) {   // one thread: fetch the aux chunk of tile t2 into abuf
-    const int ph2 = t2 % p.phases;
-    const int mt2 = (t2 / p.phases) % p.m_tiles;
-    const int nt2 = t2 / (p.phases * p.m_tiles);
-    const int tx2 = mt2 % p.tiles_x, ty2 = (mt2 / p.tiles_x) % p.tiles_y, tn2 = mt2 / (p.tiles_x * p.tiles_y);
-    tc::mbar_expect_tx(&aux_full_bar[wg], (uint32_t)p.rows * OUT_ROW_BYTES);
-    tc::tma_load_4d(abuf, &p.tmX[ph2], &aux_full_bar[wg], p.n_off + nt2 * BN + chunk2 * OUT_CW, tx2 * p.bw,
-                    ty2 * p.bh, tn2 * p.bn);
-  };
-  if (aux_mode != 0 && wtid == 0 && my_chunks > 0 && (int)blockIdx.x < total_tiles) issue_aux(blockIdx.x, wg);
-  // this CTA's row of per-channel partial sums; zeroed here, before the first flush (several barriers later)
-  float* red_row = g_conv_red + (size_t)blockIdx.x * p.red_stride;
-  const int red_half = p.red_stride >> 1;
-  if (do_red)
-    for (int i = threadIdx.x - 128; i < p.red_stride; i += 256) red_row[i] = 0.f;
-  auto flush_reductions = [&]() {
-    if (racc_nt >= 0 && wtid < OUT_CW) {
+    for (int j = 0; j < OUT_CHUNKS; ++j) racc1[j] = racc2[j] = 0.f;
+    int racc_nt = -1;
+    // aux chunks travel through a ring of two buffers in (tile, chunk) order: while one is processed the next one is
+    // in flight, and a freed buffer is refilled at once with the chunk two positions ahead
+    uint32_t aux_q = 0;   // aux chunks consumed so far
+    auto issue_aux = [&](int t2, int chunk2, int slot) {   // one thread: chunk2 of tile t2, if that tile exists
+      t2 += (chunk2 / OUT_CHUNKS) * (int)gridDim.x;
+      chunk2 %= OUT_CHUNKS;
+      if (t2 >= total_tiles) return;
+      const int ph2 = t2 % p.phases;
+      const int mt2 = (t2 / p.phases) % p.m_tiles;
+      const int nt2 = t2 / (p.phases * p.m_tiles);
+      const int tx2 = mt2 % p.tiles_x, ty2 = (mt2 / p.tiles_x) % p.tiles_y, tn2 = mt2 / (p.tiles_x * p.tiles_y);
+      tc::mbar_expect_tx(&aux_full_bar[slot], (uint32_t)p.rows * OUT_ROW_BYTES);
+      tc::tma_load_4d(aux_stage + (size_t)slot * OUT_CHUNK_BYTES, &p.tmX[ph2], &aux_full_bar[slot],
+                      p.n_off + nt2 * BN + chunk2 * OUT_CW, tx2 * p.bw, ty2 * p.bh, tn2 * p.bn);
+    };
+    if (aux_mode != 0 && wtid == 0) {
+      issue_aux(blockIdx.x, 0, 0);
+      issue_aux(blockIdx.x, 1, 1);
+    }
+    // this CTA's row of per-channel partial sums; zeroed here, before the first flush (several barriers later)
+    float* red_row = g_conv_red + (size_t)blockIdx.x * p.red_stride;
+    const int red_half = p.red_stride >> 1;
+    if (do_red)
+      for (int i = wtid; i < p.red_stride; i += 128) red_row[i] = 0.f;
+    auto flush_reductions = [&]() {
+      if (racc_nt >= 0 && wtid < OUT_CW) {
 #pragma unroll
-      for (int j = 0; j < CH; ++j) {
-        if (j < my_chunks) {
-          const int ch = racc_nt * BN + (wg + 2 * j) * OUT_CW + wtid;   // relative to p.n_off
+        for (int j = 0; j < OUT_CHUNKS; ++j) {
+          const int ch = racc_nt * BN + j * OUT_CW + wtid;   // relative to p.n_off
           red_row[ch] += racc1[j];
           red_row[red_half + ch] += racc2[j];
           racc1[j] = racc2[j] = 0.f;
         }
       }
+    };
+
+    int it = 0;
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++it) {
+      const int phase_id = t % p.phases;
+      const int mt = (t / p.phases) % p.m_tiles;
+      const int nt = t / (p.phases * p.m_tiles);
+      const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tn = mt / (p.tiles_x * p.tiles_y);
+      const int x0 = tx * p.bw, y0 = ty * p.bh, n0 = tn * p.bn;
+      const int ncol0 = nt * BN;
+      // every row of the tile is a real output pixel (the common case): the second pass skips the per-row checks
+      const bool tile_full = p.rows == 128 && x0 + p.bw <= p.Wv && y0 + p.bh <= p.Hv && n0 + p.bn <= p.Nimg;
+      if (do_red && nt != racc_nt) {
+        flush_reductions();
+        racc_nt = nt;
+      }
+      if (pass2 && !tile_full) {   // (published by the barrier at the top of the first chunk)
+        const int wi = wtid % p.bw, hi = (wtid / p.bw) % p.bh, ni = wtid / (p.bw * p.bh);
+        row_ok[wtid] = wtid < p.rows && x0 + wi < p.Wv && y0 + hi < p.Hv && n0 + ni < p.Nimg;
+      }
+      const int b = it % out_bufs;
+      tc::mbar_wait(&staged_bar[b], (uint32_t)(it / out_bufs) & 1);
+      uint8_t* obuf = out_stage + (size_t)b * OUT_TILE_BYTES;
+
+#pragma unroll 1
+      for (int chunk = 0; chunk < OUT_CHUNKS; ++chunk) {
+        uint8_t* cbuf = obuf + (size_t)chunk * OUT_CHUNK_BYTES;
+        const int aslot = aux_q & 1;
+        if (pass2) {
+          // Second pass over the STORED (bf16) chunk in a (row group, 8-channel group) layout: 16-byte smem accesses,
+          // per-channel coefficients in registers.
+          //   forward:  (sum v, sum v^2) of the valid rows -> BatchNorm batch statistics of the following layer
+          //   aux 1:    g = v * (y > 0), written back in place
+          //   aux 2:    g = v * (bn(z) > 0) written back, (sum g, sum g * xhat) -> dbeta / dgamma of that BatchNorm
+          epi_wg_sync();   // the scratch table of the previous chunk has been read; row_ok is written
+          const uint8_t* abuf = aux_stage + (size_t)aslot * OUT_CHUNK_BYTES;
+          if (aux_mode != 0) tc::mbar_wait(&aux_full_bar[aslot], (aux_q >> 1) & 1);
+          const bool bnred = aux_mode == 2;
+          const int cg = wtid % CGc, rg = wtid / CGc;
+          const int ch0 = p.n_off + ncol0 + chunk * OUT_CW + cg * 8;
+          float s1[8], s2[8], mu[8], is[8], sc[8], sh[8];
+#pragma unroll
+          for (int j = 0; j < 8; ++j) s1[j] = s2[j] = mu[j] = is[j] = sc[j] = sh[j] = 0.f;
+          if (bnred) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              mu[j] = __ldg(p.bn_mean + ch0 + j);
+              is[j] = __ldg(p.bn_invstd + ch0 + j);
+              sc[j] = __ldg(p.bn_gamma + ch0 + j) * is[j];       // same expressions as the forward's
+              sh[j] = __ldg(p.bn_beta + ch0 + j) - mu[j] * sc[j];  // bn_train_coef (elementwise.cu)
+            }
+          }
+          // rows rg*ROWSc .. +ROWSc-1; the swizzle term of row r depends only on rr (OUT_CW 64: r & 7 == rr; 32:
+          // (r >> 1) & 3 == ((rg & 1) * 2 + (rr >> 1))), so every offset is base + compile-time pieces
+          const uint32_t row0_off = (uint32_t)(rg * ROWSc) * OUT_ROW_BYTES;
+          const int swz_rg = (OUT_CW == 64) ? 0 : (rg & 1) * 2;
+#pragma unroll
+          for (int rr = 0; rr < ROWSc; ++rr) {
+            if (!tile_full && !row_ok[rg * ROWSc + rr]) continue;   // ragged tiles only
+            const int unit = (OUT_CW == 64) ? (cg ^ rr) : (cg ^ (swz_rg + (rr >> 1)));
+            const uint32_t off = row0_off + (uint32_t)rr * OUT_ROW_BYTES + (uint32_t)unit * 16;
+            const uint4 pk = *reinterpret_cast<const uint4*>(cbuf + off);
+            const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&pk);
+            if (aux_mode == 0) {
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const float2 xy = __bfloat1622float2(h2[j]);
+                s1[2 * j] += xy.x; s2[2 * j] += xy.x * xy.x;
+                s1[2 * j + 1] += xy.y; s2[2 * j + 1] += xy.y * xy.y;
+              }
+            } else if (aux_mode == 1) {
+              const uint4 ak = *reinterpret_cast<const uint4*>(abuf + off);
+              const uint32_t w[4] = {ak.x, ak.y, ak.z, ak.w};
+              uint32_t o[4] = {pk.x, pk.y, pk.z, pk.w};
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                // bf16 > 0  <=>  sign bit clear and magnitude nonzero
+                const uint32_t lo = w[e] & 0xFFFFu, hi2 = w[e] >> 16;
+                if (!(lo != 0 && lo < 0x8000u)) o[e] &= 0xFFFF0000u;
+                if (!(hi2 != 0 && hi2 < 0x8000u)) o[e] &= 0x0000FFFFu;
+              }
+              *reinterpret_cast<uint4*>(cbuf + off) = make_uint4(o[0], o[1], o[2], o[3]);
+              if (do_red) {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                  s1[2 * e] += __uint_as_float(o[e] << 16);
+                  s1[2 * e + 1] += __uint_as_float(o[e] & 0xFFFF0000u);
+                }
+              }
+            } else {
+              const uint4 zk = *reinterpret_cast<const uint4*>(abuf + off);
+              const __nv_bfloat162* z2 = reinterpret_cast<const __nv_bfloat162*>(&zk);
+              uint32_t o[4] = {pk.x, pk.y, pk.z, pk.w};
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                float2 g = __bfloat1622float2(h2[j]);
+                const float2 zz = __bfloat1622float2(z2[j]);
+                if (!(fmaf(zz.x, sc[2 * j], sh[2 * j]) > 0.f)) { g.x = 0.f; o[j] &= 0xFFFF0000u; }
+                if (!(fmaf(zz.y, sc[2 * j + 1], sh[2 * j + 1]) > 0.f)) { g.y = 0.f; o[j] &= 0x0000FFFFu; }
+                s1[2 * j] += g.x; s2[2 * j] += g.x * ((zz.x - mu[2 * j]) * is[2 * j]);
+                s1[2 * j + 1] += g.y; s2[2 * j + 1] += g.y * ((zz.y - mu[2 * j + 1]) * is[2 * j + 1]);
+              }
+              *reinterpret_cast<uint4*>(cbuf + off) = make_uint4(o[0], o[1], o[2], o[3]);
+            }
+          }
+          if (aux_mode != 0) tc::fence_proxy_async_smem();  // the masked chunk is read by the TMA store below
+          if (do_red) {
+            // combine the row groups of this warp with shuffles (lanes l, l+CGc, ... share a channel group), then the
+            // four warps through a small shared-memory table
+#pragma unroll
+            for (int off = CGc; off < 32; off <<= 1) {
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {
+                s1[j] += __shfl_xor_sync(0xffffffffu, s1[j], off);
+                s2[j] += __shfl_xor_sync(0xffffffffu, s2[j], off);
+              }
+            }
+            if (lane < CGc) {
+              float4* scq = reinterpret_cast<float4*>(stat_scratch + ((size_t)ww * CGc + lane) * 16);
+              scq[0] = make_float4(s1[0], s2[0], s1[1], s2[1]);
+              scq[1] = make_float4(s1[2], s2[2], s1[3], s2[3]);
+              scq[2] = make_float4(s1[4], s2[4], s1[5], s2[5]);
+              scq[3] = make_float4(s1[6], s2[6], s1[7], s2[7]);
+            }
+          }
+          epi_wg_sync();   // the table is complete, and every thread is done with the chunk and its aux buffer
+          if (do_red && wtid < OUT_CW) {
+            float a1 = 0.f, a2 = 0.f;
+#pragma unroll
+            for (int w4 = 0; w4 < 4; ++w4) {
+              const float2 v2 = *reinterpret_cast<const float2*>(stat_scratch + ((size_t)w4 * CGc + (wtid >> 3)) * 16 + (wtid & 7) * 2);
+              a1 += v2.x;
+              a2 += v2.y;
+            }
+#pragma unroll
+            for (int j = 0; j < OUT_CHUNKS; ++j)
+              if (j == chunk) { racc1[j] += a1; racc2[j] += a2; }
+          }
+        }
+
+        if (wtid == 0) {
+          const CUtensorMap* mD = &p.tmD[phase_id];
+          if (p.accumulate) tc::tma_reduce_add_4d(mD, cbuf, p.n_off + ncol0 + chunk * OUT_CW, x0, y0, n0);
+          else tc::tma_store_4d(mD, cbuf, p.n_off + ncol0 + chunk * OUT_CW, x0, y0, n0);
+          if (aux_mode != 0) issue_aux(t, chunk + 2, aslot);   // the aux buffer just processed is free
+        }
+        ++aux_q;
+      }
+      if (wtid == 0) {
+        tc::tma_store_commit();
+        tc::tma_store_wait_read0();
+        tc::mbar_arrive(&drained_bar[b]);   // the MMA warpgroups may stage tile it + out_bufs into buffer b
+      }
     }
-  };
+    if (do_red) flush_reductions();
+    return;
+  }
+
+  // ===================================================== MMA + pass 1 (warpgroups 1, 2)
+  tc::regs_alloc<kConvMmaRegs>();
+  const int wg = (warp >> 2) - 1;              // rows 64 * wg .. 64 * wg + 63 of the tile
+  const int wtid = threadIdx.x & 127;          // thread index inside the warpgroup
+  const int r_lo = wg * 64 + (wtid >> 5) * 16 + (lane >> 2);  // accumulator rows r_lo and r_lo + 8 (tc::wgmma_bf16 layout)
 
   float acc[ACC];
 #pragma unroll
@@ -349,7 +524,16 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
         for (int k = 0; k < BK / 16; ++k) {
           const uint64_t da = da0 + (uint64_t)((k * 32) >> 4);
           const uint64_t db = B_MN ? db0 + (uint64_t)((k * 16 * BMN_ROW_BYTES) >> 4) : db0 + (uint64_t)((k * 32) >> 4);
-          tc::wgmma_bf16<BN, 0, B_MN ? 1 : 0>(acc, da, db, (!first || k > 0) ? 1u : 0u);
+          if constexpr (BN == 256) {
+            // two n = 128 halves: in a 512-thread CTA no instruction may need more than 128 registers, and one
+            // m64n256 wgmma holds 128 accumulators plus its operands.  Same accumulator layout, same K order.
+            constexpr uint32_t B_HALF = B_MN ? 2 * BMN_SUB_BYTES : 128 * A_ROW_BYTES;
+            tc::wgmma_bf16<128, 0, B_MN ? 1 : 0>(*reinterpret_cast<float(*)[64]>(acc), da, db, (!first || k > 0) ? 1u : 0u);
+            tc::wgmma_bf16<128, 0, B_MN ? 1 : 0>(*reinterpret_cast<float(*)[64]>(acc + 64), da, db + (B_HALF >> 4),
+                                                 (!first || k > 0) ? 1u : 0u);
+          } else {
+            tc::wgmma_bf16<BN, 0, B_MN ? 1 : 0>(acc, da, db, (!first || k > 0) ? 1u : 0u);
+          }
         }
         tc::wgmma_commit();
         tc::wgmma_wait<1>();
@@ -402,41 +586,30 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
       release_prev();
     }
 
-    // ---------------------------------------------------- epilogue
+    // ---------------------------------------------------- pass 1
     const int mt = (t / p.phases) % p.m_tiles;
     const int nt = t / (p.phases * p.m_tiles);
     const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tn = mt / (p.tiles_x * p.tiles_y);
     const int x0 = tx * p.bw, y0 = ty * p.bh, n0 = tn * p.bn;
     const int ncol0 = nt * BN;
-    // every row of the tile is a real output pixel (the common case): the second pass skips the per-row checks
-    const bool tile_full = p.rows == 128 && x0 + p.bw <= p.Wv && y0 + p.bh <= p.Hv && n0 + p.bn <= p.Nimg;
-    if (do_red && nt != racc_nt) {
-      flush_reductions();
-      racc_nt = nt;
-    }
-    // staging buffer of this tile: the TMA stores that last read it (OUT_BUFS tiles ago) must have finished reading
-    if (wtid == 0) tc::tma_store_wait_read<OUT_BUFS - 1>();
-    mma_wg_sync();
-    uint8_t* obuf = out_stage + (size_t)(it % OUT_BUFS) * OUT_CHUNKS * OUT_CHUNK_BYTES;
+    // staging buffer of this tile: the TMA stores of the tile that used it before (out_bufs tiles ago) have read it
+    const int b = it % out_bufs;
+    tc::mbar_wait(&drained_bar[b], ((uint32_t)(it / out_bufs) & 1) ^ 1);
+    uint8_t* obuf = out_stage + (size_t)b * OUT_TILE_BYTES;
     // registers -> scale / bias / residual / ReLU -> bf16 -> swizzled staging (the layout the TMA store reads)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = r_lo + 8 * h;
-      const int wi = row % p.bw, hi = (row / p.bw) % p.bh, ni = row / (p.bw * p.bh);
-      const int ox = x0 + wi, oy = y0 + hi, on = n0 + ni;
-      const bool valid = row < p.rows && ox < p.Wv && oy < p.Hv && on < p.Nimg;
-      int pix = -1;
-      if (valid) {
-        pix = 0;
-        if (p.mask_H > 0) {
+      const __nv_bfloat16* rrow = nullptr;
+      if (p.residual != nullptr) {
+        const int wi = row % p.bw, hi = (row / p.bw) % p.bh, ni = row / (p.bw * p.bh);
+        const int ox = x0 + wi, oy = y0 + hi, on = n0 + ni;
+        if (row < p.rows && ox < p.Wv && oy < p.Hv && on < p.Nimg) {
           const int fy = oy * p.mask_s + (p.mask_s == 2 ? (phase_id >> 1) : 0);
           const int fx = ox * p.mask_s + (p.mask_s == 2 ? (phase_id & 1) : 0);
-          pix = (on * p.mask_H + fy) * p.mask_W + fx;
+          rrow = p.residual + (size_t)((on * p.mask_H + fy) * p.mask_W + fx) * p.mask_C + p.n_off + ncol0;
         }
       }
-      if ((lane & 3) == 0) row_pix[row] = pix;
-      const __nv_bfloat16* rrow = nullptr;
-      if (p.residual != nullptr && valid) rrow = p.residual + (size_t)pix * p.mask_C + p.n_off + ncol0;
       uint8_t* rowp = obuf + (size_t)row * OUT_ROW_BYTES;
       const int swz = (OUT_CW == 64) ? (row & 7) : ((row >> 1) & 3);   // SWIZZLE_128B / SWIZZLE_64B
 #pragma unroll
@@ -462,141 +635,10 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
             tc::pack_bf16x2(v0, v1);
       }
     }
-    tc::fence_proxy_async_smem();
-    mma_wg_sync();
-
-    for (int cj = 0; cj < my_chunks; ++cj) {
-      const int chunk = wg + 2 * cj;
-      uint8_t* cbuf = obuf + (size_t)chunk * OUT_CHUNK_BYTES;
-      if (do_red || aux_mode != 0) {
-        // Second pass over the STORED (bf16) chunk in a (row group, 8-channel group) layout: 16-byte smem accesses,
-        // per-channel coefficients in registers.
-        //   forward:  (sum v, sum v^2) of the valid rows -> BatchNorm batch statistics of the following layer
-        //   aux 1:    g = v * (y > 0), written back in place
-        //   aux 2:    g = v * (bn(z) > 0) written back, (sum g, sum g * xhat) -> dbeta / dgamma of that BatchNorm
-        if (cj > 0) asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");   // scratch of the previous chunk read
-        if (aux_mode != 0) {
-          tc::mbar_wait(&aux_full_bar[wg], aux_n & 1);
-          ++aux_n;
-        }
-        const bool bnred = aux_mode == 2;
-        const int cg = wtid % CGc, rg = wtid / CGc;
-        const int ch0 = p.n_off + ncol0 + chunk * OUT_CW + cg * 8;
-        float s1[8], s2[8], mu[8], is[8], sc[8], sh[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) s1[j] = s2[j] = mu[j] = is[j] = sc[j] = sh[j] = 0.f;
-        if (bnred) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            mu[j] = __ldg(p.bn_mean + ch0 + j);
-            is[j] = __ldg(p.bn_invstd + ch0 + j);
-            sc[j] = __ldg(p.bn_gamma + ch0 + j) * is[j];       // same expressions as the forward's
-            sh[j] = __ldg(p.bn_beta + ch0 + j) - mu[j] * sc[j];  // bn_train_coef (elementwise.cu)
-          }
-        }
-        // rows rg*ROWSc .. +ROWSc-1; the swizzle term of row r depends only on rr (OUT_CW 64: r & 7 == rr; 32:
-        // (r >> 1) & 3 == ((rg & 1) * 2 + (rr >> 1))), so every offset is base + compile-time pieces
-        const uint32_t row0_off = (uint32_t)(rg * ROWSc) * OUT_ROW_BYTES;
-        const int swz_rg = (OUT_CW == 64) ? 0 : (rg & 1) * 2;
-#pragma unroll
-        for (int rr = 0; rr < ROWSc; ++rr) {
-          if (!tile_full && row_pix[rg * ROWSc + rr] < 0) continue;   // ragged tiles only
-          const int unit = (OUT_CW == 64) ? (cg ^ rr) : (cg ^ (swz_rg + (rr >> 1)));
-          const uint32_t off = row0_off + (uint32_t)rr * OUT_ROW_BYTES + (uint32_t)unit * 16;
-          const uint4 pk = *reinterpret_cast<const uint4*>(cbuf + off);
-          const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&pk);
-          if (aux_mode == 0) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float2 xy = __bfloat1622float2(h2[j]);
-              s1[2 * j] += xy.x; s2[2 * j] += xy.x * xy.x;
-              s1[2 * j + 1] += xy.y; s2[2 * j + 1] += xy.y * xy.y;
-            }
-          } else if (aux_mode == 1) {
-            const uint4 ak = *reinterpret_cast<const uint4*>(abuf + off);
-            const uint32_t w[4] = {ak.x, ak.y, ak.z, ak.w};
-            uint32_t o[4] = {pk.x, pk.y, pk.z, pk.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              // bf16 > 0  <=>  sign bit clear and magnitude nonzero
-              const uint32_t lo = w[e] & 0xFFFFu, hi2 = w[e] >> 16;
-              if (!(lo != 0 && lo < 0x8000u)) o[e] &= 0xFFFF0000u;
-              if (!(hi2 != 0 && hi2 < 0x8000u)) o[e] &= 0x0000FFFFu;
-            }
-            *reinterpret_cast<uint4*>(cbuf + off) = make_uint4(o[0], o[1], o[2], o[3]);
-            if (do_red) {
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                s1[2 * e] += __uint_as_float(o[e] << 16);
-                s1[2 * e + 1] += __uint_as_float(o[e] & 0xFFFF0000u);
-              }
-            }
-          } else {
-            const uint4 zk = *reinterpret_cast<const uint4*>(abuf + off);
-            const __nv_bfloat162* z2 = reinterpret_cast<const __nv_bfloat162*>(&zk);
-            uint32_t o[4] = {pk.x, pk.y, pk.z, pk.w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              float2 g = __bfloat1622float2(h2[j]);
-              const float2 zz = __bfloat1622float2(z2[j]);
-              if (!(fmaf(zz.x, sc[2 * j], sh[2 * j]) > 0.f)) { g.x = 0.f; o[j] &= 0xFFFF0000u; }
-              if (!(fmaf(zz.y, sc[2 * j + 1], sh[2 * j + 1]) > 0.f)) { g.y = 0.f; o[j] &= 0x0000FFFFu; }
-              s1[2 * j] += g.x; s2[2 * j] += g.x * ((zz.x - mu[2 * j]) * is[2 * j]);
-              s1[2 * j + 1] += g.y; s2[2 * j + 1] += g.y * ((zz.y - mu[2 * j + 1]) * is[2 * j + 1]);
-            }
-            *reinterpret_cast<uint4*>(cbuf + off) = make_uint4(o[0], o[1], o[2], o[3]);
-          }
-        }
-        if (aux_mode != 0) tc::fence_proxy_async_smem();  // the masked chunk is read by the TMA store below
-        if (do_red) {
-          // combine the row groups of this warp with shuffles (lanes l, l+CGc, ... share a channel group), then the
-          // four warps through a small shared-memory table
-#pragma unroll
-          for (int off = CGc; off < 32; off <<= 1) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              s1[j] += __shfl_xor_sync(0xffffffffu, s1[j], off);
-              s2[j] += __shfl_xor_sync(0xffffffffu, s2[j], off);
-            }
-          }
-          if (lane < CGc) {
-            float4* scq = reinterpret_cast<float4*>(my_scratch + ((size_t)ww * CGc + lane) * 16);
-            scq[0] = make_float4(s1[0], s2[0], s1[1], s2[1]);
-            scq[1] = make_float4(s1[2], s2[2], s1[3], s2[3]);
-            scq[2] = make_float4(s1[4], s2[4], s1[5], s2[5]);
-            scq[3] = make_float4(s1[6], s2[6], s1[7], s2[7]);
-          }
-        }
-        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-        if (do_red && wtid < OUT_CW) {
-          float a1 = 0.f, a2 = 0.f;
-#pragma unroll
-          for (int w4 = 0; w4 < 4; ++w4) {
-            const float2 v2 = *reinterpret_cast<const float2*>(my_scratch + ((size_t)w4 * CGc + (wtid >> 3)) * 16 + (wtid & 7) * 2);
-            a1 += v2.x;
-            a2 += v2.y;
-          }
-#pragma unroll
-          for (int j = 0; j < CH; ++j)
-            if (j == cj) { racc1[j] += a1; racc2[j] += a2; }
-        }
-      }
-
-      if (wtid == 0) {
-        const CUtensorMap* mD = &p.tmD[phase_id];
-        if (p.accumulate) tc::tma_reduce_add_4d(mD, cbuf, p.n_off + ncol0 + chunk * OUT_CW, x0, y0, n0);
-        else tc::tma_store_4d(mD, cbuf, p.n_off + ncol0 + chunk * OUT_CW, x0, y0, n0);
-        if (aux_mode != 0) {
-          // abuf is free (every thread of the warpgroup passed the barrier after its last read): fetch the next chunk
-          if (cj + 1 < my_chunks) issue_aux(t, chunk + 2);
-          else if (t + (int)gridDim.x < total_tiles) issue_aux(t + (int)gridDim.x, wg);
-        }
-      }
-    }
-    if (wtid == 0 && my_chunks > 0) tc::tma_store_commit();   // one bulk group per tile (see the wait above)
+    tc::fence_proxy_async_smem();   // the epilogue's TMA stores read the buffer through the async proxy
+    __syncwarp();
+    if (lane == 0) tc::mbar_arrive(&staged_bar[b]);
   }
-  if (do_red) flush_reductions();
-  if (wtid == 0) tc::tma_store_wait_read0();
 }
 
 // -------------------------------------------------------------------------------------------------
