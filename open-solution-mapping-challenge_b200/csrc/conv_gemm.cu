@@ -41,6 +41,7 @@ static void pick_tile(int Wv, int Hv, int N, int max_rows, int row_mult, int* pb
 // them the fp32 summation order: rewriting one can change a rounding, a split count and so the results' last bits.
 constexpr int kSmemBudget = 227 * 1024;               // dynamic shared memory of one CTA (the sm_90 maximum)
 constexpr int kMaxStagesHalo = 9, kMaxStages = 6;     // operand ring depth, haloed / per-tap path
+constexpr int kWgradMaxStages = 8;                    // ... of the weight-gradient GEMMs
 constexpr int kTwoStagingMinStages = 3;               // two epilogue staging buffers while the ring keeps this many stages
 constexpr int kHaloMinChannels = 128;                 // haloed tile from this many channels per tap
 constexpr int kBn256MinWaveX10 = 6;                   // 256-wide N tiles down to 0.6 of a wave
@@ -48,6 +49,9 @@ constexpr int kWgradWavesX10 = 10;                    // weight-gradient grid: o
 constexpr int kWgradMinKb = 6;                        // K blocks (pixel tiles) per weight-gradient CTA, at least
 constexpr int kWgradKbTarget = 64;                    // ... and aimed at for short reductions
 constexpr int kWgradMinWaveX10 = 4;                   // ... keeping at least 0.4 of a wave busy
+
+static_assert(conv_smem(32, 32, true, kMaxStagesHalo, 1, 0).fits && conv_smem(32, 32, false, kMaxStages, 1, 0).fits &&
+                  wgrad_smem(32, kWgradMaxStages).fits, "the mbarriers outgrow their reserve at the deepest rings");
 
 // Test hooks: they force a regime that a test's shapes would not reach under the launch rules.  Unset (the default),
 // the rules decide, and that is the only path the library takes in use.  Read on every launch, so that a test can
@@ -64,60 +68,53 @@ static TestHooks test_hooks() {
   return {get("MCB_FORCE_BN", 0), get("MCB_HALO", 2), get("MCB_WGRAD_SPLITS", 0)};
 }
 
-template <int BN, int BK, bool B_MN, bool HALO>
-static int launch_conv_inst(const ConvGemmParams& p, dim3 grid, size_t smem, cudaStream_t st) {
+// Launches one kernel instantiation; its first launch raises its dynamic shared-memory limit to kSmemBudget
+template <auto Kernel, class Params>
+static int launch_kernel(const Params& p, dim3 grid, int threads, size_t smem, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    MCB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, BK, B_MN, HALO>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
+    MCB_CHECK_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
     attr_set = true;
   }
-  conv_gemm_kernel<BN, BK, B_MN, HALO><<<grid, kConvThreads, smem, st>>>(p);
+  Kernel<<<grid, threads, smem, st>>>(p);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }
 
-template <int BK, bool B_MN, bool HALO>
-static int launch_conv_bn(int BN, const ConvGemmParams& p, dim3 grid, size_t smem, cudaStream_t st) {
-  switch (BN) {
-    case 256: return launch_conv_inst<256, BK, B_MN, HALO>(p, grid, smem, st);
-    case 128: return launch_conv_inst<128, BK, B_MN, HALO>(p, grid, smem, st);
-    case 64: return launch_conv_inst<64, BK, B_MN, HALO>(p, grid, smem, st);
-    case 32: return launch_conv_inst<32, BK, B_MN, HALO>(p, grid, smem, st);
-  }
-  return fail(MCB_ERR_UNSUPPORTED, "unsupported BN %d", BN);
+// the conv_gemm_kernel instantiation for (BN, BK, b_mn, halo); with_flag passes a run-time flag as a template argument
+static int launch_conv_kernel(int BN, int BK, bool b_mn, bool halo, const ConvGemmParams& p, dim3 grid, size_t smem,
+                              cudaStream_t st) {
+  auto with_flag = [](bool v, auto f) { return v ? f(std::true_type()) : f(std::false_type()); };
+  return with_flag(BK == 64, [&](auto bk64) { return with_flag(b_mn, [&](auto mn) { return with_flag(halo, [&](auto h) {
+    constexpr int K = decltype(bk64)::value ? 64 : 32;
+    constexpr bool M = decltype(mn)::value, H = decltype(h)::value;
+    switch (BN) {
+      case 256: return launch_kernel<conv_gemm_kernel<256, K, M, H>>(p, grid, kConvThreads, smem, st);
+      case 128: return launch_kernel<conv_gemm_kernel<128, K, M, H>>(p, grid, kConvThreads, smem, st);
+      case 64: return launch_kernel<conv_gemm_kernel<64, K, M, H>>(p, grid, kConvThreads, smem, st);
+      case 32: return launch_kernel<conv_gemm_kernel<32, K, M, H>>(p, grid, kConvThreads, smem, st);
+    }
+    return fail(MCB_ERR_UNSUPPORTED, "unsupported BN %d", BN);
+  }); }); });
 }
 
 static int launch_conv(int BN, int BK, bool b_mn, ConvGemmParams& p, int m_tiles, int n_tiles, int phases,
                        cudaStream_t st, bool halo = false) {
-  const int a_bytes = halo ? ((kHaloW * kHaloH * BK * 2 + 1023) / 1024) * 1024 : 128 * BK * 2;
-  const int b_bytes = BN * BK * 2;
-  const int stage = halo ? b_bytes : a_bytes + b_bytes;
-  const int out_buf_bytes = 128 * BN * 2;  // one bf16 staging buffer
-  const int aux_bytes = p.aux_mode != 0 ? 2 * 128 * (BN >= 64 ? 64 : 32) * 2 : 0;  // the epilogue's ring of two aux chunks
-  const int base = aux_bytes + kStatBytes + 1024 /*align*/ + 1536 /*barriers, row table*/ + (halo ? 2 * a_bytes : 0);
-  const int out_bufs = (kSmemBudget - base - 2 * out_buf_bytes) / stage >= kTwoStagingMinStages ? 2 : 1;
-  const int fixed = base + out_bufs * out_buf_bytes;
-  const int stages = std::max(2, std::min(halo ? kMaxStagesHalo : kMaxStages, (kSmemBudget - fixed) / stage));
-  p.stages = stages;
-  p.out_bufs = out_bufs;
+  auto layout = [&](int stages, int out_bufs) { return conv_smem(BN, BK, halo, stages, out_bufs, p.aux_mode != 0); };
+  // (layout(0, b).bytes: everything but the operand ring)
+  const int stage = layout(0, 0).stage, max_stages = halo ? kMaxStagesHalo : kMaxStages;
+  p.out_bufs = (kSmemBudget - layout(0, 2).bytes) / stage >= kTwoStagingMinStages ? 2 : 1;
+  p.stages = std::max(2, std::min(max_stages, (kSmemBudget - layout(0, p.out_bufs).bytes) / stage));
   p.m_tiles = m_tiles; p.n_tiles = n_tiles; p.phases = phases;
-  const size_t smem = (size_t)stages * stage + fixed;
+  const size_t smem = layout(p.stages, p.out_bufs).bytes;
   const long total = (long)m_tiles * n_tiles * phases;
   dim3 grid((unsigned)std::min<long>(total, num_sms()), 1, 1);
   const int nch = n_tiles * BN;  // N extent of this launch, channels p.n_off ..
-  const bool red = p.stats != nullptr || p.aux_mode == 2 || (p.aux_mode == 1 && p.bn_dbeta != nullptr);
+  const bool red = conv_reduces(p);
   p.red_stride = 2 * nch;
   if (red && (long)grid.x * p.red_stride > kConvRedCap)
     return fail(MCB_ERR_UNSUPPORTED, "conv: reduction rows %u x %d exceed the workspace", grid.x, p.red_stride);
-  int r;
-  if (halo) {
-    if (BK == 64) r = b_mn ? launch_conv_bn<64, true, true>(BN, p, grid, smem, st) : launch_conv_bn<64, false, true>(BN, p, grid, smem, st);
-    else r = b_mn ? launch_conv_bn<32, true, true>(BN, p, grid, smem, st) : launch_conv_bn<32, false, true>(BN, p, grid, smem, st);
-  } else {
-    if (BK == 64) r = b_mn ? launch_conv_bn<64, true, false>(BN, p, grid, smem, st) : launch_conv_bn<64, false, false>(BN, p, grid, smem, st);
-    else r = b_mn ? launch_conv_bn<32, true, false>(BN, p, grid, smem, st) : launch_conv_bn<32, false, false>(BN, p, grid, smem, st);
-  }
+  const int r = launch_conv_kernel(BN, BK, b_mn, halo, p, grid, smem, st);
   if (r || !red) return r;
   // per-channel sums of the CTAs' rows, in CTA order (detsum.cuh)
   const int rows = (int)grid.x;
@@ -148,11 +145,15 @@ static bool use_halo(int ksize, int stride, int W, int H, int k_channels) {
   return eff >= 0.8;
 }
 
+// the widest N tile that divides n channels
+static int widest_bn(int n) {
+  for (int bn : {256, 128, 64})
+    if (n % bn == 0) return bn;
+  return 32;
+}
+
 static int pick_bn(int n_total, long m_tiles, int phases) {
-  int bn = 32;
-  for (int cand : {256, 128, 64, 32}) {
-    if (n_total % cand == 0) { bn = cand; break; }
-  }
+  int bn = widest_bn(n_total);
   // keep the machine filled when the pixel dimension is small
   const long sms = num_sms();
   // (fat tiles beat many thin ones: go below 128 only when even 128-wide tiles leave most SMs idle; one round of
@@ -274,29 +275,16 @@ static int plan_conv(ConvGemmParams& p, const TapRule& rule, const View* a, int 
                               halo ? kHaloH : p.bh, p.bn)) return r;
 
   const int BN = pick_bn(out.c, m_tiles, phases);
-  const int cw = BN >= 64 ? 64 : 32;  // channel width of the output / aux boxes and of the MN-major weight box
   const int wtaps = rule.ksize * rule.ksize;
-  if (int r = b_mn ? encode_weight(&p.tmB, w, wtaps, a[0].c, w_pitch, w_off, out.c, cw, BK)
+  if (int r = b_mn ? encode_weight(&p.tmB, w, wtaps, a[0].c, w_pitch, w_off, out.c, chunk_width(BN), BK)
                    : encode_weight(&p.tmB, w, wtaps, out.c, w_pitch, 0, w_pitch, BK, BN)) return r;
   const View aux_view = {aux, out.n, out.h, out.w, out.c};
   for (int ph = 0; ph < phases; ++ph) {
-    if (int r = encode_view(&p.tmD[ph], out, phase_slot[ph], cw, p.bw, p.bh, p.bn)) return r;
+    if (int r = encode_view(&p.tmD[ph], out, phase_slot[ph], chunk_width(BN), p.bw, p.bh, p.bn)) return r;
     if (aux)
-      if (int r = encode_view(&p.tmX[ph], aux_view, phase_slot[ph], cw, p.bw, p.bh, p.bn)) return r;
+      if (int r = encode_view(&p.tmX[ph], aux_view, phase_slot[ph], chunk_width(BN), p.bw, p.bh, p.bn)) return r;
   }
   return launch_conv(BN, BK, b_mn, p, (int)m_tiles, out.c / BN, phases, st, halo);
-}
-
-template <int BN>
-static int launch_wgrad_inst(const WgradParams& p, dim3 grid, size_t smem, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    MCB_CHECK_CUDA(cudaFuncSetAttribute(wgrad_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget));
-    attr_set = true;
-  }
-  wgrad_kernel<BN><<<grid, kGemmThreads, smem, st>>>(p);
-  MCB_LAUNCH_CHECK();
-  return MCB_OK;
 }
 
 // Region of g_wgrad_red for launches on stream st.  Launches of one stream are serialised; launches of different
@@ -319,10 +307,7 @@ static long wgrad_region_offset(cudaStream_t st) {
   return (long)r * kWgradRegionCap;
 }
 
-static int launch_wgrad(WgradParams& p, int cin_src, cudaStream_t st) {
-  int BN = 32;
-  for (int cand : {256, 128, 64, 32})
-    if (cin_src % cand == 0) { BN = cand; break; }
+static int launch_wgrad(WgradParams& p, int BN, int cin_src, cudaStream_t st) {
   const int m_tiles = (p.cout + 127) / 128;
   const int n_tiles = cin_src / BN;
   // split-K over the pixel tiles so the grid covers the machine a few times
@@ -348,18 +333,16 @@ static int launch_wgrad(WgradParams& p, int cin_src, cudaStream_t st) {
   if (splits > 1) splits = (int)std::max(1L, std::min((long)splits, kWgradRegionCap / p.slice));
   p.ws_off = splits > 1 ? wgrad_region_offset(st) : 0;
   p.splits = splits;
-  const int b_cw = BN >= 64 ? 64 : 32;
-  const int stage = 2 * 64 * 128 + (BN / b_cw) * 64 * b_cw * 2;
   const int per = (p.tiles_total + splits - 1) / splits;
-  p.stages = std::max(2, std::min(std::min(per, 8), kSmemBudget / stage));
-  const size_t smem = (size_t)p.stages * stage + 1024 + 512;
+  p.stages = std::max(2, std::min(std::min(per, kWgradMaxStages), kSmemBudget / wgrad_smem(BN, 0).stage));
+  const size_t smem = wgrad_smem(BN, p.stages).bytes;
   dim3 grid(n_tiles, m_tiles, p.ntaps * splits);
   int r;
   switch (BN) {
-    case 256: r = launch_wgrad_inst<256>(p, grid, smem, st); break;
-    case 128: r = launch_wgrad_inst<128>(p, grid, smem, st); break;
-    case 64: r = launch_wgrad_inst<64>(p, grid, smem, st); break;
-    default: r = launch_wgrad_inst<32>(p, grid, smem, st); break;
+    case 256: r = launch_kernel<wgrad_kernel<256>>(p, grid, kGemmThreads, smem, st); break;
+    case 128: r = launch_kernel<wgrad_kernel<128>>(p, grid, kGemmThreads, smem, st); break;
+    case 64: r = launch_kernel<wgrad_kernel<64>>(p, grid, kGemmThreads, smem, st); break;
+    default: r = launch_kernel<wgrad_kernel<32>>(p, grid, kGemmThreads, smem, st); break;
   }
   if (r || splits == 1) return r;
   // the splits that own pixel tiles, summed in split order into dW[tap][cout][ci_off + ci] (detsum.cuh)
@@ -403,14 +386,15 @@ static int plan_wgrad(WgradParams& p, const TapRule& rule, const View& dy, const
   });
   p.ntaps = nt;
   const bool parity = rule.stride == 2;
-  const int b_cw = (x.c % 64 == 0) ? 64 : 32;
+  const int BN = widest_bn(x.c);
   for (int v = 0; v < 4; ++v) {
     if (used_a[v])
       if (int r = encode_view(&p.tmA[v], dy, taps_on_dy && parity ? v : -1, p.a_cw, p.bw, p.bh, p.bn)) return r;
     if (used_b[v])
-      if (int r = encode_view(&p.tmB[v], x, !taps_on_dy && parity ? v : -1, b_cw, p.bw, p.bh, p.bn)) return r;
+      if (int r = encode_view(&p.tmB[v], x, !taps_on_dy && parity ? v : -1, chunk_width(BN), p.bw, p.bh, p.bn))
+        return r;
   }
-  return launch_wgrad(p, x.c, st);
+  return launch_wgrad(p, BN, x.c, st);
 }
 
 }  // namespace mcb

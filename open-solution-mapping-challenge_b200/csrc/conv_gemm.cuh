@@ -115,14 +115,13 @@ __device__ __forceinline__ uint8_t* align_up_1024(uint8_t* p) {
 
 
 // -------------------------------------------------------------------------------------------------
-// Persistent, warp-specialised: one CTA per SM walks tiles t = blockIdx.x, += gridDim.x (n fastest, so CTAs that run
-// together share the A pixel tile in L2).  The TMA ring (full/empty mbarriers) runs continuously across tiles, and so
-// do the MMA warpgroups: after a tile's main loop they only write the accumulators through scale / bias / residual /
-// ReLU to a bf16 staging buffer (pass 1), signal staged[b] and start the next tile's main loop.  The epilogue
-// warpgroup runs the second pass over the staged tile (BatchNorm statistics, ReLU / BatchNorm-backward masks and
-// their channel sums), issues the TMA stores and signals drained[b] once they have read the buffer.  With two staging
-// buffers pass 1 of tile i+1 never waits for the epilogue of tile i; with one it waits for the drain of tile i, which
-// had the whole main loop of tile i+1 to finish.
+// Persistent, warp-specialised: one CTA per SM walks tiles t = blockIdx.x, += gridDim.x in conv_tile's order (below).
+// The TMA ring (full/empty mbarriers) runs continuously across tiles, and so do the MMA warpgroups: after a tile's
+// main loop they only write the accumulators through scale / bias / residual / ReLU to a bf16 staging buffer (pass 1),
+// signal staged[b] and start the next tile's main loop.  The epilogue warpgroup runs the second pass over the staged
+// tile (BatchNorm statistics, ReLU / BatchNorm-backward masks and their channel sums), issues the TMA stores and
+// signals drained[b] once they have read the buffer.  With two staging buffers pass 1 of tile i+1 never waits for the
+// epilogue of tile i; with one it waits for the drain of tile i, which had the whole main loop of tile i+1 to finish.
 constexpr int kConvThreads = 512;  // warpgroup 0 TMA producer, warpgroups 1, 2 MMA + pass 1, warpgroup 3 epilogue
 // 128 x 24 + 128 x 120 + 256 x 184 = 64 K registers: BN = 256's 128 fp32 accumulators in the MMA warpgroups, pass 2's
 // per-thread state in the epilogue warpgroup, neither spilling (ptxas -v)
@@ -138,6 +137,58 @@ constexpr int kHaloW = 10, kHaloH = 18;  // (8 + 2) x (16 + 2)
 // per-channel reduction scratch of the epilogue warpgroup: 4 warps x (up to) 8 channel groups x 16 floats
 constexpr int kStatBytes = 4 * 8 * 16 * 4;
 
+// Channels per chunk of an N tile: the epilogue's staging and aux chunks and their TMA boxes, the MN-major B sub-tiles
+// of conv_gemm_kernel and the B sub-tiles of wgrad_kernel.  64 (SW128 rows) from BN = 64 up, else 32 (SW64).
+__host__ __device__ constexpr int chunk_width(int bn) { return bn >= 64 ? 64 : 32; }
+
+// the launch sums per-channel values into g_conv_red: BatchNorm statistics (stats), dbeta / dgamma (aux 2), or the
+// masked gradient (aux 1 with bn_dbeta: the bias gradient of the producing layer)
+__host__ __device__ __forceinline__ bool conv_reduces(const ConvGemmParams& p) {
+  return p.stats != nullptr || p.aux_mode == 2 || (p.aux_mode == 1 && p.bn_dbeta != nullptr);
+}
+
+// A launch's dynamic shared memory adds to the kernel's 1024-byte-aligned pieces the slack of aligning the window up to
+// 1024 bytes, and a fixed reserve after the pieces for the mbarriers (and conv_gemm_kernel's row table)
+constexpr int kSmemAlignSlack = 1024, kConvBarrierReserve = 1536, kWgradBarrierReserve = 512;
+
+// conv_gemm_kernel's dynamic shared memory, byte offsets from the 1024-aligned base: the operand ring of `stages` slots
+// (A + B tiles; HALO: B tiles only), two haloed A slots (HALO), out_bufs bf16 staging buffers, the epilogue's ring of
+// two aux chunks (aux modes) and its reduction scratch, the mbarriers and the row table.  launch_conv sizes from it.
+struct ConvSmem { int a_tile, stage, a_ring, out_stage, aux_stage, stat_scratch, bars, row_ok, bytes; bool fits; };
+__host__ __device__ constexpr ConvSmem conv_smem(int bn, int bk, bool halo, int stages, int out_bufs, bool aux) {
+  ConvSmem l{};
+  l.a_tile = halo ? (kHaloW * kHaloH * bk * 2 + 1023) / 1024 * 1024 : 128 * bk * 2;  // haloed: rounded up to 1024
+  l.stage = (halo ? 0 : l.a_tile) + bn * bk * 2;
+  l.a_ring = stages * l.stage;
+  l.out_stage = l.a_ring + (halo ? 2 * l.a_tile : 0);
+  l.aux_stage = l.out_stage + out_bufs * 128 * bn * 2;
+  l.stat_scratch = l.aux_stage + (aux ? 2 * 128 * chunk_width(bn) * 2 : 0);
+  l.bars = l.stat_scratch + kStatBytes;
+  l.row_ok = l.bars + (2 * stages + 10) * 8;  // full, empty [stages]; a_full, a_empty, aux_full, staged, drained [2]
+  l.bytes = kSmemAlignSlack + l.bars + kConvBarrierReserve;
+  l.fits = l.row_ok + 128 * 4 <= l.bars + kConvBarrierReserve;  // the mbarriers and the row table fit the reserve
+  return l;
+}
+
+// wgrad_kernel's dynamic shared memory: the operand ring of `stages` slots (A: two 64-pixel x 64-channel sub-tiles,
+// B: 64 pixels x BN channels), then the full / empty mbarriers
+struct WgradSmem { int stage, bars, bytes; bool fits; };
+__host__ __device__ constexpr WgradSmem wgrad_smem(int bn, int stages) {
+  const int stage = 2 * 64 * 128 + 64 * bn * 2, bars = stages * stage;
+  return {stage, bars, kSmemAlignSlack + bars + kWgradBarrierReserve, 2 * stages * 8 <= kWgradBarrierReserve};
+}
+
+// Tile t of conv_gemm_kernel's persistent tile space: phase (tap range, tmD), N tile, its first column (from p.n_off)
+// and its pixel box.  Order: phase fastest (the phases of one pixel tile share the A tile in L2), then pixel tile, N
+// tile slowest (CTAs running together share the weight tile; a CTA keeps its N tile for many tiles in a row).
+struct ConvTile { int phase, nt, ncol0, x0, y0, n0; };
+template <int BN>
+__device__ __forceinline__ ConvTile conv_tile(const ConvGemmParams& p, int t) {
+  const int mt = (t / p.phases) % p.m_tiles, nt = t / (p.phases * p.m_tiles);
+  const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tn = mt / (p.tiles_x * p.tiles_y);
+  return {t % p.phases, nt, nt * BN, tx * p.bw, ty * p.bh, tn * p.bn};
+}
+
 __device__ __forceinline__ void epi_wg_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 
 template <int BN, int BK, bool B_MN, bool HALO>
@@ -145,21 +196,17 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
   static_assert(BK == 64 || BK == 32, "BK");
   static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN");
   constexpr int A_ROW_BYTES = BK * 2;              // 128 (SW128) or 64 (SW64)
-  constexpr int A_BYTES = HALO ? ((kHaloW * kHaloH * A_ROW_BYTES + 1023) / 1024) * 1024 : 128 * A_ROW_BYTES;
+  constexpr ConvSmem SIZES = conv_smem(BN, BK, HALO, 0, 0, false);
+  constexpr int A_BYTES = SIZES.a_tile, STAGE_BYTES = SIZES.stage;  // HALO: the ring holds B tiles; A has 2 own slots
   constexpr int B_BYTES = BN * BK * 2;
-  constexpr int STAGE_BYTES = HALO ? B_BYTES : A_BYTES + B_BYTES;  // HALO: the ring holds B tiles; A has its own 2 slots
-  constexpr int A_RING_BYTES = HALO ? 2 * A_BYTES : 0;
   constexpr uint32_t A_LAYOUT = (BK == 64) ? tc::LAYOUT_SW128 : tc::LAYOUT_SW64;
-  // MN-major B: rows are K (BK of them), each row holds min(BN,64) n-values
-  constexpr int BMN_CW = (BN >= 64) ? 64 : 32;          // n-values per sub-tile row
-  constexpr int BMN_ROW_BYTES = BMN_CW * 2;             // 128 or 64
-  constexpr int BMN_SUB_BYTES = BK * BMN_ROW_BYTES;     // one sub-tile
-  constexpr uint32_t BMN_LAYOUT = (BMN_CW == 64) ? tc::LAYOUT_SW128 : tc::LAYOUT_SW64;
-  // output staging: chunks of OUT_CW channels (one TMA store each)
-  constexpr int OUT_CW = (BN >= 64) ? 64 : 32;
-  constexpr int OUT_ROW_BYTES = OUT_CW * 2;
-  constexpr int OUT_CHUNK_BYTES = 128 * OUT_ROW_BYTES;
-  constexpr int OUT_CHUNKS = BN / OUT_CW;
+  // MN-major B: rows are K (BK of them), each row holds one chunk of n-values; output staging: one TMA store per chunk
+  constexpr int CW = chunk_width(BN);
+  constexpr uint32_t CW_LAYOUT = (CW == 64) ? tc::LAYOUT_SW128 : tc::LAYOUT_SW64;
+  constexpr int CW_ROW_BYTES = CW * 2;                  // 128 or 64
+  constexpr int BMN_SUB_BYTES = BK * CW_ROW_BYTES;      // one MN-major B sub-tile
+  constexpr int OUT_CHUNK_BYTES = 128 * CW_ROW_BYTES;
+  constexpr int OUT_CHUNKS = BN / CW;
   constexpr int OUT_TILE_BYTES = OUT_CHUNKS * OUT_CHUNK_BYTES;   // one staging buffer
   constexpr int ACC = BN / 2;  // fp32 accumulators per thread (64 x BN per warpgroup)
 
@@ -168,18 +215,19 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
   const int stages = p.stages;
   const int out_bufs = p.out_bufs;   // staging buffers: 1 or 2 (launch_conv)
   const int aux_mode = p.aux_mode;
-  uint8_t* a_ring = smem + (size_t)stages * STAGE_BYTES;               // HALO only: 2 haloed A tiles
-  uint8_t* out_stage = a_ring + A_RING_BYTES;                          // 1024-aligned (all pieces are)
-  uint8_t* aux_stage = out_stage + (size_t)out_bufs * OUT_TILE_BYTES;  // aux modes: a ring of two chunks
-  float* stat_scratch = reinterpret_cast<float*>(aux_stage + (aux_mode != 0 ? 2 * OUT_CHUNK_BYTES : 0));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stat_scratch) + kStatBytes);
+  const ConvSmem L = conv_smem(BN, BK, HALO, stages, out_bufs, aux_mode != 0);
+  uint8_t* a_ring = smem + L.a_ring;               // HALO only: 2 haloed A tiles
+  uint8_t* out_stage = smem + L.out_stage;        // 1024-aligned (all pieces are)
+  uint8_t* aux_stage = smem + L.aux_stage;         // aux modes: a ring of two chunks
+  float* stat_scratch = reinterpret_cast<float*>(smem + L.stat_scratch);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L.bars);
   uint64_t* empty_bar = full_bar + stages;
   uint64_t* a_full_bar = empty_bar + stages;      // [2] (HALO)
   uint64_t* a_empty_bar = a_full_bar + 2;         // [2] (HALO)
   uint64_t* aux_full_bar = a_empty_bar + 2;       // [2] aux ring
   uint64_t* staged_bar = aux_full_bar + 2;        // [2] per staging buffer: pass 1 done (one arrival per MMA warp)
   uint64_t* drained_bar = staged_bar + 2;         // [2] per staging buffer: its TMA stores have read it
-  int* row_ok = reinterpret_cast<int*>(drained_bar + 2);  // [128] ragged tiles: the row is an output pixel
+  int* row_ok = reinterpret_cast<int*>(smem + L.row_ok);  // [128] ragged tiles: the row is an output pixel
 
   // the shuffle makes the warp index provably warp-uniform, so the role loops below compile onto the uniform datapath
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
@@ -192,11 +240,9 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
       tc::mbar_init(&full_bar[s], 1);
       tc::mbar_init(&empty_bar[s], 2);  // one arrival per MMA warpgroup
     }
-    tc::mbar_init(&a_full_bar[0], 1);
-    tc::mbar_init(&a_full_bar[1], 1);
-    tc::mbar_init(&a_empty_bar[0], 2);
-    tc::mbar_init(&a_empty_bar[1], 2);
     for (int b = 0; b < 2; ++b) {
+      tc::mbar_init(&a_full_bar[b], 1);
+      tc::mbar_init(&a_empty_bar[b], 2);
       tc::mbar_init(&aux_full_bar[b], 1);
       tc::mbar_init(&staged_bar[b], 8);
       tc::mbar_init(&drained_bar[b], 1);
@@ -213,25 +259,17 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
     // ===================================================== TMA producer (whole warp walks the loop, one elected lane issues)
     const uint32_t a_bytes = (uint32_t)p.rows * A_ROW_BYTES;
     uint32_t ag = 0;  // HALO: haloed A tiles issued so far
-    int ring_s = 0;            // pipeline slot / phase parity, advanced without integer division: the single-thread
-    uint32_t ring_ph = 0;      // producer loop is a latency chain, every instruction in it is exposed
+    tc::RingPos ring;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      // tile order: phase fastest (the phases of one pixel tile share the A tile in L2), then pixel tile, N tile
-      // slowest (CTAs running together share the weight tile; a CTA keeps its N tile for many tiles in a row)
-      const int phase_id = t % p.phases;
-      const int mt = (t / p.phases) % p.m_tiles;
-      const int nt = t / (p.phases * p.m_tiles);
-      const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tn = mt / (p.tiles_x * p.tiles_y);
-      const int x0 = tx * p.bw, y0 = ty * p.bh, n0 = tn * p.bn;
-      const int ncol0 = nt * BN;
-      const int tap_begin = p.tap_start[phase_id], tap_end = tap_begin + p.tap_count[phase_id];
+      const ConvTile tile = conv_tile<BN>(p, t);
+      const int tap_begin = p.tap_start[tile.phase], tap_end = tap_begin + p.tap_count[tile.phase];
       auto load_b = [&](uint8_t* sb, uint64_t* bar, const TapDesc& tap, int ch) {
         if (!B_MN) {
-          tc::tma_load_3d(sb, &p.tmB, bar, tap.wk0 + ch * BK, p.n_off + ncol0, tap.wtap);
+          tc::tma_load_3d(sb, &p.tmB, bar, tap.wk0 + ch * BK, p.n_off + tile.ncol0, tap.wtap);
         } else {
 #pragma unroll
-          for (int j = 0; j < BN / BMN_CW; ++j)
-            tc::tma_load_3d(sb + j * BMN_SUB_BYTES, &p.tmB, bar, p.n_off + ncol0 + j * BMN_CW, tap.wk0 + ch * BK,
+          for (int j = 0; j < BN / CW; ++j)
+            tc::tma_load_3d(sb + j * BMN_SUB_BYTES, &p.tmB, bar, p.n_off + tile.ncol0 + j * CW, tap.wk0 + ch * BK,
                             tap.wtap);
         }
       };
@@ -245,18 +283,16 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
             tc::mbar_wait(&a_empty_bar[as], ((ag >> 1) & 1) ^ 1);
             if (tc::elect_one()) {
               tc::mbar_expect_tx(&a_full_bar[as], (uint32_t)(kHaloW * kHaloH * A_ROW_BYTES));
-              tc::tma_load_4d(a_ring + (size_t)as * A_BYTES, &p.tmA[t0.src], &a_full_bar[as], ch * BK, x0 - 1, y0 - 1, n0);
+              tc::tma_load_4d(a_ring + (size_t)as * A_BYTES, &p.tmA[t0.src], &a_full_bar[as], ch * BK, tile.x0 - 1,
+                              tile.y0 - 1, tile.n0);
             }
             for (int t = 0; t < 9; ++t) {
               const TapDesc tap = p.taps[tap_begin + t * nsrc + sidx];
-              const int s = ring_s;
-              const uint32_t ph = ring_ph;
-              if (++ring_s == stages) { ring_s = 0; ring_ph ^= 1; }
-              tc::mbar_wait(&empty_bar[s], ph ^ 1);
-              uint8_t* sb = smem + (size_t)s * STAGE_BYTES;
+              const tc::RingPos r = ring.step(stages);
+              tc::mbar_wait(&empty_bar[r.slot], r.parity ^ 1);
               if (tc::elect_one()) {
-                tc::mbar_expect_tx(&full_bar[s], B_BYTES);
-                load_b(sb, &full_bar[s], tap, ch);
+                tc::mbar_expect_tx(&full_bar[r.slot], B_BYTES);
+                load_b(smem + (size_t)r.slot * STAGE_BYTES, &full_bar[r.slot], tap, ch);
               }
             }
           }
@@ -267,15 +303,13 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
         const TapDesc tap = p.taps[tp];
         const CUtensorMap* mA = &p.tmA[tap.src];
         for (int ch = 0; ch < tap.nchunks; ++ch) {
-          const int s = ring_s;
-          const uint32_t ph = ring_ph;
-          if (++ring_s == stages) { ring_s = 0; ring_ph ^= 1; }
-          tc::mbar_wait(&empty_bar[s], ph ^ 1);
-          uint8_t* sa = smem + (size_t)s * STAGE_BYTES;
+          const tc::RingPos r = ring.step(stages);
+          tc::mbar_wait(&empty_bar[r.slot], r.parity ^ 1);
+          uint8_t* sa = smem + (size_t)r.slot * STAGE_BYTES;
           if (tc::elect_one()) {
-            tc::mbar_expect_tx(&full_bar[s], a_bytes + B_BYTES);
-            tc::tma_load_4d(sa, mA, &full_bar[s], ch * BK, x0 + tap.dx, y0 + tap.dy, n0);
-            load_b(sa + A_BYTES, &full_bar[s], tap, ch);
+            tc::mbar_expect_tx(&full_bar[r.slot], a_bytes + B_BYTES);
+            tc::tma_load_4d(sa, mA, &full_bar[r.slot], ch * BK, tile.x0 + tap.dx, tile.y0 + tap.dy, tile.n0);
+            load_b(sa + A_BYTES, &full_bar[r.slot], tap, ch);
           }
         }
       }
@@ -288,13 +322,12 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
     tc::regs_dealloc<kConvEpilogueRegs>();
     const int wtid = threadIdx.x & 127;
     const int ww = wtid >> 5;
-    constexpr int CGc = OUT_CW / 8;            // 8-channel groups per chunk
+    constexpr int CGc = CW / 8;                // 8-channel groups per chunk
     constexpr int RGc = 128 / CGc;             // row groups
     constexpr int ROWSc = 128 / RGc;           // rows per thread in the reduction
-    // aux 1 with bn_dbeta set: per-channel sum of the masked gradient (bias gradient of the producing layer)
-    const bool do_red = (p.stats != nullptr || aux_mode == 2 || (aux_mode == 1 && p.bn_dbeta != nullptr));
+    const bool do_red = conv_reduces(p);
     const bool pass2 = do_red || aux_mode != 0;
-    // per-channel reductions are kept in registers (threads wtid < OUT_CW, one channel per chunk) across all tiles of
+    // per-channel reductions are kept in registers (threads wtid < CW, one channel per chunk) across all tiles of
     // this CTA that share an N tile, and added to this CTA's row when the N tile changes / at the end
     float racc1[OUT_CHUNKS], racc2[OUT_CHUNKS];
 #pragma unroll
@@ -307,13 +340,10 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
       t2 += (chunk2 / OUT_CHUNKS) * (int)gridDim.x;
       chunk2 %= OUT_CHUNKS;
       if (t2 >= total_tiles) return;
-      const int ph2 = t2 % p.phases;
-      const int mt2 = (t2 / p.phases) % p.m_tiles;
-      const int nt2 = t2 / (p.phases * p.m_tiles);
-      const int tx2 = mt2 % p.tiles_x, ty2 = (mt2 / p.tiles_x) % p.tiles_y, tn2 = mt2 / (p.tiles_x * p.tiles_y);
-      tc::mbar_expect_tx(&aux_full_bar[slot], (uint32_t)p.rows * OUT_ROW_BYTES);
-      tc::tma_load_4d(aux_stage + (size_t)slot * OUT_CHUNK_BYTES, &p.tmX[ph2], &aux_full_bar[slot],
-                      p.n_off + nt2 * BN + chunk2 * OUT_CW, tx2 * p.bw, ty2 * p.bh, tn2 * p.bn);
+      const ConvTile tile = conv_tile<BN>(p, t2);
+      tc::mbar_expect_tx(&aux_full_bar[slot], (uint32_t)p.rows * CW_ROW_BYTES);
+      tc::tma_load_4d(aux_stage + (size_t)slot * OUT_CHUNK_BYTES, &p.tmX[tile.phase], &aux_full_bar[slot],
+                      p.n_off + tile.ncol0 + chunk2 * CW, tile.x0, tile.y0, tile.n0);
     };
     if (aux_mode != 0 && wtid == 0) {
       issue_aux(blockIdx.x, 0, 0);
@@ -325,10 +355,10 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
     if (do_red)
       for (int i = wtid; i < p.red_stride; i += 128) red_row[i] = 0.f;
     auto flush_reductions = [&]() {
-      if (racc_nt >= 0 && wtid < OUT_CW) {
+      if (racc_nt >= 0 && wtid < CW) {
 #pragma unroll
         for (int j = 0; j < OUT_CHUNKS; ++j) {
-          const int ch = racc_nt * BN + j * OUT_CW + wtid;   // relative to p.n_off
+          const int ch = racc_nt * BN + j * CW + wtid;   // relative to p.n_off
           red_row[ch] += racc1[j];
           red_row[red_half + ch] += racc2[j];
           racc1[j] = racc2[j] = 0.f;
@@ -338,12 +368,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
 
     int it = 0;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++it) {
-      const int phase_id = t % p.phases;
-      const int mt = (t / p.phases) % p.m_tiles;
-      const int nt = t / (p.phases * p.m_tiles);
-      const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tn = mt / (p.tiles_x * p.tiles_y);
-      const int x0 = tx * p.bw, y0 = ty * p.bh, n0 = tn * p.bn;
-      const int ncol0 = nt * BN;
+      const auto [phase_id, nt, ncol0, x0, y0, n0] = conv_tile<BN>(p, t);
       // every row of the tile is a real output pixel (the common case): the second pass skips the per-row checks
       const bool tile_full = p.rows == 128 && x0 + p.bw <= p.Wv && y0 + p.bh <= p.Hv && n0 + p.bn <= p.Nimg;
       if (do_red && nt != racc_nt) {
@@ -373,7 +398,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
           if (aux_mode != 0) tc::mbar_wait(&aux_full_bar[aslot], (aux_q >> 1) & 1);
           const bool bnred = aux_mode == 2;
           const int cg = wtid % CGc, rg = wtid / CGc;
-          const int ch0 = p.n_off + ncol0 + chunk * OUT_CW + cg * 8;
+          const int ch0 = p.n_off + ncol0 + chunk * CW + cg * 8;
           float s1[8], s2[8], mu[8], is[8], sc[8], sh[8];
 #pragma unroll
           for (int j = 0; j < 8; ++j) s1[j] = s2[j] = mu[j] = is[j] = sc[j] = sh[j] = 0.f;
@@ -386,15 +411,15 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
               sh[j] = __ldg(p.bn_beta + ch0 + j) - mu[j] * sc[j];  // bn_train_coef (elementwise.cu)
             }
           }
-          // rows rg*ROWSc .. +ROWSc-1; the swizzle term of row r depends only on rr (OUT_CW 64: r & 7 == rr; 32:
+          // rows rg*ROWSc .. +ROWSc-1; the swizzle term of row r depends only on rr (CW 64: r & 7 == rr; 32:
           // (r >> 1) & 3 == ((rg & 1) * 2 + (rr >> 1))), so every offset is base + compile-time pieces
-          const uint32_t row0_off = (uint32_t)(rg * ROWSc) * OUT_ROW_BYTES;
-          const int swz_rg = (OUT_CW == 64) ? 0 : (rg & 1) * 2;
+          const uint32_t row0_off = (uint32_t)(rg * ROWSc) * CW_ROW_BYTES;
+          const int swz_rg = (CW == 64) ? 0 : (rg & 1) * 2;
 #pragma unroll
           for (int rr = 0; rr < ROWSc; ++rr) {
             if (!tile_full && !row_ok[rg * ROWSc + rr]) continue;   // ragged tiles only
-            const int unit = (OUT_CW == 64) ? (cg ^ rr) : (cg ^ (swz_rg + (rr >> 1)));
-            const uint32_t off = row0_off + (uint32_t)rr * OUT_ROW_BYTES + (uint32_t)unit * 16;
+            const int unit = (CW == 64) ? (cg ^ rr) : (cg ^ (swz_rg + (rr >> 1)));
+            const uint32_t off = row0_off + (uint32_t)rr * CW_ROW_BYTES + (uint32_t)unit * 16;
             const uint4 pk = *reinterpret_cast<const uint4*>(cbuf + off);
             const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&pk);
             if (aux_mode == 0) {
@@ -460,7 +485,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
             }
           }
           epi_wg_sync();   // the table is complete, and every thread is done with the chunk and its aux buffer
-          if (do_red && wtid < OUT_CW) {
+          if (do_red && wtid < CW) {
             float a1 = 0.f, a2 = 0.f;
 #pragma unroll
             for (int w4 = 0; w4 < 4; ++w4) {
@@ -476,8 +501,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
 
         if (wtid == 0) {
           const CUtensorMap* mD = &p.tmD[phase_id];
-          if (p.accumulate) tc::tma_reduce_add_4d(mD, cbuf, p.n_off + ncol0 + chunk * OUT_CW, x0, y0, n0);
-          else tc::tma_store_4d(mD, cbuf, p.n_off + ncol0 + chunk * OUT_CW, x0, y0, n0);
+          if (p.accumulate) tc::tma_reduce_add_4d(mD, cbuf, p.n_off + ncol0 + chunk * CW, x0, y0, n0);
+          else tc::tma_store_4d(mD, cbuf, p.n_off + ncol0 + chunk * CW, x0, y0, n0);
           if (aux_mode != 0) issue_aux(t, chunk + 2, aslot);   // the aux buffer just processed is free
         }
         ++aux_q;
@@ -502,11 +527,10 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
 #pragma unroll
   for (int i = 0; i < ACC; ++i) acc[i] = 0.f;
   uint32_t ag = 0;
-  int ring_s = 0;
-  uint32_t ring_ph = 0;
+  tc::RingPos ring;
   int it = 0;
   for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++it) {
-    const int phase_id = t % p.phases;
+    const auto [phase_id, nt, ncol0, x0, y0, n0] = conv_tile<BN>(p, t);
     const int tap_begin = p.tap_start[phase_id], tap_end = tap_begin + p.tap_count[phase_id];
     // ---------------------------------------------------- main loop: one wgmma group per ring slot; the slot (and, in
     // HALO mode, the A tile after its ninth tap) is released once the NEXT group is issued and this one has completed
@@ -523,7 +547,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k) {
           const uint64_t da = da0 + (uint64_t)((k * 32) >> 4);
-          const uint64_t db = B_MN ? db0 + (uint64_t)((k * 16 * BMN_ROW_BYTES) >> 4) : db0 + (uint64_t)((k * 32) >> 4);
+          const uint64_t db = B_MN ? db0 + (uint64_t)((k * 16 * CW_ROW_BYTES) >> 4) : db0 + (uint64_t)((k * 32) >> 4);
           if constexpr (BN == 256) {
             // two n = 128 halves: in a 512-thread CTA no instruction may need more than 128 registers, and one
             // m64n256 wgmma holds 128 accumulators plus its operands.  Same accumulator layout, same K order.
@@ -540,7 +564,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
         release_prev();
       };
       auto b_desc = [&](uint32_t sb) {
-        return B_MN ? tc::make_smem_desc(sb, BMN_SUB_BYTES, 8 * BMN_ROW_BYTES, BMN_LAYOUT)
+        return B_MN ? tc::make_smem_desc(sb, BMN_SUB_BYTES, 8 * CW_ROW_BYTES, CW_LAYOUT)
                     : tc::make_smem_desc(sb, 16, 8 * A_ROW_BYTES, A_LAYOUT);
       };
       if (HALO) {
@@ -555,14 +579,12 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
             const uint32_t a_base = tc::smem_u32(a_ring + (size_t)as * A_BYTES) + (uint32_t)(wg * 8 * kHaloW * A_ROW_BYTES);
             for (int tt = 0; tt < 9; ++tt, ++i) {
               const TapDesc tap = p.taps[tap_begin + tt * nsrc + sidx];
-              const int s = ring_s;
-              const uint32_t ph = ring_ph;
-              if (++ring_s == stages) { ring_s = 0; ring_ph ^= 1; }
-              tc::mbar_wait(&full_bar[s], ph);
+              const tc::RingPos r = ring.step(stages);
+              tc::mbar_wait(&full_bar[r.slot], r.parity);
               const uint32_t sa = a_base + (uint32_t)(((1 + tap.dy) * kHaloW + (1 + tap.dx)) * A_ROW_BYTES);
               mma_block(tc::make_smem_desc(sa, 16, kHaloW * A_ROW_BYTES, A_LAYOUT),
-                        b_desc(tc::smem_u32(smem + (size_t)s * STAGE_BYTES)), i == 0);
-              prev_s = s;
+                        b_desc(tc::smem_u32(smem + (size_t)r.slot * STAGE_BYTES)), i == 0);
+              prev_s = r.slot;
               prev_as = (tt == 8) ? as : -1;
             }
           }
@@ -571,14 +593,12 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
         int num_kb = 0;
         for (int tp = tap_begin; tp < tap_end; ++tp) num_kb += p.taps[tp].nchunks;
         for (int i = 0; i < num_kb; ++i) {
-          const int s = ring_s;
-          const uint32_t ph = ring_ph;
-          if (++ring_s == stages) { ring_s = 0; ring_ph ^= 1; }
-          tc::mbar_wait(&full_bar[s], ph);
-          const uint32_t sa = tc::smem_u32(smem + (size_t)s * STAGE_BYTES);
+          const tc::RingPos r = ring.step(stages);
+          tc::mbar_wait(&full_bar[r.slot], r.parity);
+          const uint32_t sa = tc::smem_u32(smem + (size_t)r.slot * STAGE_BYTES);
           mma_block(tc::make_smem_desc(sa + (uint32_t)(wg * 64 * A_ROW_BYTES), 16, 8 * A_ROW_BYTES, A_LAYOUT),
                     b_desc(sa + A_BYTES), i == 0);
-          prev_s = s;
+          prev_s = r.slot;
         }
       }
       tc::wgmma_wait<0>();
@@ -587,11 +607,6 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
     }
 
     // ---------------------------------------------------- pass 1
-    const int mt = (t / p.phases) % p.m_tiles;
-    const int nt = t / (p.phases * p.m_tiles);
-    const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, tn = mt / (p.tiles_x * p.tiles_y);
-    const int x0 = tx * p.bw, y0 = ty * p.bh, n0 = tn * p.bn;
-    const int ncol0 = nt * BN;
     // staging buffer of this tile: the TMA stores of the tile that used it before (out_bufs tiles ago) have read it
     const int b = it % out_bufs;
     tc::mbar_wait(&drained_bar[b], ((uint32_t)(it / out_bufs) & 1) ^ 1);
@@ -610,8 +625,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
           rrow = p.residual + (size_t)((on * p.mask_H + fy) * p.mask_W + fx) * p.mask_C + p.n_off + ncol0;
         }
       }
-      uint8_t* rowp = obuf + (size_t)row * OUT_ROW_BYTES;
-      const int swz = (OUT_CW == 64) ? (row & 7) : ((row >> 1) & 3);   // SWIZZLE_128B / SWIZZLE_64B
+      uint8_t* rowp = obuf + (size_t)row * CW_ROW_BYTES;
+      const int swz = (CW == 64) ? (row & 7) : ((row >> 1) & 3);   // SWIZZLE_128B / SWIZZLE_64B
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         const int col = 8 * j + 2 * (lane & 3);
@@ -629,7 +644,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
           v0 += rv.x; v1 += rv.y;
         }
         if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-        constexpr int UNITS = OUT_CW / 8;   // 16-byte units per staged row
+        constexpr int UNITS = CW / 8;   // 16-byte units per staged row
         const int chunk = j / UNITS, unit = (j % UNITS) ^ swz;
         *reinterpret_cast<uint32_t*>(rowp + (size_t)chunk * OUT_CHUNK_BYTES + unit * 16 + 4 * (lane & 3)) =
             tc::pack_bf16x2(v0, v1);
@@ -646,20 +661,20 @@ template <int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1) wgrad_kernel(const __grid_constant__ WgradParams p) {
   static_assert(BN == 32 || BN == 64 || BN == 128 || BN == 256, "BN");
   constexpr int KROWS = 64;                       // max pixel rows per K block
-  constexpr int B_CW = (BN >= 64) ? 64 : 32;      // channels per B sub-tile row
+  constexpr int B_CW = chunk_width(BN);           // channels per B sub-tile row
   constexpr int B_ROW_BYTES = B_CW * 2;
   constexpr int B_SUB_BYTES = KROWS * B_ROW_BYTES;
   constexpr int B_SUBS = BN / B_CW;
-  constexpr int B_BYTES = B_SUBS * B_SUB_BYTES;
   constexpr uint32_t B_LAYOUT = (B_CW == 64) ? tc::LAYOUT_SW128 : tc::LAYOUT_SW64;
   constexpr int A_SUB_BYTES = KROWS * 128;        // sized for the 64-channel case
   constexpr int A_BYTES = 2 * A_SUB_BYTES;
-  constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  constexpr int STAGE_BYTES = wgrad_smem(BN, 0).stage;
+  static_assert(STAGE_BYTES == A_BYTES + B_SUBS * B_SUB_BYTES, "wgrad_smem's ring slot");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_up_1024(smem_raw);
   const int stages = p.stages;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)stages * STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + wgrad_smem(BN, stages).bars);
   uint64_t* empty_bar = full_bar + stages;
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);  // provably warp-uniform
@@ -695,28 +710,25 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgrad_kernel(const __grid_con
     const CUtensorMap* mA = &p.tmA[tap.srcA];
     const CUtensorMap* mB = &p.tmB[tap.srcB];
     const uint32_t tx_bytes = (uint32_t)p.rows * (uint32_t)(a_row_bytes * p.a_chunks + B_ROW_BYTES * B_SUBS);
-    int ring_s = 0;
-    uint32_t ring_ph = 0;
+    tc::RingPos ring;
     // pixel-tile coordinates advance incrementally (no integer division inside the single-thread issue loop)
     int tx = kb_begin % p.tiles_x;
     int ty = (kb_begin / p.tiles_x) % p.tiles_y;
     int tn = kb_begin / (p.tiles_x * p.tiles_y);
     for (int i = 0; i < num_kb; ++i) {
-      const int s = ring_s;
-      const uint32_t ph = ring_ph;
-      if (++ring_s == stages) { ring_s = 0; ring_ph ^= 1; }
+      const tc::RingPos r = ring.step(stages);
       const int x0 = tx * p.bw, y0 = ty * p.bh, n0 = tn * p.bn;
       if (++tx == p.tiles_x) { tx = 0; if (++ty == p.tiles_y) { ty = 0; ++tn; } }
-      tc::mbar_wait(&empty_bar[s], ph ^ 1);
-      uint8_t* sa = smem + (size_t)s * STAGE_BYTES;
-      uint8_t* sb = sa + A_BYTES;
+      tc::mbar_wait(&empty_bar[r.slot], r.parity ^ 1);
+      uint8_t* sa = smem + (size_t)r.slot * STAGE_BYTES;
+      uint64_t* bar = &full_bar[r.slot];
       if (tc::elect_one()) {
-        tc::mbar_expect_tx(&full_bar[s], tx_bytes);
+        tc::mbar_expect_tx(bar, tx_bytes);
         for (int j = 0; j < p.a_chunks; ++j)
-          tc::tma_load_4d(sa + j * A_SUB_BYTES, mA, &full_bar[s], m0 + j * p.a_cw, x0 + tap.ax, y0 + tap.ay, n0);
+          tc::tma_load_4d(sa + j * A_SUB_BYTES, mA, bar, m0 + j * p.a_cw, x0 + tap.ax, y0 + tap.ay, n0);
 #pragma unroll
         for (int j = 0; j < B_SUBS; ++j)
-          tc::tma_load_4d(sb + j * B_SUB_BYTES, mB, &full_bar[s], ncol0 + j * B_CW, x0 + tap.bx, y0 + tap.by, n0);
+          tc::tma_load_4d(sa + A_BYTES + j * B_SUB_BYTES, mB, bar, ncol0 + j * B_CW, x0 + tap.bx, y0 + tap.by, n0);
       }
     }
     return;
@@ -733,15 +745,12 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgrad_kernel(const __grid_con
   float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  int ring_s = 0;
-  uint32_t ring_ph = 0;
+  tc::RingPos ring;
   int prev_s = -1;
   for (int i = 0; i < num_kb; ++i) {
-    const int s = ring_s;
-    const uint32_t ph = ring_ph;
-    if (++ring_s == stages) { ring_s = 0; ring_ph ^= 1; }
-    tc::mbar_wait(&full_bar[s], ph);
-    const uint32_t sa = tc::smem_u32(smem + (size_t)s * STAGE_BYTES);
+    const tc::RingPos r = ring.step(stages);
+    tc::mbar_wait(&full_bar[r.slot], r.parity);
+    const uint32_t sa = tc::smem_u32(smem + (size_t)r.slot * STAGE_BYTES);
     const uint32_t sb = sa + A_BYTES;
     const uint64_t da0 = tc::make_smem_desc(sa + a_off, A_SUB_BYTES, 8 * a_row_bytes, a_layout);
     const uint64_t db0 = tc::make_smem_desc(sb, B_SUB_BYTES, 8 * B_ROW_BYTES, B_LAYOUT);
@@ -754,7 +763,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgrad_kernel(const __grid_con
     tc::wgmma_commit();
     tc::wgmma_wait<1>();
     if (prev_s >= 0 && wtid == 0) tc::mbar_arrive(&empty_bar[prev_s]);
-    prev_s = s;
+    prev_s = r.slot;
   }
   tc::wgmma_wait<0>();
   tc::fence_acc(acc);

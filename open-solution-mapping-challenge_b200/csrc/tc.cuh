@@ -52,6 +52,18 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
 }
+// Position in a ring of mbarrier-guarded slots: slot and phase parity, advanced without integer division (a
+// single-thread producer loop is a latency chain, every instruction in it is exposed).  Consumers wait on full[slot]
+// with `parity`, the producer on empty[slot] with `parity ^ 1`.
+struct RingPos {
+  int slot = 0;
+  uint32_t parity = 0;
+  __device__ __forceinline__ RingPos step(int n) {  // returns this position, moves on to the next of an n-slot ring
+    const RingPos cur = *this;
+    if (++slot == n) { slot = 0; parity ^= 1; }
+    return cur;
+  }
+};
 
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
@@ -92,12 +104,6 @@ __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk
 __device__ __forceinline__ void tma_store_wait_read0() {
   asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
-// at most N bulk-store groups of this thread may still be reading shared memory
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void tma_store_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // make generic-proxy smem writes visible to the async proxy (TMA store reads smem through it)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
