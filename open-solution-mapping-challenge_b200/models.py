@@ -547,15 +547,16 @@ class FusedTrainStep:
         return finish_target
 
     def step(self, X, target, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0):
-        finish_target = self._stage_inputs(X, target)
-        self.opt.t += 1
-        t = self.opt.t
         if self.adam_in_graph:
             cfg = (tuple(betas), eps, weight_decay)
             if self._adam_cfg is None:
                 self._adam_cfg = cfg
-            elif self._adam_cfg != cfg:   # baked into the captured launches
+            elif self._adam_cfg != cfg:   # baked into the captured launches; refused before the step counts
                 raise RuntimeError("Adam betas / eps / weight_decay changed after the train step was captured")
+        finish_target = self._stage_inputs(X, target)
+        self.opt.t += 1
+        t = self.opt.t
+        if self.adam_in_graph:
             host, ev = self._hyper_ring[t % len(self._hyper_ring)]
             ev.synchronize()
             host[0], host[1], host[2] = ops.adam_hyper(lr, betas, t)

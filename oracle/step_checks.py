@@ -1,7 +1,8 @@
 """TEST INFRASTRUCTURE -- the harness of the train-step tests at the benchmarks' sizes
 (tests/test_train_step_scale_gpu.py, tests/test_train_step_vgg_scale_gpu.py, tests/test_train_step_resnet_units_gpu.py
-at batch 32 and 320x320, tests/test_train_step_config5_gpu.py at BASELINE.json config 5's batch 16 and 512x512), and
-the helpers the golden-fixture encoder tests share.  Never imported by the product path.
+at batch 32 and 320x320, tests/test_train_step_config5_gpu.py at BASELINE.json config 5's batch 16 and 512x512,
+tests/test_train_step_ragged_batch_gpu.py at batch 20 and partial batches, tests/test_train_run_lifecycle_gpu.py across
+a training run's callbacks), and the helpers the golden-fixture encoder tests share.  Never imported by the product path.
 
 BenchStep is the train step the benchmarks time, for every encoder family they run, at batch n and sxs (N and S, the
 default, are bench.py's): the ResNets through PyTorchUNetWeighted._fit_loop as bench.py builds it, VGG11 and VGG16
@@ -102,22 +103,37 @@ class BenchStep:
             self.fused = model._fused_step(self.net, shape, shape, model._loss_spec())
 
     def step(self, X, T):
-        """one train step as the benchmark runs it -> the loss, shape (1,)"""
+        """one train step as the benchmark runs it -> the loss, shape (1,).  For the ResNets, fused follows the batch
+        shape: it is the captured step _fit_loop ran"""
         if self.model is not None:
-            return self.model._fit_loop([X, T])["sum"]
+            loss = self.model._fit_loop([X, T])["sum"]
+            self.fused = self.model._fused
+            return loss
         lr, betas, eps, wd = self.adam
         return self.fused.step(X, T, lr=lr, betas=betas, eps=eps, weight_decay=wd)
+
+    def is_replay(self, X, T):
+        """whether the next step on (X, T) replays captured graphs (the first step of a shape runs eagerly)"""
+        f = self.fused if self.model is None else self.model._fused_cache.get((tuple(X.shape), tuple(T.shape)))
+        return f is not None and f.graphs is not None
+
+    def lr(self):
+        """the learning rate the next step hands Adam: the optimizer's, which a scheduler may change between steps"""
+        return self.adam[0] if self.model is None else self.model.optimizer.param_groups[0]["lr"]
 
     def serial_steps(self, batches):
         """the fused step's own segments, run eagerly in program order on the current stream, with the Adam scalars
         FusedTrainStep.step sets: the side stream is the main stream, so the weight-gradient GEMMs and the per-segment
         Adam hooks run exactly where they are issued.  Program order is a valid topological order of the step, so this
-        is the schedule-free result of the same launches.  Yields the loss of every step."""
+        is the schedule-free result of the same launches.  For the ResNets a batch of another shape runs the captured
+        step _fit_loop keeps for that shape, sharing the one Adam state.  Yields the loss of every step."""
         from mcb200 import ops
-        fused = self.fused
         lr, betas, eps, wd = self.adam
-        fused.plan._side = torch.cuda.current_stream()
         for X, T in batches:
+            if self.model is not None:
+                self.fused = self.model._fused_step(self.net, X.shape, T.shape, self.model._loss_spec())
+            fused = self.fused
+            fused.plan._side = torch.cuda.current_stream()
             fused.opt.t += 1
             fused._adam_cfg = (betas, eps, wd)
             fused._hyper.copy_(torch.tensor(ops.adam_hyper(lr, betas, fused.opt.t), dtype=torch.float32))
@@ -235,30 +251,73 @@ def check_captured_equals_serial(enc, cuda, n=N, s=S):
     free_device_memory()
 
 
-def check_adam_of_own_gradients(enc, cuda, n=N, s=S):
-    """three steps (eager, then graph replays): each step's fp32 weights and Adam moments exactly whole-arena Adam of
-    that step's own final gradients, and the bf16 operand copy exactly the new fp32 weights"""
+def adam_mismatches(run, layout, X, T):
+    """one run.step on (X, T), then every difference between what it left and whole-arena Adam (ops.adam_step) of the
+    step's own final gradients from the pre-step p32, m and v, with the learning rate the optimizer held when the step
+    ran and the step count t it ran at: p32, m, v, the bf16 operand copy, and the operand copy against bf16(p32).
+    -> (loss, list of differences)"""
     from mcb200 import ops
-    run = BenchStep(enc, seeded_sd(enc), cuda, n, s)
-    net, opt = run.net, run.fused.opt
-    layout = arena_layout(net)
-    lr, betas, eps, wd = run.adam
-    for i in range(3):
-        X, T = (t.to(cuda) for t in batch(SEED + 10 + i, n, s))
-        p, m, v = net._p32.clone(), opt.m.clone(), opt.v.clone()
-        run.step(X, T)
-        assert opt.t == i + 1
-        assert bool(net._g32.any()) and not same_bits(p, net._p32), "the step must compute gradients and move weights"
-        w16 = torch.zeros_like(net._w16)
-        ops.adam_step(p, net._g32, m, v, w16, opt.t, lr, betas, eps, wd, 1.0)
-        bad = ["%s: first differing tensor %s" % (k, d) for k, d in
-               (("p32", arena_mismatch(layout, net._p32, p)), ("m", arena_mismatch(layout, opt.m, m)),
-                ("v", arena_mismatch(layout, opt.v, v)), ("w16", arena_mismatch(layout, net._w16, w16)),
-                ("w16 against bf16(p32)", arena_mismatch(layout, net._w16, net._p32.to(torch.bfloat16)))) if d]
-        print("%s step %d: fused Adam == whole-arena Adam of the step's gradients: %s" % (enc, i + 1, not bad))
-        assert not bad, "%s step %d (%s): %s" % (enc, i + 1, "eager" if i == 0 else "graph replay", "; ".join(bad))
-        del p, m, v, w16
-    del run, net, opt
+    net = run.net
+    opt = run.fused.opt
+    _, betas, eps, wd = run.adam
+    lr, t = run.lr(), opt.t + 1
+    p, m, v = net._p32.clone(), opt.m.clone(), opt.v.clone()
+    loss = run.step(X, T)
+    opt = run.fused.opt
+    assert opt.t == t, "the step must count once: t %d, expected %d" % (opt.t, t)
+    assert bool(net._g32.any()) and not same_bits(p, net._p32), "the step must compute gradients and move weights"
+    w16 = torch.zeros_like(net._w16)
+    ops.adam_step(p, net._g32, m, v, w16, t, lr, betas, eps, wd, 1.0)
+    bad = ["%s: first differing tensor %s" % (k, d) for k, d in
+           (("p32", arena_mismatch(layout, net._p32, p)), ("m", arena_mismatch(layout, opt.m, m)),
+            ("v", arena_mismatch(layout, opt.v, v)), ("w16", arena_mismatch(layout, net._w16, w16)),
+            ("w16 against bf16(p32)", arena_mismatch(layout, net._w16, net._p32.to(torch.bfloat16)))) if d]
+    del p, m, v, w16
+    return loss, bad
+
+
+def check_adam_of_own_gradients(enc, cuda, n=N, s=S, sizes=None):
+    """steps of batch sizes `sizes` (default three of n; eager, then graph replays): each step's fp32 weights and Adam
+    moments exactly whole-arena Adam of that step's own final gradients at the t it ran at, and the bf16 operand copy
+    exactly the new fp32 weights.
+
+    When `sizes` switches between batch shapes (the ResNets only: a full batch and an epoch's partial last batch through
+    _fit_loop), two captured steps are alive and share one Adam state, and every step also equals, bit for bit, the same
+    sequence of batches run in program order (BenchStep.serial_steps) on a fresh net: a replay of the full-batch step
+    after a tail step equals a serial run of the same sequence, so neither captured step keeps state of its own that the
+    other one's steps make stale."""
+    sizes = [n] * 3 if sizes is None else list(sizes)
+    switch = len(set(sizes)) > 1
+    sd = seeded_sd(enc)
+    batches = [tuple(t.to(cuda) for t in batch(SEED + 10 + i, k, s)) for i, k in enumerate(sizes)]
+    run = BenchStep(enc, sd, cuda, sizes[0], s)
+    layout = arena_layout(run.net)
+    seen, snaps = set(), []
+    for i, (X, T) in enumerate(batches):
+        replay = run.is_replay(X, T)
+        loss, bad = adam_mismatches(run, layout, X, T)
+        assert run.fused.opt.t == i + 1, "step %d ran at t %d" % (i + 1, run.fused.opt.t)
+        seen.add(id(run.fused))
+        print("%s step %d (batch %d, %s): fused Adam == whole-arena Adam of the step's gradients: %s" % (
+            enc, i + 1, sizes[i], "graph replay" if replay else "eager", not bad))
+        assert not bad, "%s step %d (batch %d, %s): %s" % (enc, i + 1, sizes[i], "graph replay" if replay else "eager",
+                                                          "; ".join(bad))
+        if switch:
+            snaps.append(snapshot(run, loss))
+    if switch:
+        assert len(seen) == len(set(sizes)) and len(run.model._fused_cache) == len(set(sizes))
+        assert all(f.opt is run.model._opt_state for f in run.model._fused_cache.values()), "one Adam state"
+    del run
+    free_device_memory()
+    if not switch:
+        return
+    run = BenchStep(enc, sd, cuda, sizes[0], s)
+    for i, loss in enumerate(run.serial_steps(batches)):
+        bad = snapshot_mismatches(layout, snaps[i], snapshot(run, loss))
+        print("%s step %d (batch %d): captured == serial: %s" % (enc, i + 1, sizes[i], not bad))
+        assert not bad, "%s step %d (batch %d): %s" % (enc, i + 1, sizes[i], "; ".join(bad))
+    assert run.fused.opt.t == len(sizes)
+    del run, snaps
     free_device_memory()
 
 
