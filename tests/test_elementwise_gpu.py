@@ -11,21 +11,10 @@ import torch.nn.functional as F
 
 from oracle import synthetic
 from oracle import unet_oracle as O
+from oracle.conv_checks import bf16r, nchw, nhwc
 
 pytestmark = pytest.mark.gpu
 BF = torch.bfloat16
-
-
-def nhwc(x):
-    return x.permute(0, 2, 3, 1).contiguous()
-
-
-def nchw(x):
-    return x.permute(0, 3, 1, 2).contiguous()
-
-
-def bf16r(x):
-    return x.to(BF).float()
 
 
 def close(got, ref, rtol=2 ** -7, atol=1e-3):
