@@ -463,6 +463,10 @@ int mcb_sync_exchange(const float* partial, void* const* peer_recv, int rank, in
 int mcb_rle_pair_iou(const uint32_t* dt_cnts, const long long* dt_starts, const uint32_t* gt_cnts,
                      const long long* gt_starts, const uint8_t* gt_crowd, const int* pair_dt, const int* pair_gt,
                      const long long* pair_out, double* iou, int npairs, void* stream);
+/* get_iou over get_iou_matrix (src/postprocessing.py:306-328): out[r] = max of iou[row_off[r], row_off[r + 1]) (fp64),
+ * NaN for an empty row (no ground truth of the instance's image and category: the reference's `None`).
+ * row_off int64 [rows + 1].  One thread per row. */
+int mcb_iou_row_max(const double* iou, const long long* row_off, int rows, double* out, void* stream);
 /* COCOeval.evaluateImg (src/cocoeval.py:242-320) for every (unit, area range); a unit is one (image, category) with
  * nd[u] detections (score-ordered, already cut to maxDets[-1]) at dt_off[u] and ng[u] ground truths (file order) at
  * gt_off[u]; its IoU table is iou[iou_off[u] + d * ng[u] + g].  dt_id int64, dt_area fp64; gt_id int64, gt_crowd uint8

@@ -205,6 +205,7 @@ for _n, _a in _SIGS5.items():
 
 _SIGS6 = {
     "mcb_rle_pair_iou": [vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, vp],
+    "mcb_iou_row_max": [vp, vp, ci, vp, vp],
     "mcb_coco_match": [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, C.c_longlong, C.c_longlong, vp,
                        vp, vp, vp, vp],
 }

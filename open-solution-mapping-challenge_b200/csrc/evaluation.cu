@@ -116,6 +116,20 @@ __global__ void coco_match_kernel(const double* __restrict__ iou, const long lon
   }
 }
 
+// ------------------------------------------------------------------------------------------ get_iou
+// Row r of a ragged IoU table (one instance against the ground truths of its image and category) reduces to its
+// maximum, NaN for a row without ground truths (the reference's `None`).  One thread per row: rows are a few dozen
+// entries, and the maximum of non-NaN values does not depend on the visiting order.
+__global__ void iou_row_max_kernel(const double* __restrict__ iou, const long long* __restrict__ row_off, int rows,
+                                   double* __restrict__ out) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  const long long b = row_off[r], e = row_off[r + 1];
+  double m = b < e ? iou[b] : __longlong_as_double(0x7FF8000000000000LL);
+  for (long long j = b + 1; j < e; ++j) m = fmax(m, iou[j]);
+  out[r] = m;
+}
+
 }  // namespace mcb
 
 using namespace mcb;
@@ -129,6 +143,15 @@ extern "C" int mcb_rle_pair_iou(const uint32_t* dt_cnts, const long long* dt_sta
               "rle_pair_iou: null pointer");
   rle_pair_iou_kernel<<<(npairs + 127) / 128, 128, 0, ST>>>(dt_cnts, dt_starts, gt_cnts, gt_starts, gt_crowd, pair_dt,
                                                             pair_gt, pair_out, iou, npairs);
+  MCB_LAUNCH_CHECK();
+  return MCB_OK;
+}
+
+extern "C" int mcb_iou_row_max(const double* iou, const long long* row_off, int rows, double* out, void* stream) {
+  MCB_REQUIRE(rows >= 0, "iou_row_max: negative row count %d", rows);
+  if (rows == 0) return MCB_OK;
+  MCB_REQUIRE(iou && row_off && out, "iou_row_max: null pointer");
+  iou_row_max_kernel<<<(rows + 127) / 128, 128, 0, ST>>>(iou, row_off, rows, out);
   MCB_LAUNCH_CHECK();
   return MCB_OK;
 }

@@ -9,14 +9,36 @@ Two surfaces:
 
 All arithmetic is in libmcb200.so (csrc/postproc.cu); torch only owns the device buffers.  No CPU fallback.
 """
+import importlib.util
+import itertools
+import warnings
+
 import numpy as np
 import torch
 
 from . import _lib as L
 
 CATEGORY_LAYERS = [1, 1]  # src/pipeline_config.py:18
+CATEGORY_IDS = [None, 100]  # src/pipeline_config.py:17
 MEAN = [0.485, 0.456, 0.406]
 STD = [0.229, 0.224, 0.225]
+
+
+def category_config():
+    """(CATEGORY_LAYERS, CATEGORY_IDS) of the reference's src/pipeline_config.py when the reference package is
+    importable, else this module's [1, 1] / [None, 100].  Read on every call: the scoring workflow edits the reference
+    config to [1, 19] (one background layer, 19 building thresholds 0.05 ... 0.95) and the per-image functions,
+    get_thresholds, instance_features and FeatureExtractor follow it as the reference's own module does."""
+    if importlib.util.find_spec("src") is None:      # no reference package on the path: the defaults
+        return list(CATEGORY_LAYERS), list(CATEGORY_IDS)
+    try:
+        from src import pipeline_config as pc
+        return list(pc.CATEGORY_LAYERS), list(pc.CATEGORY_IDS)
+    except Exception as e:  # a `src` package whose pipeline_config does not import
+        warnings.warn("mcb200: a `src` package is importable but src.pipeline_config is not (%s: %s); using "
+                      "CATEGORY_LAYERS %s and CATEGORY_IDS %s" % (type(e).__name__, e, CATEGORY_LAYERS, CATEGORY_IDS),
+                      RuntimeWarning, stacklevel=2)
+        return list(CATEGORY_LAYERS), list(CATEGORY_IDS)
 
 
 def _dev():
@@ -33,7 +55,7 @@ def _to_dev(a, dtype):
 
 def layer_thresholds(category_layers=None):
     """threshold list and source channel of every output layer (src/postprocessing.py:77-84)"""
-    category_layers = CATEGORY_LAYERS if category_layers is None else category_layers
+    category_layers = category_config()[0] if category_layers is None else category_layers
     thr, chan = [], []
     for c, n_layers in enumerate(category_layers):
         step = 1. / (n_layers + 1)
@@ -65,7 +87,7 @@ def threshold_batch(probs, category_layers=None):
     assert probs.is_cuda and probs.is_contiguous() and probs.dtype in (torch.float32, torch.float64)
     n, c, h, w = probs.shape
     thr, chan = layer_thresholds(category_layers)
-    assert len(category_layers or CATEGORY_LAYERS) <= c or max(chan) < c
+    assert max(chan) < c
     key = (probs.device, tuple(thr), tuple(chan))
     if key not in _THRESHOLD_CONSTS:   # tiny device constants, created once (and never inside a graph capture)
         _THRESHOLD_CONSTS[key] = (torch.tensor(thr, dtype=torch.float64, device=probs.device),
@@ -383,49 +405,330 @@ class NonMaximumSupression:
 
 
 def get_thresholds(category_layers=None):
-    """src/postprocessing.py:321-327"""
+    """src/postprocessing.py:331-337"""
     return layer_thresholds(category_layers)[0]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# second-level scoring: instance features and the ground-truth IoU target (src/postprocessing.py:18-33, 261-337)
+# ---------------------------------------------------------------------------------------------------------------------
+FEATURE_COLUMNS = ('iou', 'threshold', 'area', 'mean_prob', 'max_prob', 'bbox_ar', 'bbox_area', 'bbox_fill',
+                   'min_dist_to_border', 'max_dist_to_border', 'contour_length')
+
+
+def _starts(lengths):
+    return np.concatenate([[0], np.cumsum(np.asarray(lengths, np.int64))]).astype(np.int64)
+
+
+def ground_truth_runs(annotation_groups, height, width):
+    """the masks get_iou_matrix compares against (src/postprocessing.py:311-315), as COCO run lists: per annotation the
+    FIRST polygon of its segmentation only, `frPyObjects(segm, h, w)[0]`, rasterised on the device exactly as
+    pycocotools does; a segmentation that is already an RLE dict (compressed or uncompressed counts,
+    mcb200.evaluation.segmentation_counts) is used as is.  The caller's annotations are not modified.
+    annotation_groups: list of lists of COCO annotations -> (cnts uint32, starts int64 [G + 1], group offsets int64
+    [groups + 1]) on the host, annotations numbered group by group."""
+    from . import utils as U
+    from .evaluation import segmentation_counts
+    from .preparation import polygons_csr, rasterize_polygons, segmentation_polygons
+    h, w = int(height), int(width)
+    runs, polys, poly_slot = [], [], []
+    for anns in annotation_groups:
+        for ann in anns:
+            segm = ann['segmentation']
+            if isinstance(segm, dict):
+                c, size = segmentation_counts(segm, h, w)
+                if size != (h, w):
+                    raise ValueError("an RLE segmentation of size %s on a %d x %d label map" % (size, h, w))
+                runs.append(c.astype(np.uint32))
+            else:
+                polys.append(segmentation_polygons(segm)[0])
+                poly_slot.append(len(runs))
+                runs.append(None)
+    if polys:
+        planes = rasterize_polygons(*polygons_csr(polys), h, w).to(torch.int32)
+        cnts, starts, _, _ = U.rle_encode_instances(planes, torch.ones(len(polys), dtype=torch.int32,
+                                                                       device=planes.device))
+        for j, g in enumerate(poly_slot):
+            runs[g] = cnts[starts[j]:starts[j + 1]]
+    cnts = np.concatenate(runs).astype(np.uint32) if runs else np.zeros(0, np.uint32)
+    return cnts, _starts([len(r) for r in runs]), _starts([len(a) for a in annotation_groups])
+
+
+def pair_iou(dt_cnts, dt_starts, gt_cnts, gt_starts, pair_dt, pair_gt):
+    """cocomask.iou(dt, gt, [0] * len(gt)) entries of the listed (dt, gt) pairs: run lists on the host (uint32 counts,
+    int64 starts), pairs int arrays -> float64 cuda [pairs]"""
+    dev = _dev()
+    npairs = len(pair_dt)
+    iou = torch.empty(max(npairs, 1), dtype=torch.float64, device=dev)
+    if npairs:
+        t = [torch.from_numpy(np.ascontiguousarray(a)).to(dev) for a in (
+            np.asarray(dt_cnts, np.uint32).view(np.int32), np.asarray(dt_starts, np.int64),
+            np.asarray(gt_cnts, np.uint32).view(np.int32), np.asarray(gt_starts, np.int64),
+            np.zeros(max(len(gt_starts) - 1, 1), np.uint8), np.asarray(pair_dt, np.int32),
+            np.asarray(pair_gt, np.int32), np.arange(npairs, dtype=np.int64))]
+        L.fcall("mcb_rle_pair_iou", *[x.data_ptr() for x in t], iou.data_ptr(), int(npairs))
+    return iou[:npairs]
+
+
+def scoring_features_batch(labels, probs, annotations=None, category_layers=None, category_ids=None):
+    """get_features_for_image (src/postprocessing.py:261-303) for every layer of a batch in one device pass.
+    labels (N, L, H, W) int32 cuda (the dilated label maps), probs (N, C, H, W) float32|float64 cuda (the resized
+    probabilities), annotations: None or N dicts {category id: [COCO annotations]}.  Layer l reads channel c(l) of
+    CATEGORY_LAYERS; with annotations, an instance's `iou` is the max of cocomask.iou against its image's annotations
+    of CATEGORY_IDS[c(l)] (get_mask_with_iou / get_iou_matrix / get_iou), NaN where there are none (the reference's
+    None).  Read back once per batch -> dict of host arrays per instance slot (slot order = plane-major, label order)
+    plus 'counts' (instances per plane), 'has_gt' (per plane) and the shapes."""
+    from . import utils as U
+    layers, ids = category_config()
+    category_layers = layers if category_layers is None else list(category_layers)
+    category_ids = ids if category_ids is None else list(category_ids)
+    assert labels.is_cuda and labels.dtype == torch.int32 and labels.dim() == 4
+    assert probs.is_cuda and probs.dtype in (torch.float32, torch.float64) and probs.dim() == 4
+    n, nl, h, w = labels.shape
+    thr, chan = layer_thresholds(category_layers)
+    if nl != len(thr):
+        raise ValueError("%d label layers, but CATEGORY_LAYERS %s give %d" % (nl, category_layers, len(thr)))
+    if probs.shape[0] != n or tuple(probs.shape[2:]) != (h, w) or probs.shape[1] <= max(chan):
+        raise ValueError("probabilities %s do not pair with label maps %s" % (tuple(probs.shape), tuple(labels.shape)))
+    if annotations is not None and len(annotations) != n:
+        raise ValueError("%d annotation dicts for %d images" % (len(annotations), n))
+    planes = labels.reshape(n * nl, h, w).contiguous()
+    counts = planes.reshape(n * nl, -1).amax(dim=1).to(torch.int32) if n * nl else torch.zeros(0, dtype=torch.int32)
+    chan_d = torch.tensor(chan, dtype=torch.int64, device=labels.device)
+    pr = probs.contiguous().index_select(1, chan_d).reshape(n * nl, h, w)
+    geo = U.instance_geometry(planes, counts, pr)
+    total = int(geo["counts"].sum())
+    if total and (geo["area"] == 0).any():
+        s = int(np.flatnonzero(geo["area"] == 0)[0])
+        p = int(geo["plane"][s])
+        raise ValueError("label %d of layer %d of image %d is empty: get_bbox has no box for it"
+                         % (s - int(geo["offsets"][p]) + 1, p % nl, p // nl))
+    clen = torch.zeros(max(total, 1), dtype=torch.int32, device=labels.device)
+    if total:
+        L.fcall("mcb_contour_length", planes.data_ptr(), geo["_offsets"].data_ptr(), geo["_counts"].data_ptr(),
+                clen.data_ptr(), n * nl, h, w)
+    plane = geo["plane"].astype(np.int64)
+    n_cat = len(category_layers)
+    ng_group = np.zeros(n * n_cat, np.int64)
+    iou = np.full(total, np.nan)
+    if annotations is not None:
+        groups = [list(annotations[i].get(category_ids[c], []) or []) for i in range(n) for c in range(n_cat)]
+        gt_cnts, gt_starts, goff = ground_truth_runs(groups, h, w)
+        ng_group = np.diff(goff)
+        grp = (plane // nl) * n_cat + np.asarray(chan, np.int64)[plane % nl]
+        ng_slot = ng_group[grp]
+        row_off = _starts(ng_slot)
+        npairs = int(row_off[-1])
+        if npairs:
+            dt_cnts, dt_starts, _, _ = U.rle_encode_instances(planes, counts, geometry=geo)
+            local = np.arange(npairs, dtype=np.int64) - np.repeat(row_off[:-1], ng_slot)
+            pair_dt = np.repeat(np.arange(total, dtype=np.int64), ng_slot)
+            pair_gt = np.repeat(goff[grp], ng_slot) + local
+            iou_pairs = pair_iou(dt_cnts, dt_starts, gt_cnts, gt_starts, pair_dt, pair_gt)
+            best = torch.empty(total, dtype=torch.float64, device=labels.device)
+            row_off_d = torch.from_numpy(row_off).to(labels.device)
+            L.fcall("mcb_iou_row_max", iou_pairs.data_ptr(), row_off_d.data_ptr(), int(total), best.data_ptr())
+            iou = best.cpu().numpy()
+    has_gt = ng_group.reshape(n, n_cat)[:, chan].reshape(-1) > 0 if n * nl else np.zeros(0, bool)
+    return {"n": n, "layers": nl, "h": h, "w": w, "thresholds": thr, "counts": geo["counts"], "plane": plane,
+            "area": geo["area"].astype(np.int64), "rmin": geo["rmin"].astype(np.int64),
+            "rmax": geo["rmax"].astype(np.int64), "cmin": geo["cmin"].astype(np.int64),
+            "cmax": geo["cmax"].astype(np.int64), "psum": geo["psum"], "pmax": geo["pmax"],
+            "prob_dtype": np.float64 if probs.dtype == torch.float64 else np.float32,
+            "contour_length": clen[:total].cpu().numpy().astype(np.int64), "iou": iou, "has_gt": has_gt}
+
+
+def _feature_columns(t):
+    """the per-slot feature columns of a scoring_features_batch table, with get_features_for_mask's arithmetic"""
+    h, w = t["h"], t["w"]
+    area = t["area"]
+    r0, r1, c0, c1 = t["rmin"], t["rmax"] + 1, t["cmin"], t["cmax"] + 1
+    bh, bw = r1 - r0, c1 - c0
+    dists = np.stack([r0, h - r1, c0, w - c1])
+    with np.errstate(divide='ignore', invalid='ignore'):
+        mean = t["psum"] / area
+        # np.where(mask, probabilities, 0).max(): the zeros outside the mask take part
+        pmax = np.where(area < h * w, np.maximum(t["pmax"], 0.0), t["pmax"])
+        cols = {'area': area, 'mean_prob': mean, 'max_prob': pmax.astype(t["prob_dtype"]), 'bbox_ar': bh / bw,
+                'bbox_area': bw * bh, 'bbox_fill': area / (bw * bh), 'min_dist_to_border': dists.min(0),
+                'max_dist_to_border': dists.max(0), 'contour_length': t["contour_length"]}
+    return cols
+
+
+def feature_frames(table):
+    """scoring_features_batch table -> [[DataFrame per layer] per image] with get_features_for_image's columns, column
+    order and dtypes (float64 probabilities, which the pipelines feed, give the reference's dtypes exactly); a layer
+    without instances is an empty DataFrame, a layer without ground truth has an object `iou` column of None"""
+    import pandas as pd
+    cols = _feature_columns(table)
+    offs = _starts(table["counts"])
+    nl = table["layers"]
+    thresholds = [round(np.float64(t), 2) for t in table["thresholds"]]
+    out = []
+    for i in range(table["n"]):
+        image_features = []
+        for li in range(nl):
+            p = i * nl + li
+            a, b = int(offs[p]), int(offs[p + 1])
+            if a == b:
+                image_features.append(pd.DataFrame([]))
+                continue
+            iou = table["iou"][a:b] if table["has_gt"][p] else np.full(b - a, None, dtype=object)
+            d = {'iou': iou, 'threshold': np.full(b - a, thresholds[li], np.float64)}
+            d.update({k: v[a:b] for k, v in cols.items()})
+            image_features.append(pd.DataFrame(d, columns=list(FEATURE_COLUMNS)))
+        out.append(image_features)
+    return out
 
 
 def instance_features(labels, probabilities, category_layers=None):
     """get_features_for_image without ground truth (src/postprocessing.py:261-306): per layer a list of per-instance
     feature dicts {iou: None, threshold, area, mean_prob, max_prob, bbox_ar, bbox_area, bbox_fill, min_dist_to_border,
     max_dist_to_border, contour_length}.  labels (L, H, W) int32, probabilities (C, H, W)."""
-    from . import utils as U
-    category_layers = CATEGORY_LAYERS if category_layers is None else category_layers
+    category_layers = category_config()[0] if category_layers is None else category_layers
     lab = _to_dev(np.asarray(labels).astype(np.int32), torch.int32)
-    n_layers, h, w = lab.shape
-    inds = np.cumsum(category_layers)
     probs = np.asarray(probabilities)
-    chan = [int(np.searchsorted(inds, li, side='right')) for li in range(n_layers)]
-    pr = _to_dev(probs[chan], torch.float64 if probs.dtype == np.float64 else torch.float32)
-    counts = lab.reshape(n_layers, -1).max(dim=1).values.to(torch.int32)
-    geo = U.instance_geometry(lab, counts, pr)
-    total = int(geo["counts"].sum())
-    clen = torch.zeros(max(total, 1), dtype=torch.int32, device=lab.device)
-    if total:
-        L.fcall("mcb_contour_length", lab.data_ptr(), geo["_offsets"].data_ptr(), geo["_counts"].data_ptr(),
-                clen.data_ptr(), n_layers, h, w)
-    clen = clen.cpu().numpy()
+    pr = _to_dev(probs, torch.float64 if probs.dtype == np.float64 else torch.float32)
+    t = scoring_features_batch(lab[None], pr[None], None, category_layers)
+    cols = _feature_columns(t)
+    offs = _starts(t["counts"])
     thresholds = get_thresholds(category_layers)
     out = []
-    for li in range(n_layers):
+    for li in range(t["layers"]):
         feats = []
-        for i in range(int(geo["counts"][li])):
-            s = int(geo["offsets"][li]) + i
-            area = int(geo["area"][s])
-            bbox = (int(geo["rmin"][s]), int(geo["rmax"][s]) + 1, int(geo["cmin"][s]), int(geo["cmax"][s]) + 1)
-            bh, bw = bbox[1] - bbox[0], bbox[3] - bbox[2]
-            dists = (bbox[0], h - bbox[1], bbox[2], w - bbox[3])
-            feats.append({'iou': None, 'threshold': round(thresholds[li], 2), 'area': area,
-                          'mean_prob': float(geo["psum"][s]) / area,
-                          # np.where(mask, probabilities, 0).max(): the zeros outside the mask take part
-                          'max_prob': max(float(geo["pmax"][s]), 0.0) if area < h * w else float(geo["pmax"][s]),
-                          'bbox_ar': bh / bw, 'bbox_area': bw * bh, 'bbox_fill': area / (bw * bh),
-                          'min_dist_to_border': min(dists), 'max_dist_to_border': max(dists),
-                          'contour_length': int(clen[s])})
+        for s in range(int(offs[li]), int(offs[li + 1])):
+            f = {'iou': None, 'threshold': round(thresholds[li], 2)}
+            f.update({k: v[s].item() for k, v in cols.items()})
+            f['max_prob'] = float(t["pmax"][s]) if f['area'] == t["h"] * t["w"] else max(float(t["pmax"][s]), 0.0)
+            feats.append(f)
         out.append(feats)
     return out
+
+
+def get_features_for_image(image, probabilities, annotations):
+    """src/postprocessing.py:261-272: [DataFrame per layer] of one image, on the device"""
+    return FeatureExtractor().transform([image], [probabilities], [annotations])['features'][0]
+
+
+def get_iou_matrix(labels, annotations):
+    """src/postprocessing.py:306-321: cocomask.iou of every instance of one label layer (rows, label order) against the
+    annotations (columns), float64; None without annotations.  The annotations are left as they are (the reference
+    replaces their segmentations by the first polygon's RLE)."""
+    from . import utils as U
+    if annotations is None or annotations == []:
+        return None
+    lab = _to_dev(np.asarray(labels).astype(np.int32), torch.int32)
+    h, w = lab.shape
+    k = int(lab.max()) if lab.numel() else 0
+    if k == 0:
+        return []                 # cocomask.iou of an empty list
+    gt_cnts, gt_starts, _ = ground_truth_runs([list(annotations)], h, w)
+    g = len(gt_starts) - 1
+    dt_cnts, dt_starts, _, _ = U.rle_encode_instances(lab[None], torch.full((1,), k, dtype=torch.int32,
+                                                                            device=lab.device))
+    pair_dt = np.repeat(np.arange(k), g)
+    pair_gt = np.tile(np.arange(g), k)
+    return pair_iou(dt_cnts, dt_starts, gt_cnts, gt_starts, pair_dt, pair_gt).cpu().numpy().reshape(k, g)
+
+
+def get_iou(iou_matrix, label_nr):
+    """src/postprocessing.py:324-328"""
+    if iou_matrix is not None:
+        return iou_matrix[label_nr - 1].max()
+    return None
+
+
+def get_mask_with_iou(category_ind, category_instances, category_layers_inds, annotations, probabilities):
+    """src/postprocessing.py:275-283"""
+    category_ids = category_config()[1]
+    category_nr = np.searchsorted(category_layers_inds, category_ind, side='right')
+    category_annotations = annotations.get(category_ids[category_nr], [])
+    iou_matrix = get_iou_matrix(category_instances, category_annotations)
+    category_probabilities = probabilities[category_nr]
+    for label_nr in range(1, category_instances.max() + 1):
+        mask = category_instances == label_nr
+        yield mask, get_iou(iou_matrix, label_nr), category_probabilities
+
+
+def _prob_tensor(x):
+    """probabilities on the device, float32 kept, anything else as float64 (what skimage's resize hands over)"""
+    t = x.to(_dev()) if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x)).to(_dev())
+    return (t if t.dtype in (torch.float32, torch.float64) else t.to(torch.float64)).contiguous()
+
+
+def _label_tensor(x):
+    t = x.to(_dev()) if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x)).to(_dev())
+    return t.to(torch.int32).contiguous()
+
+
+def image_batches(images, probabilities, annotations, batch_size):
+    """(labels (B, L, H, W) int32 cuda, probabilities (B, C, H, W) cuda, [annotations]) for consecutive images, at most
+    `batch_size` of one size each.  Two device tensors are sliced; anything else is consumed once, in step, as the
+    reference's zip does: per-image lists, or the generators the Step chain passes in stream mode
+    (make_apply_transformer_stream, which scoring_model_train switches on)."""
+    if isinstance(images, torch.Tensor) and isinstance(probabilities, torch.Tensor):
+        n = images.shape[0]
+        ann = [{}] * n if annotations is None else list(annotations)
+        for b in range(0, n, batch_size):
+            yield _label_tensor(images[b:b + batch_size]), _prob_tensor(probabilities[b:b + batch_size]), \
+                ann[b:b + batch_size]
+        return
+    group = []
+
+    def stacked():
+        return (torch.stack([g[0] for g in group]), torch.stack([g[1] for g in group]), [g[2] for g in group])
+
+    for im, pr, ann in zip(images, probabilities, itertools.repeat({}) if annotations is None else annotations):
+        im, pr = _label_tensor(im), _prob_tensor(pr)
+        if group and (len(group) == batch_size or group[0][0].shape != im.shape or group[0][1].shape != pr.shape):
+            yield stacked()
+            group = []
+        group.append((im, pr, ann))
+    if group:
+        yield stacked()
+
+
+class _Stateless:
+    """BaseTransformer contract (src/steps/base.py:254-269) of a transformer without state"""
+
+    def fit(self, *args, **kwargs):
+        return self
+
+    def fit_transform(self, *args, **kwargs):
+        self.fit(*args, **kwargs)
+        return self.transform(*args, **kwargs)
+
+    def load(self, filepath):
+        return self
+
+    def save(self, filepath):
+        import joblib
+        joblib.dump({}, filepath)
+
+
+class FeatureExtractor(_Stateless):
+    """src/postprocessing.py:18-25: transform(images, probabilities, annotations=None) -> {'features': [[DataFrame per
+    layer] per image]}.  images: the dilated label maps, a list of (L, H, W) arrays or an (N, L, H, W) device tensor;
+    probabilities: the resized probabilities, (C, H, W) arrays or an (N, C, H, W) device tensor (the fast path: nothing
+    crosses PCIe but the feature table); annotations: per image {category id: [COCO annotations]}.  Lists and the
+    generators of stream mode are consumed once; images go through scoring_features_batch up to `batch_size` of one
+    size at a time, so tiles of different sizes may be mixed."""
+
+    def __init__(self, batch_size=20):
+        self.batch_size = int(batch_size)
+
+    def transform(self, images, probabilities, annotations=None):
+        features = []
+        for lab, pr, ann in image_batches(images, probabilities, annotations, self.batch_size):
+            features.extend(feature_frames(scoring_features_batch(lab, pr, ann)))
+        return {'features': features}
+
+
+class ScoreImageJoiner(_Stateless):
+    """src/postprocessing.py:28-33"""
+
+    def transform(self, images, scores):
+        return {'images_with_scores': list(zip(images, scores))}
 
 
 # ---------------------------------------------------------------------------------------------------------------------
