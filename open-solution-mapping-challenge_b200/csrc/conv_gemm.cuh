@@ -17,6 +17,7 @@
 #pragma once
 #include "tc.cuh"
 #include "detsum.cuh"
+#include "nanmax.cuh"
 
 namespace mcb {
 
@@ -66,9 +67,9 @@ struct ConvGemmParams {
   int accumulate;
   // Auxiliary tile (dgrad only): a tensor with the geometry of the OUTPUT, fetched chunk by chunk with TMA (tmX, same
   // boxes as tmD) into shared memory while the main loop of the tile still runs.
-  //   aux_mode 1: the ReLU output y of the producing layer:  g = acc * (y > 0)
+  //   aux_mode 1: the ReLU output y of the producing layer:  g = (y <= 0) ? 0 : acc  (a NaN y passes, as in torch)
   //   aux_mode 2: the BatchNorm input z of the producing conv-BN-ReLU unit: the mask is that unit's own output sign,
-  //               (fma(z, gamma*invstd, beta - mean*gamma*invstd) > 0), and the BatchNorm-backward reductions of the
+  //               (zero where fma(z, gamma*invstd, beta - mean*gamma*invstd) <= 0), and the BatchNorm-backward reductions of the
   //               stored gradient ride along:  dbeta += sum g,  dgamma += sum g * (z - mean) * invstd
   CUtensorMap tmX[4];
   int aux_mode;
@@ -435,10 +436,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
               uint32_t o[4] = {pk.x, pk.y, pk.z, pk.w};
 #pragma unroll
               for (int e = 0; e < 4; ++e) {
-                // bf16 > 0  <=>  sign bit clear and magnitude nonzero
-                const uint32_t lo = w[e] & 0xFFFFu, hi2 = w[e] >> 16;
-                if (!(lo != 0 && lo < 0x8000u)) o[e] &= 0xFFFF0000u;
-                if (!(hi2 != 0 && hi2 < 0x8000u)) o[e] &= 0x0000FFFFu;
+                if (bf16_le0(w[e] << 16)) o[e] &= 0xFFFF0000u;
+                if (bf16_le0(w[e])) o[e] &= 0x0000FFFFu;
               }
               *reinterpret_cast<uint4*>(cbuf + off) = make_uint4(o[0], o[1], o[2], o[3]);
               if (do_red) {
@@ -456,8 +455,9 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
               for (int j = 0; j < 4; ++j) {
                 float2 g = __bfloat1622float2(h2[j]);
                 const float2 zz = __bfloat1622float2(z2[j]);
-                if (!(fmaf(zz.x, sc[2 * j], sh[2 * j]) > 0.f)) { g.x = 0.f; o[j] &= 0xFFFF0000u; }
-                if (!(fmaf(zz.y, sc[2 * j + 1], sh[2 * j + 1]) > 0.f)) { g.y = 0.f; o[j] &= 0x0000FFFFu; }
+                // zero where the unit's output y <= 0 (torch's relu backward: a NaN y passes the gradient)
+                if (fmaf(zz.x, sc[2 * j], sh[2 * j]) <= 0.f) { g.x = 0.f; o[j] &= 0xFFFF0000u; }
+                if (fmaf(zz.y, sc[2 * j + 1], sh[2 * j + 1]) <= 0.f) { g.y = 0.f; o[j] &= 0x0000FFFFu; }
                 s1[2 * j] += g.x; s2[2 * j] += g.x * ((zz.x - mu[2 * j]) * is[2 * j]);
                 s1[2 * j + 1] += g.y; s2[2 * j + 1] += g.y * ((zz.y - mu[2 * j + 1]) * is[2 * j + 1]);
               }
@@ -643,7 +643,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_gemm_kernel(const __grid
           const float2 rv = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(rrow + col));
           v0 += rv.x; v1 += rv.y;
         }
-        if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+        if (p.relu) { v0 = relu_nan(v0); v1 = relu_nan(v1); }
         constexpr int UNITS = CW / 8;   // 16-byte units per staged row
         const int chunk = j / UNITS, unit = (j % UNITS) ^ swz;
         *reinterpret_cast<uint32_t*>(rowp + (size_t)chunk * OUT_CHUNK_BYTES + unit * 16 + 4 * (lane & 3)) =

@@ -4,6 +4,7 @@
 #include "host_common.h"
 #include "../../include/mcb200.h"
 #include "detsum.cuh"
+#include "nanmax.cuh"
 #include <algorithm>
 #include <math.h>
 
@@ -201,7 +202,7 @@ __global__ void bn_finalize_kernel(const float* __restrict__ stats, float count,
   if (c >= C) return;
   const float mean = stats[c] / count;
   float var = stats[C + c] / count - mean * mean;
-  var = fmaxf(var, 0.f);
+  if (var < 0.f) var = 0.f;   // cancellation; a NaN variance stays NaN, as torch's does
   const float invstd = rsqrtf(var + eps);
   const float sc = gamma[c] * invstd;
   scale[c] = sc;
@@ -275,7 +276,7 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const uint4* __restrict__
       f[j] = fmaf(f[j], sc[j], sh[j]);
       if (RES == 1) f[j] += g[j];
       if (RES == 2) f[j] += fmaf(g[j], rs[j], rh[j]);
-      if (relu) f[j] = fmaxf(f[j], 0.f);
+      if (relu) f[j] = relu_nan(f[j]);
     }
     y[i] = pack8(f);
     if (has2) {
@@ -286,7 +287,7 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const uint4* __restrict__
         f[j] = fmaf(f[j], sc[j], sh[j]);
         if (RES == 1) f[j] += g[j];
         if (RES == 2) f[j] += fmaf(g[j], rs[j], rh[j]);
-        if (relu) f[j] = fmaxf(f[j], 0.f);
+        if (relu) f[j] = relu_nan(f[j]);
       }
       y[i2] = pack8(f);
     }
@@ -311,7 +312,8 @@ __device__ __forceinline__ void bn_train_coef(const BNTrain& b, int C, int c0, f
   for (int j = 0; j < 8; ++j) {
     const int c = c0 + j;
     const float mean = __ldg(b.stats + c) / count;
-    const float var = fmaxf(__ldg(b.stats + C + c) / count - mean * mean, 0.f);
+    float var = __ldg(b.stats + C + c) / count - mean * mean;
+    if (var < 0.f) var = 0.f;   // cancellation; a NaN variance stays NaN, as torch's does
     const float invstd = rsqrtf(var + eps);
     sc[j] = __ldg(b.gamma + c) * invstd;
     sh[j] = __ldg(b.beta + c) - mean * sc[j];
@@ -353,7 +355,7 @@ __global__ void __launch_bounds__(256) bn_train_apply_kernel(const uint4* __rest
       f[j] = fmaf(f[j], sc[j], sh[j]);
       if (RES == 1) f[j] += g[j];
       if (RES == 2) f[j] += fmaf(g[j], rs[j], rh[j]);
-      if (relu) f[j] = fmaxf(f[j], 0.f);
+      if (relu) f[j] = relu_nan(f[j]);
     }
     y[i] = pack8(f);
     if (has2) {
@@ -364,7 +366,7 @@ __global__ void __launch_bounds__(256) bn_train_apply_kernel(const uint4* __rest
         f[j] = fmaf(f[j], sc[j], sh[j]);
         if (RES == 1) f[j] += g[j];
         if (RES == 2) f[j] += fmaf(g[j], rs[j], rh[j]);
-        if (relu) f[j] = fmaxf(f[j], 0.f);
+        if (relu) f[j] = relu_nan(f[j]);
       }
       y[i2] = pack8(f);
     }
@@ -380,7 +382,7 @@ MCB_DET_WORKSPACE(float, g_final_red, kFinalRedCap, final_red_finish_kernel)
 
 // Per-channel reductions over NHWC: block = 256 threads = (256 / C8) pixel lanes x C8 channel groups (C8 = C/8 <= 256).
 // MODE 0: sum(x)                                  -> out0                 (bias gradient)
-// MODE 1: g = dy * (y > 0); sum(g), sum(g * xhat) -> out0 (dbeta), out1 (dgamma)   xhat = (z - mean) * invstd
+// MODE 1: g = (y <= 0) ? 0 : dy; sum(g), sum(g * xhat) -> out0 (dbeta), out1 (dgamma)   xhat = (z - mean) * invstd
 template <int MODE>
 __global__ void channel_reduce_kernel(const uint4* __restrict__ a, const uint4* __restrict__ ymask,
                                       const uint4* __restrict__ z, const float* __restrict__ mean,
@@ -432,7 +434,7 @@ __global__ void channel_reduce_kernel(const uint4* __restrict__ a, const uint4* 
           if (ymask != nullptr) {
             unpack8(u ? mb : ma, m);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] = (m[j] > 0.f) ? f[j] : 0.f;
+            for (int j = 0; j < 8; ++j) f[j] = (m[j] <= 0.f) ? 0.f : f[j];
           }
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
@@ -465,7 +467,7 @@ __global__ void channel_reduce_kernel(const uint4* __restrict__ a, const uint4* 
   }
 }
 
-// dz = gamma*invstd * (g - dbeta/M - xhat * dgamma/M),  g = dy * (y > 0); optionally also emits g (the gradient that
+// dz = gamma*invstd * (g - dbeta/M - xhat * dgamma/M),  g = (y <= 0) ? 0 : dy; optionally also emits g (the gradient that
 // flows to the residual branch): g_out = g (store) or g_out += g (accumulate).  Per-channel coefficients in registers
 // (fixed channel group per thread), two independent loads per stream in flight.
 template <bool MASK, int GOUT>  // GOUT 0: none, 1: store, 2: accumulate
@@ -510,7 +512,7 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const uint4* __restri
         float m[8];
         unpack8(vm[u], m);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) g[j] = (m[j] > 0.f) ? g[j] : 0.f;
+        for (int j = 0; j < 8; ++j) g[j] = (m[j] <= 0.f) ? 0.f : g[j];
       }
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -547,12 +549,21 @@ __global__ void maxpool2_fwd_kernel(const uint4* __restrict__ x, uint4* __restri
     unpack8(__ldg(x + base + (long)W * C8), c);
     unpack8(__ldg(x + base + (long)W * C8 + C8), d);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) a[j] = fmaxf(fmaxf(a[j], b[j]), fmaxf(c[j], d[j]));
+    for (int j = 0; j < 8; ++j) a[j] = max_nan(max_nan(a[j], b[j]), max_nan(c[j], d[j]));
     y[i] = pack8(a);
   }
 }
-// gradient goes to the FIRST maximum in window scan order (torch's max_pool2d backward);
-// dx = (store | accumulate) routed gradient
+// torch's max_pool2d index rule: scanning the window in order, a position takes over when it is greater than the
+// current maximum or is NaN -- the FIRST maximum, or the LAST NaN of a window that holds one
+__device__ __forceinline__ int pool_argmax(const float (&v)[4][8], int j) {
+  int best = 0;
+  float m = v[0][j];
+#pragma unroll
+  for (int k = 1; k < 4; ++k)
+    if (v[k][j] > m || isnan(v[k][j])) { m = v[k][j]; best = k; }
+  return best;
+}
+// gradient goes to the window's pool_argmax (torch's max_pool2d backward); dx = (store | accumulate) routed gradient
 __global__ void maxpool2_bwd_kernel(const uint4* __restrict__ x, const uint4* __restrict__ dy, uint4* __restrict__ dx,
                                     int accumulate, int N, int H, int W, int C8) {
   const int Ho = H / 2, Wo = W / 2;
@@ -570,11 +581,7 @@ __global__ void maxpool2_bwd_kernel(const uint4* __restrict__ x, const uint4* __
     unpack8(__ldg(dy + i), g);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      int best = 0;
-      float m = v[0][j];
-#pragma unroll
-      for (int k = 1; k < 4; ++k)
-        if (v[k][j] > m) { m = v[k][j]; best = k; }
+      const int best = pool_argmax(v, j);
 #pragma unroll
       for (int k = 0; k < 4; ++k) o[k][j] = (k == best) ? g[j] : 0.f;
     }
@@ -592,8 +599,8 @@ __global__ void maxpool2_bwd_kernel(const uint4* __restrict__ x, const uint4* __
 }
 // Backward of the 2x2 max-pool over an encoder output y = relu(conv + b) that also feeds a decoder concat (VGG
 // encoders).  g holds the concat's data gradient on entry (the decoder runs first in the backward); in place,
-//   g = bf16(g + routed dpool) * (y > 0),
-// the pooled gradient going to the first maximum in window order like maxpool2_bwd_kernel.  The per-channel sums of the
+//   g = (y <= 0) ? 0 : bf16(g + routed dpool),
+// the pooled gradient going to the window's pool_argmax like maxpool2_bwd_kernel.  The per-channel sums of the
 // STORED bf16 g (the conv's bias gradient; the same values the dgrad epilogue's dx_channel_sum adds) go into this
 // block's row of g_channel_red.  Block = lanes x C8 threads with a fixed channel group per thread, like
 // channel_reduce_kernel; a pooled pixel is one 2x2 window.
@@ -621,15 +628,11 @@ __global__ void maxpool2_bwd_skip_relu_kernel(const uint4* __restrict__ y, const
     unpack8(__ldg(dpool + p * C8 + cg), d);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      int best = 0;
-      float m = v[0][j];
-#pragma unroll
-      for (int k = 1; k < 4; ++k)
-        if (v[k][j] > m) { m = v[k][j]; best = k; }
+      const int best = pool_argmax(v, j);
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         const float t = (k == best) ? o[k][j] + d[j] : o[k][j];
-        o[k][j] = v[k][j] > 0.f ? t : 0.f;
+        o[k][j] = v[k][j] <= 0.f ? 0.f : t;   // torch's relu backward: zero where y <= 0, so a NaN y passes g
       }
     }
 #pragma unroll
@@ -677,7 +680,7 @@ __global__ void final_conv_fwd_kernel(const uint4* __restrict__ x, const float* 
     for (int k = 0; k < K; ++k) logits[(n * K + k) * pixels_per_img + q] = acc[k] + sw[K * C + k];
   }
 }
-// backward: dx[p][c] = (x[p][c] > 0) * sum_k dlogits[k][p] W[k][c];  dW[k][c] += sum_p dlogits[k][p] x[p][c];
+// backward: dx[p][c] = (x[p][c] <= 0) ? 0 : sum_k dlogits[k][p] W[k][c];  dW[k][c] += sum_p dlogits[k][p] x[p][c];
 // db[k] += sum_p dlogits[k][p].   x is the ReLU output of dec0, so the mask folds dec0's ReLU backward in.
 __global__ void final_conv_bwd_kernel(const uint4* __restrict__ x, const float* __restrict__ w,
                                       const float* __restrict__ dlogits, uint4* __restrict__ dx,
@@ -712,7 +715,7 @@ __global__ void final_conv_bwd_kernel(const uint4* __restrict__ x, const float* 
         const int c = g * 8 + j;
         lw[0][c] = fmaf(d[0], f[j], lw[0][c]);
         lw[1][c] = fmaf(d[1], f[j], lw[1][c]);
-        o[j] = (f[j] > 0.f) ? (d[0] * sw[c] + d[1] * sw[C + c]) : 0.f;
+        o[j] = (f[j] <= 0.f) ? 0.f : (d[0] * sw[c] + d[1] * sw[C + c]);
       }
       dx[p * C8 + g] = pack8(o);
     }
