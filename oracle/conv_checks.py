@@ -2,8 +2,9 @@
 tests/test_conv_gemm_gpu.py (small shapes, about one tile per CTA), tests/test_conv_gemm_persistent_gpu.py (several
 tiles per CTA, every test hook), tests/test_conv_gemm_epilogue_overlap_gpu.py (the hand-off to the epilogue warpgroup),
 tests/test_conv_gemm_encoders_gpu.py (the 3x3 transposed conv) and tests/test_vgg_kernels_gpu.py (the VGG input and
-concat convs).  tests/test_elementwise_gpu.py takes its layout helpers.  Never imported by the product path; mcb200 is
-imported inside the functions, once the mcb fixture has built it.
+concat convs).  tests/test_elementwise_gpu.py takes its layout helpers and its bars for the stem's im2col GEMM, and
+oracle/elementwise_checks.py, the harness of the element-wise kernel tests, takes its bars.  Never imported by the
+product path; mcb200 is imported inside the functions, once the mcb fixture has built it.
 
 A case is a dict: desc (the seed key), n, h, w, cout, k, s (stride, 1 if absent), and the input channels of the conv:
 c0 and c1 (a concatenated second source, 0 if absent) for the forward references, cin for the others.

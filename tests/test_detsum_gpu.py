@@ -1,45 +1,16 @@
 """The fixed-order finishing sum of every cross-CTA reduction (csrc/detsum.cuh), run over caller-provided rows through
-mcb_det_sum_f32 and compared bit for bit with a float32 re-summation in the documented order: per lane l < 32 the rows
-l, l + 32, ... added in turn, then the lanes combined as a butterfly (16, 8, 4, 2, 1).  The BatchNorm statistics, the
-split-K weight gradients, the classifier and loss sums of the train step all end in this sum, so its order is what
-keeps their last bits the same from build to build.  Up to 32 rows the kernel runs one thread per element, above that
-one warp per element; row counts cover both: one row, fewer than a warp, exactly a warp, and several lanes' worth
-(133 rows: more than the 132 SMs of an H100, the most CTAs a persistent producer launches)."""
+mcb_det_sum_f32 and compared bit for bit with a float32 re-summation in the documented order
+(oracle/elementwise_checks.py reference_sum).  The BatchNorm statistics, the split-K weight gradients, the classifier
+and loss sums of the train step all end in this sum, so its order is what keeps their last bits the same from build to
+build.  Up to 32 rows the kernel runs one thread per element, above that one warp per element; row counts cover both:
+one row, fewer than a warp, exactly a warp, and several lanes' worth (133 rows: more than the 132 SMs of an H100, the
+most CTAs a persistent producer launches)."""
 import numpy as np
 import pytest
-import torch
+
+from oracle.elementwise_checks import reference_sum, run_det_sum, wide_range_rows
 
 pytestmark = pytest.mark.gpu
-
-
-def reference_sum(rows):
-    """float32, the library's order: rows [R, n] -> [n]"""
-    lanes = []
-    for l in range(32):
-        t = np.zeros(rows.shape[1], np.float32)
-        for r in range(l, rows.shape[0], 32):
-            t = (t + rows[r]).astype(np.float32)
-        lanes.append(t)
-    o = 16
-    while o:
-        for l in range(o):
-            lanes[l] = (lanes[l] + lanes[l + o]).astype(np.float32)
-        o //= 2
-    return lanes[0]
-
-
-def wide_range_rows(rng, nrows, n):
-    """magnitudes over six decades, so that a different association changes the rounding"""
-    return (rng.standard_normal((nrows, n)) * 10.0 ** rng.uniform(-3, 3, (nrows, n))).astype(np.float32)
-
-
-def run(rows_h, n, inner, out_stride, out_h, cuda):
-    from mcb200 import _lib as L
-    rows = torch.from_numpy(rows_h).to(cuda)
-    out = torch.from_numpy(out_h.copy()).to(cuda)
-    L.fcall("mcb_det_sum_f32", rows.data_ptr(), rows_h.shape[0], rows_h.shape[1], n, inner, out.data_ptr(), out_stride)
-    torch.cuda.synchronize()
-    return out.cpu().numpy()
 
 
 @pytest.mark.parametrize("nrows", [1, 7, 32, 33, 70, 133])
@@ -48,7 +19,7 @@ def test_det_sum_matches_fixed_order_bitwise(mcb, cuda, nrows):
     n = 1000                                  # not a multiple of the 256-thread CTA
     rows = wide_range_rows(rng, nrows, n)
     out0 = rng.standard_normal(n).astype(np.float32)
-    got = run(rows, n, n, 0, out0, cuda)
+    got = run_det_sum(rows, n, n, 0, out0)
     want = (out0 + reference_sum(rows)).astype(np.float32)
     assert np.array_equal(got.view(np.int32), want.view(np.int32)), \
         "%d of %d elements differ" % (int((got.view(np.int32) != want.view(np.int32)).sum()), n)
@@ -70,7 +41,7 @@ def test_det_sum_wide_output_and_strided_destination(mcb, cuda):
     n = inner * groups
     rows = wide_range_rows(rng, 9, n)
     dest = rng.standard_normal(groups * out_stride).astype(np.float32)
-    got = run(rows, n, inner, out_stride, dest, cuda)
+    got = run_det_sum(rows, n, inner, out_stride, dest)
     want = dest.copy()
     idx = (np.arange(n) // inner) * out_stride + np.arange(n) % inner
     want[idx] = (dest[idx] + reference_sum(rows)).astype(np.float32)

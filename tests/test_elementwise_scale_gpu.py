@@ -1,247 +1,31 @@
 """The HBM-bound kernels (csrc/elementwise.cu, csrc/loss.cu) at the batch-32 sizes of the ResNet101-UNet at 320x320,
 where every thread of their capped grid-stride loops runs several iterations.
 
-grid_for() caps a grid at 8 x SMs blocks of 256 threads; the BatchNorm apply kernels handle two 16-byte groups (i,
-i + stride) per iteration; channel_reduce_kernel and final_conv_bwd_kernel cap at 4 x SMs blocks and keep a private
-partial per thread that detsum.cuh adds in block order; the loss kernels cap at 8 x SMs blocks.  Every case asserts,
-from the device's SM count and these launch formulas, that each thread (or each pixel lane of a reduction block) owns
-at least 3 work items, and the cases marked ragged also assert a partial last pass (for the BatchNorm kernels: a
-thread whose second group falls off the end).  Shapes are the network's layers "C@HxW" at batch 32, or at a larger
-batch where 32 images do not give every thread 3 items; one tensor case lives in device memory at a time.
-
-References are float64 from the bf16-rounded operands; A is the same operation on |operands|.
-  * integer-exact cases (channel sums, BatchNorm backward sums, the classifier) and pure data movement (max-pool with
-    its first-maximum tie rule, layout conversions, stem im2col, fp32 -> bf16) must match exactly; sums stay < 2^24;
-  * real-valued reductions: |got - ref| <= 2^-16 A, and a second run repeats the first bitwise;
-  * bf16 outputs: |got - ref| <= 2^-8 |ref| (half a bf16 ulp) + 2^-20 A;
-  * BatchNorm statistics (mean, invstd, running mean / unbiased running variance) within a few fp32 ulps of the
-    float64 finalisation, scaled by the magnitudes the fp32 arithmetic cancels;
-  * the loss within 1e-6 relative, d(loss)/d(logits) per pixel within 2^-18 of that pixel's own CE weight / M and
-    Dice term;
-  * Adam, one step at a time from the kernel's own state, within 2^-18 of the step's update size (magnitudes) plus
-    one fp32 ulp of p; m and v within 2^-20 of their terms' magnitudes."""
+Every case asserts, from the device's SM count and the launch model of oracle/elementwise_checks.py, that each thread
+(or each pixel lane of a reduction block) owns at least 3 work items, and the cases marked ragged also assert a partial
+last pass (for the BatchNorm kernels: a thread whose second group falls off the end).  Shapes are the network's layers
+"C@HxW" at batch 32, or at a larger batch where 32 images do not give every thread 3 items; one tensor case lives in
+device memory at a time.  References and bars: oracle/elementwise_checks.py."""
 import ctypes as C
-import math
-import zlib
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from oracle import synthetic
 from oracle import unet_oracle as O
+from oracle.conv_checks import assert_bound, assert_exact, assert_same
+from oracle.elementwise_checks import (ADAM_EPS, BETAS, BF, BN, CSUM, EPS, F64, GRAD_SCALE, LOSS_N, LOSS_S, POOL,
+                                       SIZE_C, STEPS, WD, adam_lr, affine, assert_bf16, assert_reduce_regime,
+                                       assert_stride_regime, bn_bwd_reduce_ref, bn_case, check_adam, check_bn_apply,
+                                       check_bn_bwd_apply, check_fin, check_reduction, chunks, classifier_bwd_ref,
+                                       classifier_fwd_ref, free_case, gen, ids, ints, loss_case, loss_ref, pool_ref,
+                                       rand, randn, resnet101_unet_layout, with_ties)
 
 pytestmark = pytest.mark.gpu
-
-BF, F64 = torch.bfloat16, torch.float64
-U = 2.0 ** -24                       # fp32 unit roundoff
-MOM, EPS = C.c_float(0.1).value, C.c_float(1e-5).value   # BatchNorm momentum / eps as the kernels receive them
-
-_CASE = {}    # the current case's tensors: one case at a time, so device memory stays bounded
-_LAYOUT = {}  # UNetResNet(101)'s arena length and BatchNorm widths
-
-
-# ---------------------------------------------------------------------------------------------------------- helpers
-def cached(key, make):
-    if key not in _CASE:
-        _CASE.clear()
-        _CASE[key] = make()
-    return _CASE[key]
-
-
-def gen(*key):
-    return torch.Generator(device="cuda").manual_seed(zlib.crc32(repr(key).encode()))
-
-
-def randn(g, *shape):
-    return torch.randn(shape, generator=g, device="cuda")
-
-
-def rand(g, *shape):
-    return torch.rand(shape, generator=g, device="cuda")
-
-
-def ints(g, lo, hi, *shape):
-    """integers in [lo, hi] as float32"""
-    return torch.randint(lo, hi + 1, shape, generator=g, device="cuda", dtype=torch.int8).float()
-
-
-def chunks(n, per_image, limit=1 << 23):
-    """batch slices of at most `limit` elements: bounds the float64 temporaries of a reference"""
-    step = max(1, limit // per_image)
-    return [slice(i, min(n, i + step)) for i in range(0, n, step)]
-
-
-def assert_bound(got, ref, tol, what):
-    """|got - ref| <= tol element-wise (NaN counts as a failure)"""
-    got = got.double()
-    ref = ref.to(got.device, F64)
-    err = (got - ref).abs()
-    bad = ~(err <= tol)
-    if bad.any():
-        i = tuple(int(v) for v in bad.nonzero()[0])
-        t = float(tol[i]) if torch.is_tensor(tol) else tol
-        raise AssertionError("%s: %d/%d elements off, max err %g; first at %s: got %r, ref %r, bound %g" % (
-            what, int(bad.sum()), bad.numel(), float(err.nan_to_num(float("inf")).max()), i, float(got[i]),
-            float(ref[i]), t))
-
-
-def assert_exact(got, ref, what):
-    """equal values (+0 and -0 alike)"""
-    ref = ref.to(got.device)
-    if got.dtype != ref.dtype:
-        got, ref = got.double(), ref.double()
-    bad = got != ref
-    if bad.any():
-        i = tuple(int(v) for v in bad.nonzero()[0])
-        raise AssertionError("%s: %d/%d elements differ; first at %s: got %r, ref %r" % (
-            what, int(bad.sum()), bad.numel(), i, float(got[i]), float(ref[i])))
-
-
-def assert_same(a, b, what):
-    """bitwise repeat of a run"""
-    assert torch.equal(a, b), "%s: two runs differ in %d elements" % (what, int((a != b).sum()))
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def grid_for(work, threads, per_sm=8):
-    """elementwise.cu grid_for (also loss.cu loss_grid with 256 threads)"""
-    return max(1, min(-(-work // threads), sms() * per_sm))
-
-
-def assert_stride_regime(work, threads, per_sm=8, ragged=False, pair=False):
-    """a grid-stride loop over `work` items launched with grid_for: every thread owns at least 3 items; ragged: the last
-    pass is partial.  pair: the BatchNorm apply kernels, launched over ceil(work / 2) items, take items i and
-    i + stride per iteration -- ragged then means some thread's last iteration has no second item"""
-    grid = grid_for((work + 1) // 2 if pair else work, threads, per_sm)
-    t = grid * threads
-    assert work // t >= 3, "%d items over %d threads (%d SMs)" % (work, t, sms())
-    if ragged:
-        span = 2 * t if pair else t
-        assert work % span, "%d items fill every pass of %d threads" % (work, span)
-
-
-def assert_reduce_regime(pixels, c, ragged=False):
-    """channel_reduce_kernel: 256 - 256 % (C/8) threads = lanes x C/8, grid min(pixels / (4 lanes), 4 x SMs); each
-    pixel lane owns at least 3 pixels; ragged: some lane's last iteration has no second pixel"""
-    c8 = c // 8
-    threads = max(256 - 256 % c8, c8)
-    lanes = threads // c8
-    grid = max(1, min(-(-pixels // (lanes * 4)), sms() * 4))
-    assert pixels // (grid * lanes) >= 3, "%d pixels over %d lanes (%d SMs)" % (pixels, grid * lanes, sms())
-    if ragged:
-        assert pixels % (2 * grid * lanes)
-
-
-def ulp32(x):
-    """spacing of fp32 at the fp32 value nearest x"""
-    a = x.float().abs()
-    return (torch.nextafter(a, torch.full_like(a, float("inf"))) - a).double()
-
-
-def resnet101_unet_layout():
-    """(fp32 arena length, BatchNorm widths) of UNetResNet(101, 2)"""
-    if not _LAYOUT:
-        from mcb200 import unet_models
-        net = unet_models.UNetResNet(101, 2, is_deconv=True)
-        _LAYOUT["arena"] = net._p32.numel()
-        _LAYOUT["bns"] = [m.num_features for m in net.modules() if isinstance(m, torch.nn.BatchNorm2d)]
-    return _LAYOUT["arena"], _LAYOUT["bns"]
 
 
 # =====================================================================================================================
 # BatchNorm: train-apply (finalisation folded in), finalize + eval apply, backward apply and reduce, channel sums
-BN = [
-    dict(desc="64@160x160", c=64, h=160, w=160, n=32),      # the stem BatchNorm
-    dict(desc="64@80x80", c=64, h=80, w=80, n=32),
-    dict(desc="256@80x80", c=256, h=80, w=80, n=8),
-    dict(desc="128@40x40", c=128, h=40, w=40, n=64),
-    dict(desc="512@40x40", c=512, h=40, w=40, n=16),
-    dict(desc="256@20x20", c=256, h=20, w=20, n=128),
-    dict(desc="1024@20x20", c=1024, h=20, w=20, n=32),
-    dict(desc="512@10x10", c=512, h=10, w=10, n=256),
-    dict(desc="2048@10x10", c=2048, h=10, w=10, n=64),
-    # odd pixel counts: the last pass is partial
-    dict(desc="2048@10x10 x33", c=2048, h=10, w=10, n=33, ragged=True),
-    dict(desc="64@97x101 x31", c=64, h=97, w=101, n=31, ragged=True),
-]
-
-
-def ids(cases):
-    return [c["desc"].replace(" ", "_") for c in cases]
-
-
-def channel_stats(x):
-    """[sum, sumsq] per channel of an NHWC bf16 tensor, as the conv epilogue hands them over (fp32)"""
-    v = x.view(-1, x.shape[-1])
-    return torch.cat([v.sum(0, dtype=F64), (v.float() ** 2).sum(0, dtype=F64)]).float()
-
-
-def bn_case(c):
-    def make():
-        g = gen("bn", c["desc"])
-        n, h, w, ch = c["n"], c["h"], c["w"], c["c"]
-        s = rand(g, ch) * 1.5 + 0.5
-        o = (rand(g, ch) - 0.5) * s                      # per-channel offsets, |mean| <= std / 2
-        d = dict(z=(randn(g, n, h, w, ch) * s + o).to(BF), r=(randn(g, n, h, w, ch) * 1.2 - 0.1).to(BF),
-                 dy=randn(g, n, h, w, ch).to(BF), ym=randn(g, n, h, w, ch).clamp_min(0).to(BF),
-                 gamma=rand(g, ch) + 0.5, beta=randn(g, ch) * 0.3, rgamma=rand(g, ch) + 0.5, rbeta=randn(g, ch) * 0.3,
-                 rm0=randn(g, ch) * 0.1, rv0=rand(g, ch) + 0.5, rrm0=randn(g, ch) * 0.1, rrv0=rand(g, ch) + 0.5)
-        m = n * h * w
-        # backward operands: the forward's saved mean / invstd, gamma and the global dbeta / dgamma
-        d.update(bmean=randn(g, ch) * 0.2, binv=rand(g, ch) + 0.5, bgamma=randn(g, ch),
-                 dbeta=randn(g, ch) * 0.3 * m, dgamma=randn(g, ch) * 0.3 * m)
-        d["zstats"], d["rstats"] = channel_stats(d["z"]), channel_stats(d["r"])
-        return d
-    return cached(("bn", c["desc"]), make)
-
-
-def fin_ref(stats, count, rm0, rv0):
-    """float64 finalisation of fp32 [sum, sumsq] and bounds for the fp32 kernel: the variance E[x^2] - mean^2 cancels,
-    so its error scales with E[x^2] + mean^2"""
-    ch = stats.numel() // 2
-    s = stats.double()
-    mean, e2 = s[:ch] / count, s[ch:] / count
-    var = (e2 - mean * mean).clamp_min(0)
-    invstd = (var + EPS).rsqrt()
-    unbiased = var * count / (count - 1)
-    rm0, rv0 = rm0.double(), rv0.double()
-    var_tol = 4 * U * (e2 + mean * mean)
-    ref = dict(mean=mean, invstd=invstd, rm=(1 - MOM) * rm0 + MOM * mean, rv=(1 - MOM) * rv0 + MOM * unbiased)
-    tol = dict(mean=2 * U * mean.abs(), invstd=invstd * (6 * U + 0.5 * var_tol / (var + EPS)),
-               rm=4 * U * ((1 - MOM) * rm0.abs() + MOM * mean.abs()) + MOM * 2 * U * mean.abs(),
-               rv=4 * U * ((1 - MOM) * rv0.abs() + MOM * unbiased) + MOM * var_tol * count / (count - 1))
-    return ref, tol
-
-
-def check_fin(got, stats, count, rm0, rv0, what):
-    ref, tol = fin_ref(stats, count, rm0, rv0)
-    for k, v in got.items():
-        assert_bound(v, ref[k], tol[k], "%s %s" % (what, k))
-
-
-def check_apply(y, d, sc, sh, sh_abs, res, rsc, rsh, rsh_abs, relu, what):
-    """y = [relu](z * sc + sh [+ r | + r * rsc + rsh]); sh_abs, rsh_abs: magnitudes of the terms inside the shifts"""
-    z, r = d["z"], d["r"]
-    n = z.shape[0]
-    for sl in chunks(n, z[0].numel()):
-        zz = z[sl].double()
-        f = zz * sc + sh
-        a = (zz * sc).abs() + sh_abs
-        if res == 1:
-            rr = r[sl].double()
-            f, a = f + rr, a + rr.abs()
-        elif res == 2:
-            rr = r[sl].double()
-            f, a = f + rr * rsc + rsh, a + (rr * rsc).abs() + rsh_abs
-        if relu:
-            f = f.clamp_min(0)
-        assert_bound(y[sl], f, 2.0 ** -8 * f.abs() + 2.0 ** -20 * a, "%s [images %d:%d]" % (what, sl.start, sl.stop))
-
-
 BN_FWD = [(c, res, relu) for c in BN for res in (0, 1, 2) for relu in (True, False)]
 
 
@@ -262,23 +46,18 @@ def test_bn_forward(mcb, cuda, c, res, relu):
     # train-apply
     rm, rv, mean, inv = d["rm0"].clone(), d["rv0"].clone(), e(), e()
     tr = ops.make_bn_train(d["zstats"], d["gamma"], d["beta"], rm, rv, mean, inv)
-    rtr = None
+    rtr = rbn = None
     if res == 2:
         rrm, rrv, rmean, rinv = d["rrm0"].clone(), d["rrv0"].clone(), e(), e()
         rtr = ops.make_bn_train(d["rstats"], d["rgamma"], d["rbeta"], rrm, rrv, rmean, rinv)
     y = torch.empty_like(z)
     ops.bn_train_apply(z, tr, y, relu, resid, rtr)
     check_fin(dict(mean=mean, invstd=inv, rm=rm, rv=rv), d["zstats"], pixels, d["rm0"], d["rv0"], "bn_train_apply")
-    sc = d["gamma"].double() * inv.double()
-    sh, sh_abs = d["beta"].double() - mean.double() * sc, d["beta"].double().abs() + (mean.double() * sc).abs()
-    rsc = rsh = rsh_abs = None
     if res == 2:
         check_fin(dict(mean=rmean, invstd=rinv, rm=rrm, rv=rrv), d["rstats"], pixels, d["rrm0"], d["rrv0"],
                   "bn_train_apply residual BN")
-        rsc = d["rgamma"].double() * rinv.double()
-        rsh = d["rbeta"].double() - rmean.double() * rsc
-        rsh_abs = d["rbeta"].double().abs() + (rmean.double() * rsc).abs()
-    check_apply(y, d, sc, sh, sh_abs, res, rsc, rsh, rsh_abs, relu, "bn_train_apply")
+        rbn = affine(d["rgamma"], d["rbeta"], rmean, rinv)
+    check_bn_apply(y, z, affine(d["gamma"], d["beta"], mean, inv), relu, "bn_train_apply", resid, rbn)
     # finalize + eval apply
     rm, rv, mean, inv, scale, shift = d["rm0"].clone(), d["rv0"].clone(), e(), e(), e(), e()
     ops.bn_finalize(d["zstats"], pixels, d["gamma"], d["beta"], rm, rv, scale, shift, mean, inv)
@@ -287,10 +66,10 @@ def test_bn_forward(mcb, cuda, c, res, relu):
     if res == 2:
         rscale, rshift, rmean, rinv = e(), e(), e(), e()
         ops.bn_finalize(d["rstats"], pixels, d["rgamma"], d["rbeta"], None, None, rscale, rshift, rmean, rinv)
-        rsc, rsh, rsh_abs = rscale.double(), rshift.double(), rshift.double().abs()
+        rbn = (rscale, rshift, rshift.abs())
     y = torch.empty_like(z)
     ops.bn_apply(z, scale, shift, y, relu, resid, rscale, rshift)
-    check_apply(y, d, scale.double(), shift.double(), shift.double().abs(), res, rsc, rsh, rsh_abs, relu, "bn_apply")
+    check_bn_apply(y, z, (scale, shift, shift.abs()), relu, "bn_apply", resid, rbn)
 
 
 BN_BWD = [(c, mask, gout) for c in BN for mask, gout in ((False, "none"), (True, "none"), (True, "store"),
@@ -312,18 +91,8 @@ def test_bn_bwd_apply(mcb, cuda, c, mask, gout):
     g_out = {"none": None, "store": torch.empty_like(z), "accumulate": d["r"].clone()}[gout]
     ops.bn_bwd_apply(dy, ym, z, d["bmean"], d["binv"], d["bgamma"], d["dbeta"], d["dgamma"], dz, g_out,
                      gout == "accumulate")
-    mu, iv = d["bmean"].double(), d["binv"].double()
-    a = d["bgamma"].double() * iv
-    k1, k2 = d["dbeta"].double() / pixels, d["dgamma"].double() / pixels
-    for sl in chunks(n, z[0].numel()):
-        gg = dy[sl].double()
-        if mask:
-            gg = gg * (ym[sl] > 0)
-        zz = z[sl].double()
-        ref = a * (gg - k1 - (zz - mu) * iv * k2)
-        A = a.abs() * (gg.abs() + k1.abs() + (zz.abs() + mu.abs()) * iv * k2.abs())
-        assert_bound(dz[sl], ref, 2.0 ** -8 * ref.abs() + 2.0 ** -20 * A, "bn_bwd_apply dz [images %d:%d]" % (
-            sl.start, sl.stop))
+    check_bn_bwd_apply(dz, dy, ym, z, d["bmean"], d["binv"], d["bgamma"], d["dbeta"], d["dgamma"], pixels,
+                       "bn_bwd_apply dz")
     if gout != "none":
         g = dy.masked_fill(ym <= 0, 0) if mask else dy
         if gout == "accumulate":
@@ -355,32 +124,12 @@ def test_bn_bwd_reduce(mcb, cuda, c, kind):
         db, dgm = pre_b.clone(), pre_g.clone()
         ops.bn_bwd_reduce(dy, ym, z, mean, inv, db, dgm)
         runs.append((db, dgm))
-    mu, iv = mean.double(), inv.double()
-    sb = sg = ab = ag = 0
-    for sl in chunks(n, z[0].numel()):
-        gg = dy[sl].double()
-        if ym is not None:
-            gg = gg * (ym[sl] > 0)
-        zz = z[sl].double()
-        sb = sb + gg.sum((0, 1, 2))
-        sg = sg + (gg * (zz - mu) * iv).sum((0, 1, 2))
-        ab = ab + gg.abs().sum((0, 1, 2))
-        ag = ag + (gg.abs() * (zz.abs() + mu.abs()) * iv).sum((0, 1, 2))
+    sb, sg, ab, ag = bn_bwd_reduce_ref(dy, ym, z, mean, inv)
     (db, dgm), (db2, dgm2) = runs
-    ref_b, ref_g = pre_b.double() + sb, pre_g.double() + sg
-    ab, ag = ab + pre_b.double().abs(), ag + pre_g.double().abs()
-    if kind == "exact":
-        assert max(float(ab.max()), float(ag.max())) < 2 ** 24
-        assert_exact(db, ref_b, "dbeta")
-        assert_exact(dgm, ref_g, "dgamma")
-    else:
-        assert_bound(db, ref_b, 2.0 ** -16 * ab, "dbeta")
-        assert_bound(dgm, ref_g, 2.0 ** -16 * ag, "dgamma")
+    check_reduction(db, pre_b, sb, ab, kind == "exact", "dbeta")
+    check_reduction(dgm, pre_g, sg, ag, kind == "exact", "dgamma")
     assert_same(db, db2, "dbeta")
     assert_same(dgm, dgm2, "dgamma")
-
-
-CSUM = BN + [dict(desc="32@320x320", c=32, h=320, w=320, n=32, ragged=True)]   # dec0's bias gradient
 
 
 @pytest.mark.parametrize("c,exact", [pytest.param(c, e, id="%s-%s" % (i, e)) for c, i in zip(CSUM, ids(CSUM))
@@ -401,13 +150,7 @@ def test_channel_sum(mcb, cuda, c, exact):
         ops.channel_sum(x, out)
         runs.append(out)
     v = x.view(-1, ch)
-    ref = pre.double() + v.sum(0, dtype=F64)
-    A = pre.double().abs() + v.abs().sum(0, dtype=F64)
-    if exact == "exact":
-        assert float(A.max()) < 2 ** 24
-        assert_exact(runs[0], ref, "channel_sum")
-    else:
-        assert_bound(runs[0], ref, 2.0 ** -16 * A, "channel_sum")
+    check_reduction(runs[0], pre, v.sum(0, dtype=F64), v.abs().sum(0, dtype=F64), exact == "exact", "channel_sum")
     assert_same(runs[0], runs[1], "channel_sum")
 
 
@@ -501,14 +244,10 @@ def test_bn_eval_params_batched(mcb, cuda):
 
 # =====================================================================================================================
 # 2x2 max-pool
-POOL = [dict(desc="64@160x160->80x80", c=64, h=160, w=160, n=32),     # after the stem
-        dict(desc="2048@10x10->5x5", c=2048, h=10, w=10, n=160, ragged=True)]
-
-
 @pytest.mark.parametrize("c", POOL, ids=ids(POOL))
 def test_maxpool(mcb, cuda, c):
-    """forward max, and the backward routing every gradient to the FIRST maximum of its window in scan order, stored
-    (all four positions overwritten) or added to an existing gradient"""
+    """forward max, and the backward routing every gradient to the FIRST maximum of its window in scan order (pool_ref),
+    stored (all four positions overwritten) or added to an existing gradient"""
     from mcb200 import ops
     n, h, w, ch = c["n"], c["h"], c["w"], c["c"]
     ho, wo = h // 2, w // 2
@@ -519,20 +258,10 @@ def test_maxpool(mcb, cuda, c):
     x[0, 0:2, 0:2] = 1.5                                     # fully tied windows
     x[1 % n, 2:4, 2:4] = -0.75
     dy = randn(g, n, ho, wo, ch).to(BF)
-    xv = x.view(n, ho, 2, wo, 2, ch)
-    cands = [xv[:, :, ky, :, kx] for ky in (0, 1) for kx in (0, 1)]   # scan order
-    m, best = cands[0], torch.zeros(cands[0].shape, dtype=torch.int8, device=cuda)
-    for k in (1, 2, 3):
-        upd = cands[k] > m
-        m = torch.where(upd, cands[k], m)
-        best = torch.where(upd, torch.full_like(best, k), best)
-    assert bool((cands[0] == cands[1]).any()), "no ties"
+    assert bool((x[:, 0::2, 0::2] == x[:, 0::2, 1::2]).any()), "no ties"
+    m, routed = pool_ref(x, dy)
     assert_exact(ops.maxpool2_fwd(x), m, "maxpool2_fwd")
-    routed = torch.zeros_like(x)
-    rv = routed.view(n, ho, 2, wo, 2, ch)
-    for k in range(4):
-        rv[:, :, k // 2, :, k % 2] = torch.where(best == k, dy, torch.zeros_like(dy))
-    del best, m, cands
+    del m
     dx = randn(g, n, h, w, ch).to(BF)
     ops.maxpool2_bwd(x, dy, dx, False)
     assert_exact(dx, routed, "maxpool2_bwd store")
@@ -572,36 +301,22 @@ def test_final_conv(mcb, cuda, exact):
         dx, dw, db = torch.empty_like(x), pre_w.clone(), pre_b.clone()
         ops.final_conv_bwd(x, wt.view(-1), dl, dx, dw, db)
         runs.append((dx, dw, db))
-    w64, b64 = wt.double(), b.double().view(1, k, 1, 1)
     sw = sb = aw = ab = 0
     dx = runs[0][0]
     for sl in chunks(n, h * w * ch):
-        xs, ds = x[sl].double(), dl[sl].double()
-        lg = torch.einsum("nhwc,kc->nkhw", xs, w64) + b64
-        la = torch.einsum("nhwc,kc->nkhw", xs.abs(), w64.abs()) + b64.abs()
-        gx = torch.einsum("nkhw,kc->nhwc", ds, w64)
-        gx = torch.where(xs > 0, gx, torch.zeros_like(gx))
-        ga = torch.einsum("nkhw,kc->nhwc", ds.abs(), w64.abs())
-        sw = sw + torch.einsum("nkhw,nhwc->kc", ds, xs)
-        aw = aw + torch.einsum("nkhw,nhwc->kc", ds.abs(), xs.abs())
-        sb, ab = sb + ds.sum((0, 2, 3)), ab + ds.abs().sum((0, 2, 3))
+        lg, la = classifier_fwd_ref(x[sl], wt, b)
+        gx, ga, *sums = classifier_bwd_ref(x[sl], wt, dl[sl])
+        sw, aw, sb, ab = (u + v for u, v in zip((sw, aw, sb, ab), sums))
         what = " [images %d:%d]" % (sl.start, sl.stop)
         if exact:
             assert_exact(logits[sl], lg, "final_conv_fwd" + what)
             assert_exact(dx[sl], gx, "final_conv_bwd dx" + what)
         else:
-            assert_bound(logits[sl], lg, 2.0 ** -16 * la, "final_conv_fwd" + what)
-            assert_bound(dx[sl], gx, 2.0 ** -8 * gx.abs() + 2.0 ** -20 * ga, "final_conv_bwd dx" + what)
-    ref_w, ref_b = pre_w.double() + sw.reshape(-1), pre_b.double() + sb
-    aw, ab = pre_w.double().abs() + aw.reshape(-1), pre_b.double().abs() + ab
+            assert_bound(logits[sl], lg, la, "final_conv_fwd" + what, rel=0.0)
+            assert_bf16(dx[sl], gx, ga, "final_conv_bwd dx" + what)
     (dx, dw, db), (dx2, dw2, db2) = runs
-    if exact:
-        assert max(float(aw.max()), float(ab.max())) < 2 ** 24
-        assert_exact(dw, ref_w, "final_conv_bwd dW")
-        assert_exact(db, ref_b, "final_conv_bwd db")
-    else:
-        assert_bound(dw, ref_w, 2.0 ** -16 * aw, "final_conv_bwd dW")
-        assert_bound(db, ref_b, 2.0 ** -16 * ab, "final_conv_bwd db")
+    check_reduction(dw, pre_w, sw, aw, exact, "final_conv_bwd dW")
+    check_reduction(db, pre_b, sb, ab, exact, "final_conv_bwd db")
     assert_same(dx, dx2, "final_conv_bwd dx")
     assert_same(dw, dw2, "final_conv_bwd dW")
     assert_same(db, db2, "final_conv_bwd db")
@@ -609,23 +324,6 @@ def test_final_conv(mcb, cuda, exact):
 
 # =====================================================================================================================
 # losses at 32 x 320 x 320
-LOSS_N, LOSS_S = 32, 320
-SIZE_C = math.sqrt(LOSS_S * LOSS_S) / 2.0   # the size weight's constant for 320 x 320 tiles
-
-
-def loss_case():
-    def make():
-        _, t = synthetic.train_batch(LOSS_N, LOSS_S, seed=320, n_rect=40)
-        t = torch.from_numpy(t)
-        t[:, 2, ::9, ::7] = 0                # size 0 (weight 1) pixels, inside and outside buildings
-        t = t.to("cuda")
-        g = gen("loss")
-        logits = randn(g, LOSS_N, 2, LOSS_S, LOSS_S) * 2
-        logits[:, 1] += 1.5 * (2 * t[:, 0] - 1)   # a partly trained net: mostly, not always, right
-        return logits, t
-    return cached(("loss",), make)
-
-
 @pytest.mark.parametrize("mode", [0, 1], ids=["weighted_ce_dice", "plain_ce"])
 def test_loss(mcb, cuda, mode):
     """loss_partials (the four global sums) + loss_grad (loss, dlogits) against the float64 mixed_loss /
@@ -655,38 +353,18 @@ def test_loss(mcb, cuda, mode):
         ref = O.plain_ce_loss(lg, t64[:, :1])
     ref.backward()
     ref = ref.detach()
-    with torch.no_grad():
-        z = logits.double()
-        p = torch.softmax(z, 1)
-        p0, p1 = p[:, 0], p[:, 1]
-        t1 = (t64[:, 0].long() == 1).double()
-        w = O.loss_weights(t64, imsize=(LOSS_S, LOSS_S)) if mode == 0 else torch.ones_like(p1)
-        ce = torch.logsumexp(z, 1) - torch.where(t64[:, 0].long() != 0, z[:, 1], z[:, 0])
-        ref_sums = torch.stack([(p1 * t1).sum(), p1.sum(), t1.sum(), (w * ce).sum()])
+    ref_sums, p, tol = loss_ref(logits, t, mode)
     # every term is non-negative: A = ref
-    assert_bound(sums, ref_sums, 2.0 ** -16 * ref_sums, "loss sums [I, P, T, S]")
+    assert_bound(sums, ref_sums, ref_sums, "loss sums [I, P, T, S]", rel=0.0)
     assert_exact(sums[2], ref_sums[2], "loss sum T")
     assert abs(float(loss) - float(ref)) <= 1e-6 * abs(float(ref)), (float(loss), float(ref))
-    tol = w / pixels
+    assert_bound(dlog, lg.grad, 0.0, "dlogits", rel=0.0, extra=tol)
     if mode == 0:
-        I, P, T = (float(v) for v in ref_sums[:3])
-        dn, num = P + T + 1.0 + 1e-7, 2 * I + 1.0
-        tol = tol + 0.2 * (t1 * 2 / dn + num / dn ** 2) * p1 * p0
-    assert_bound(dlog, lg.grad, 2.0 ** -18 * tol.unsqueeze(1), "dlogits")
-    if mode == 0:
-        pr = ops.softmax2(logits)
-        assert_bound(pr, p, 2.0 ** -18 * p, "softmax2")
+        assert_bound(ops.softmax2(logits), p, 0.0, "softmax2", rel=0.0, extra=2.0 ** -18 * p)
 
 
 # =====================================================================================================================
 # fused Adam over the ResNet101-UNet parameter arena
-BETAS, ADAM_EPS, WD, GRAD_SCALE, STEPS = (0.9, 0.999), 1e-8, 1e-4, 0.3, 10
-
-
-def adam_lr(t):
-    return 5e-4 * (1 - 0.05 * t)
-
-
 def adam_zero_block(n):
     """parameters that are zero with zero gradients: v stays 0, the denominator is eps, the update 0"""
     return slice(n // 3, n // 3 + 4097)
@@ -707,32 +385,6 @@ def adam_grad(n, t):
     return grad
 
 
-def check_adam(t, lr, p0, m0, v0, grad, p, m, v, what):
-    """one step against float64 Adam (L2 decay folded into the gradient).  As in torch.optim.Adam, the bias
-    corrections come from the caller's double betas; the moment updates, lr, eps, weight decay and gradient scale
-    take the fp32 values the kernel receives"""
-    f = lambda x: C.c_float(x).value
-    b1, b2, lr, eps, wd, gs = f(BETAS[0]), f(BETAS[1]), f(lr), f(ADAM_EPS), f(WD), f(GRAD_SCALE)
-    bc1, bc2s = 1 - BETAS[0] ** t, math.sqrt(1 - BETAS[1] ** t)
-    step = 1 << 22
-    for lo in range(0, p.numel(), step):
-        s = slice(lo, lo + step)
-        P0, M0, V0, G = p0[s].double(), m0[s].double(), v0[s].double(), grad[s].double()
-        gi = G * gs + wd * P0
-        gmag = (G * gs).abs() + (wd * P0).abs()
-        mr = b1 * M0 + (1 - b1) * gi
-        vr = b2 * V0 + (1 - b2) * gi * gi
-        denom = vr.sqrt() / bc2s + eps
-        pr = P0 - lr / bc1 * mr / denom
-        mmag = b1 * M0.abs() + (1 - b1) * gmag
-        vmag = b2 * V0 + (1 - b2) * gmag * gmag
-        umag = lr / bc1 * mmag / denom
-        at = " step %d [%d:%d]" % (t, lo, min(lo + step, p.numel()))
-        assert_bound(m[s], mr, 2.0 ** -20 * mmag, what + " m" + at)
-        assert_bound(v[s], vr, 2.0 ** -20 * vmag, what + " v" + at)
-        assert_bound(p[s], pr, 2.0 ** -18 * umag + ulp32(pr), what + " p" + at)
-
-
 @pytest.mark.parametrize("entry", ["adam_step", "adam_step_dyn"])
 def test_adam_arena(mcb, cuda, entry):
     """STEPS steps over a vector the length of UNetResNet(101)'s fp32 arena, each checked from the kernel's own state;
@@ -740,7 +392,7 @@ def test_adam_arena(mcb, cuda, entry):
     from mcb200 import ops
     n, _ = resnet101_unet_layout()
     assert_stride_regime(n, 256, ragged=True)
-    _CASE.clear()
+    free_case()
     p = adam_init(n)
     m, v = torch.zeros_like(p), torch.zeros_like(p)
     p16 = torch.empty(n, dtype=BF, device=cuda)
@@ -771,7 +423,7 @@ def test_adam_dyn_segments_equal_adam_step(mcb, cuda):
     slices, gaps = [(0, a), (a, b), (c, e)], [(b, c), (e, n)]
     for lo, hi in slices:
         assert_stride_regime(hi - lo, 256)
-    _CASE.clear()
+    free_case()
     pa = adam_init(n)
     ma, va, ha = torch.zeros_like(pa), torch.zeros_like(pa), torch.zeros(n, dtype=BF, device=cuda)
     pb, mb, vb, hb = pa.clone(), ma.clone(), va.clone(), ha.clone()
@@ -795,19 +447,11 @@ def test_adam_dyn_segments_equal_adam_step(mcb, cuda):
 
 # =====================================================================================================================
 # layout conversion, stem im2col, fp32 -> bf16
-def with_ties(x, g):
-    """plant fp32 values exactly halfway between two bf16 values (round to nearest even decides)"""
-    k = min(x.numel(), 1 << 16)
-    y = randn(g, k).to(BF).float()
-    x.view(-1)[:k] = (y.view(torch.int32) | 0x8000).view(torch.float32)
-    return x
-
-
 def test_layout_conversions(mcb, cuda):
     from mcb200 import ops
     n, ch, h, w = 32, 3, 320, 320
     assert_stride_regime(n * ch * h * w, 256, ragged=True)
-    _CASE.clear()
+    free_case()
     g = gen("layout")
     x = with_ties(randn(g, n, ch, h, w), g)
     y = ops.nchw_to_nhwc_bf16(x)
@@ -824,7 +468,7 @@ def test_stem_im2col(mcb, cuda, w):
     wo = w // 2
     if w == 300:
         assert wo % 32
-    _CASE.clear()
+    free_case()
     g = gen("stem", w)
     x = with_ties(randn(g, n, 3, h, w), g)
     col = ops.stem_im2col(x)
@@ -840,7 +484,7 @@ def test_cast_f32_bf16(mcb, cuda):
     from mcb200 import ops
     n, _ = resnet101_unet_layout()
     assert_stride_regime(n, 256, ragged=True)
-    _CASE.clear()
+    free_case()
     g = gen("cast")
     x = with_ties(randn(g, n) * torch.pow(10.0, rand(g, n) * 6 - 3), g)
     assert_same(ops.cast_bf16(x, torch.empty(n, dtype=BF, device=cuda)), x.to(BF), "cast_f32_bf16")

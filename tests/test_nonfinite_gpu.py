@@ -4,16 +4,16 @@ A diverged run is only visible if its NaN travels: one NaN weight (what Adam lea
 NaN loss and NaN running statistics, as it does in the reference.  Every other test of the suite feeds finite operands,
 so a kernel that quietly turns a NaN into 0 (fmaxf-based ReLU, a max-pool that skips NaN, a variance clamp) passes them.
 
-assert_nonfinite_like(got, ref, bar): NaN, +Inf and -Inf of got sit at exactly ref's positions, and the finite elements
-meet `bar`, the bar the kernel already has in oracle/conv_checks.py or tests/test_elementwise_scale_gpu.py (None: the
-positions only).
+assert_nonfinite_like: NaN, +Inf and -Inf of got sit at exactly ref's positions, and the finite elements meet the bar
+the kernel already has in oracle/conv_checks.py or oracle/elementwise_checks.py.
 
-A. Each kernel against torch in float64 on the CPU (float32 where torch itself runs in float32), the non-finite values
-   planted in three kinds of place: inside the first tile or pass, in the ragged last tile or channel group, and in an
-   element that the kernel's grid-stride loop (or persistent tile loop) reaches only on a later pass, at the batch-32
-   shapes of tests/test_elementwise_scale_gpu.py.  torch's rules: relu(NaN) = NaN; max_pool2d's output is NaN if its
-   window holds a NaN, and its index is the first maximum or the last NaN in scan order; a NaN BatchNorm variance
-   makes invstd, scale, shift and the running variance NaN; relu's backward zeroes the gradient where y <= 0 only.
+A. Each kernel against torch, or against a float64 reference of oracle/elementwise_checks.py that follows torch's
+   rules, the non-finite values planted in three kinds of place: inside the first tile or pass, in the ragged last tile
+   or channel group, and in an element that the kernel's grid-stride loop (or persistent tile loop) reaches only on a
+   later pass, at the batch-32 shapes of oracle/elementwise_checks.py.  torch's rules: relu(NaN) = NaN; max_pool2d's
+   output is NaN if its window holds a NaN, and its index is the first maximum or the last NaN in scan order; a NaN
+   BatchNorm variance makes invstd, scale, shift and the running variance NaN; relu's backward zeroes the gradient where
+   y <= 0 only.
 B. The whole network against the reference (baseline/torch_cudnn_unet.py in fp32, oracle.step_checks.reference_step):
    the eval forward with a NaN or +Inf input pixel or a NaN encoder weight, and the fused train step with a NaN encoder
    weight, eager and through the captured graph.
@@ -27,9 +27,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-import test_detsum_gpu as DS
-import test_elementwise_scale_gpu as ES
 from oracle import conv_checks as CC
+from oracle import elementwise_checks as EC
 from oracle import make_golden_sigmoid_dice as SD
 from oracle import step_checks as SC
 from oracle.step_checks import no_tf32, rng_and_peak_memory  # noqa: F401  (fixtures)
@@ -39,12 +38,14 @@ pytestmark = pytest.mark.gpu
 BF, F64 = torch.bfloat16, torch.float64
 NAN, INF = float("nan"), float("inf")
 NONFINITE = (NAN, INF, -INF)
-_CACHE = {}
+_CACHE = {}   # conv_checks' references of CONV and GRAD
 
 
 # ---------------------------------------------------------------------------------------------------------- helpers
-def assert_nonfinite_like(got, ref, bar, what):
-    """NaN, +Inf, -Inf at exactly ref's positions; bar(got, ref, keep) on the elements ref has finite (keep: that mask)"""
+def assert_nonfinite_like(got, ref, what, absref=None, rel=2.0 ** -8, extra=0.0, finite_ref=None):
+    """NaN, +Inf, -Inf at exactly ref's positions; with absref given, conv_checks.assert_bound(absref, rel, extra) on
+    the elements ref has finite, against finite_ref there if given.  The non-finite elements of absref and extra count
+    as 0: a finite ref there is a ReLU or mask zero of a non-finite term, and got must equal it"""
     got = got.detach().double().cpu()
     ref = ref.detach().double().cpu()
     assert got.shape == ref.shape, (what, got.shape, ref.shape)
@@ -54,28 +55,11 @@ def assert_nonfinite_like(got, ref, bar, what):
             i = tuple(int(v) for v in (g != r).nonzero()[0])
             raise AssertionError("%s: %s at %d positions, the reference at %d; %d differ, first at %s: got %r, ref %r" % (
                 what, name, int(g.sum()), int(r.sum()), int((g != r).sum()), i, float(got[i]), float(ref[i])))
-    if bar is not None:
-        bar(got, ref, torch.isfinite(ref))
-
-
-def bound_bar(absref, what, rel=2.0 ** -8):
-    """oracle.conv_checks.assert_bound on the finite elements: rel |ref| + 2^-16 A"""
-    def bar(got, ref, keep):
-        # A is non-finite where a finite ref is a ReLU / mask zero of a non-finite term: there got must equal ref
-        a = absref.detach().double().cpu().nan_to_num(0, 0, 0)[keep] if torch.is_tensor(absref) else absref
-        CC.assert_bound(got[keep], ref[keep], a, what, rel=rel)
-    return bar
-
-
-def exact_bar(what):
-    return bound_bar(0.0, what, rel=0.0)
-
-
-def tol_bar(tol, what):
-    """tests/test_elementwise_scale_gpu.py's assert_bound with an explicit element-wise tolerance"""
-    def bar(got, ref, keep):
-        ES.assert_bound(got[keep], ref[keep], tol.detach().double().cpu()[keep], what)
-    return bar
+    if absref is not None:
+        keep = torch.isfinite(ref)
+        fin = lambda t: t.detach().double().cpu().nan_to_num(0, 0, 0)[keep] if torch.is_tensor(t) else t
+        want = ref if finite_ref is None else finite_ref.detach().double().cpu()
+        CC.assert_bound(got[keep], want[keep], fin(absref), what, rel=rel, extra=fin(extra))
 
 
 def plant(x, flat, values=NONFINITE):
@@ -86,16 +70,6 @@ def plant(x, flat, values=NONFINITE):
     return x
 
 
-def stride_places(total, threads, per_sm=8, pair=False):
-    """work-item indices of a grid_for grid-stride loop over `total` items: inside the first pass, on the second item of
-    a pair (pair: the BatchNorm apply kernels take i and i + stride), on the second pass, and the last item"""
-    grid = ES.grid_for((total + 1) // 2 if pair else total, threads, per_sm)
-    t = grid * threads
-    step = 2 * t if pair else t
-    assert total > step + t, "%d items do not reach a second pass of %d threads" % (total, step)
-    return [5, t + 3 if pair else 17, step + 11, total - 1]
-
-
 def cpu(t):
     return t.detach().cpu()
 
@@ -104,42 +78,21 @@ def cpu(t):
 # A. kernels
 # =====================================================================================================================
 # ---------------------------------------------------------------------------------- BatchNorm apply (train and eval)
-BN_CASES = [ES.BN[1], ES.BN[10]]      # 64@80x80 at batch 32; 64@97x101 x31, a partial last pass
+BN_CASES = [EC.BN[1], EC.BN[10]]      # 64@80x80 at batch 32; 64@97x101 x31, a partial last pass
 
 
 def poisoned_bn(c):
-    def make(_g):
-        d = ES.bn_case(c)
+    def make():
+        d = EC.bn_case(c)
         z, r = d["z"].clone(), d["r"].clone()
         ch = z.shape[-1]
-        groups = stride_places(z.numel() // 8, 256, pair=True)
+        groups = EC.stride_places(z.numel() // 8, 256, pair=True)
         # the non-finite values of z at channels 1, 4, 6 of each 8-channel group, r's at 2, 5, 7: both in the last one
         plant(z, [g * 8 + j for g in groups for j in (1, 4, 6)])
         plant(r, [g * 8 + j for g in groups for j in (2, 5, 7)])
         plant(z, [z.numel() - ch + 3], (NAN,))          # the last pixel's first channel group
         return dict(d, z=z, r=r)
-    return CC.cached(_CACHE, ("bn", c["desc"]), make)
-
-
-def bn_apply_ref(z, r, sc, sh, sh_abs, res, rsc, rsh, rsh_abs, relu):
-    """float64 on the CPU: y = [relu](z sc + sh [+ r | + r rsc + rsh]) and A, its terms' magnitudes (sh_abs, rsh_abs:
-    those of the terms inside the shifts)"""
-    zz = z.double().cpu()
-    v = lambda t: t.double().cpu()
-    f, a = zz * v(sc) + v(sh), (zz * v(sc)).abs() + v(sh_abs)
-    if res == 1:
-        rr = r.double().cpu()
-        f, a = f + rr, a + rr.abs()
-    elif res == 2:
-        rr = r.double().cpu()
-        f, a = f + rr * v(rsc) + v(rsh), a + (rr * v(rsc)).abs() + v(rsh_abs)
-    return (torch.relu(f) if relu else f), a
-
-
-def check_bn_apply(y, ref, a, what):
-    """test_elementwise_scale_gpu.check_apply's bar: 2^-8 |ref| + 2^-20 A"""
-    assert_nonfinite_like(y, ref, tol_bar(2.0 ** -8 * ref.abs().nan_to_num(0, 0, 0) + 2.0 ** -20 * a.nan_to_num(
-        0, 0, 0), what), what)
+    return EC.cached(("nonfinite bn", c["desc"]), make)
 
 
 @pytest.mark.parametrize("c,res,relu", [pytest.param(c, res, relu, id="%s-res%d-%s" % (
@@ -155,55 +108,51 @@ def test_bn_apply_nonfinite(mcb, cuda, c, res, relu):
     e = lambda: torch.empty(ch, device=cuda)
     rm, rv, mean, inv = d["rm0"].clone(), d["rv0"].clone(), e(), e()
     tr = ops.make_bn_train(d["zstats"], d["gamma"], d["beta"], rm, rv, mean, inv)
-    rtr = rsc = rsh = rsh_abs = None
+    rtr = rbn = None
     if res == 2:
         rmean, rinv = e(), e()
         rtr = ops.make_bn_train(d["rstats"], d["rgamma"], d["rbeta"], d["rrm0"].clone(), d["rrv0"].clone(), rmean, rinv)
     y = torch.empty_like(z)
     ops.bn_train_apply(z, tr, y, relu, resid, rtr)
-    sc = d["gamma"].double() * inv.double()
-    sh, sh_abs = d["beta"].double() - mean.double() * sc, d["beta"].double().abs() + (mean.double() * sc).abs()
     if res == 2:
-        rsc = d["rgamma"].double() * rinv.double()
-        rsh = d["rbeta"].double() - rmean.double() * rsc
-        rsh_abs = d["rbeta"].double().abs() + (rmean.double() * rsc).abs()
-    ref, a = bn_apply_ref(z, d["r"], sc, sh, sh_abs, res, rsc, rsh, rsh_abs, relu)
-    check_bn_apply(y, ref, a, "bn_train_apply")
+        rbn = EC.affine(d["rgamma"], d["rbeta"], rmean, rinv)
+    ref, a = EC.bn_apply_ref(z, EC.affine(d["gamma"], d["beta"], mean, inv), relu, resid, rbn)
+    assert_nonfinite_like(y, ref, "bn_train_apply", 0.0, extra=2.0 ** -20 * a)
     scale, shift = e(), e()
     ops.bn_finalize(d["zstats"], z.numel() // ch, d["gamma"], d["beta"], None, None, scale, shift, e(), e())
     rscale = rshift = None
     if res == 2:
         rscale, rshift = e(), e()
         ops.bn_finalize(d["rstats"], z.numel() // ch, d["rgamma"], d["rbeta"], None, None, rscale, rshift, e(), e())
+        rbn = (rscale, rshift, rshift.abs())
     y = torch.empty_like(z)
     ops.bn_apply(z, scale, shift, y, relu, resid, rscale, rshift)
-    ref, a = bn_apply_ref(z, d["r"], scale, shift, shift.abs(), res, rscale, rshift,
-                          None if rshift is None else rshift.abs(), relu)
-    check_bn_apply(y, ref, a, "bn_apply")
+    ref, a = EC.bn_apply_ref(z, (scale, shift, shift.abs()), relu, resid, rbn)
+    assert_nonfinite_like(y, ref, "bn_apply", 0.0, extra=2.0 ** -20 * a)
 
 
 # ------------------------------------------------------------------------------ BatchNorm statistics finalisation
 def bn_stats_case():
     """z (N, H, W, C) bf16 at 64@80x80, batch 32, with non-finite values in a few channels: one NaN (3), one +Inf (10),
     one -Inf (17), +Inf and -Inf (24: the sum reaches Inf - Inf), two +Inf (40), a NaN in the last channel (63)"""
-    def make(_g):
-        d = ES.bn_case(ES.BN[1])
+    def make():
+        d = EC.bn_case(EC.BN[1])
         z = d["z"].clone()
         n, h, w, ch = z.shape
         px = n * h * w
         at = lambda p, cc: p * ch + cc
         plant(z, [at(17, 3), at(px // 2, 10), at(px - 1, 17), at(100, 24), at(px - 7, 24), at(3, 40), at(px // 3, 40),
                   at(px - 1, 63)], (NAN, INF, -INF, INF, -INF, INF, INF, NAN))
-        return dict(d, z=z, zstats=ES.channel_stats(z))
-    return CC.cached(_CACHE, ("bnstats",), make)
+        return dict(d, z=z, zstats=EC.channel_stats(z))
+    return EC.cached(("nonfinite bnstats",), make)
 
 
 def torch_bn_train(z, gamma, beta, rm0, rv0):
     """torch.native_batch_norm(training=True) in float64 on the CPU: y, mean, invstd, running mean and variance"""
     x = z.double().cpu().permute(0, 3, 1, 2)
     rm, rv = rm0.double().cpu().clone(), rv0.double().cpu().clone()
-    y, mean, invstd = torch.native_batch_norm(x, gamma.double().cpu(), beta.double().cpu(), rm, rv, True, ES.MOM,
-                                              ES.EPS)
+    y, mean, invstd = torch.native_batch_norm(x, gamma.double().cpu(), beta.double().cpu(), rm, rv, True, EC.MOM,
+                                              EC.EPS)
     return y.permute(0, 2, 3, 1), mean, invstd, rm, rv
 
 
@@ -226,18 +175,17 @@ def test_bn_statistics_nonfinite(mcb, cuda, entry):
         ops.bn_train_apply(z, ops.make_bn_train(d["zstats"], d["gamma"], d["beta"], rm, rv, mean, inv), y, False)
         scale = d["gamma"] * inv
         shift = d["beta"] - mean * scale
-    fref, ftol = ES.fin_ref(d["zstats"], pixels, d["rm0"], d["rv0"])
+    fref, ftol = EC.fin_ref(d["zstats"], pixels, d["rm0"], d["rv0"])
     got = dict(mean=mean, invstd=inv, rm=rm, rv=rv)
     want = dict(mean=tmean, invstd=tinv, rm=trm, rv=trv)
     for k in got:
-        assert_nonfinite_like(got[k], want[k], lambda g, r, keep, k=k: ES.assert_bound(
-            g[keep], fref[k].cpu()[keep], ftol[k].cpu()[keep], "%s %s" % (entry, k)), "%s %s" % (entry, k))
+        assert_nonfinite_like(got[k], want[k], "%s %s" % (entry, k), 0.0, rel=0.0, extra=ftol[k], finite_ref=fref[k])
     tsc = d["gamma"].double().cpu() * tinv
-    assert_nonfinite_like(scale, tsc, None, entry + " scale")
-    assert_nonfinite_like(shift, d["beta"].double().cpu() - tmean * tsc, None, entry + " shift")
+    assert_nonfinite_like(scale, tsc, entry + " scale")
+    assert_nonfinite_like(shift, d["beta"].double().cpu() - tmean * tsc, entry + " shift")
     assert bool(torch.isnan(rv[[3, 10, 17, 24, 40, 63]]).all()), "a non-finite channel's running_var must be NaN"
     if entry == "bn_train_apply":
-        assert_nonfinite_like(y, ty, None, "bn_train_apply output")
+        assert_nonfinite_like(y, ty, "bn_train_apply output")
 
 
 # --------------------------------------------------------------------------------------------- conv forward epilogue
@@ -282,7 +230,7 @@ def test_conv_fwd_nonfinite(mcb, cuda, where, relu):
     ref = torch.relu(ref) if relu else ref
     A = conv(x.abs(), wt.abs()) * v(scale.abs()) + v(b.abs()) + res.double().abs()
     y = CC.run_fwd(c, x, wt, bias=b.cuda(), relu=relu, scale=scale.cuda(), residual=CC.dev(res))
-    assert_nonfinite_like(CC.nchw(y), ref, bound_bar(A, "conv_fwd"), "conv_fwd (%s non-finite)" % where)
+    assert_nonfinite_like(CC.nchw(y), ref, "conv_fwd (%s non-finite)" % where, A)
 
 
 # ----------------------------------------------------------------------------------------- conv data / weight gradient
@@ -303,7 +251,7 @@ def test_conv_wgrad_nonfinite_input(mcb, cuda):
     dw = torch.zeros(9, c["cout"], c["cin"], device=cuda)
     ops.conv_wgrad(CC.dev(dy), CC.dev(x), dw, 3, 1)
     got = ops.unpack_conv_weight(dw, 3)
-    assert_nonfinite_like(got, ref, bound_bar(A, "conv_wgrad", rel=0.0), "conv_wgrad")
+    assert_nonfinite_like(got, ref, "conv_wgrad", A, rel=0.0)
     assert bool(torch.isnan(got[:, 9]).all()), "the NaN input channel's weight gradient must be NaN at every tap"
 
 
@@ -322,7 +270,7 @@ def test_conv_dgrad_nonfinite(mcb, cuda):
     full, A = dg(wt, dy), dg(wt.abs(), dy.abs())
     ref = torch.ops.aten.threshold_backward(full, act.double(), 0.0)
     got = ops.conv_dgrad(CC.dev(dy), CC.pack(wt), 3, 1, (c["h"], c["w"]), relu_mask=CC.dev(act))
-    assert_nonfinite_like(CC.nchw(got), ref, bound_bar(A, "conv_dgrad"), "conv_dgrad")
+    assert_nonfinite_like(CC.nchw(got), ref, "conv_dgrad", A)
 
 
 # ---------------------------------------------------------------------------------------------------------- max-pool
@@ -351,35 +299,28 @@ def plant_windows(x, c8_places, windows=WINDOWS):
     return out
 
 
-def torch_pool(x, dy):
-    """max_pool2d forward and the gradient its backward routes (float32 on the CPU; bf16 values are exact)"""
-    xr = CC.nchw(x.float().cpu()).requires_grad_(True)
-    y = F.max_pool2d(xr, 2)
-    y.backward(CC.nchw(dy.float().cpu()))
-    return CC.nhwc(y.detach()), CC.nhwc(xr.grad)
-
-
 def test_maxpool_nonfinite(mcb, cuda):
     """maxpool2_fwd and maxpool2_bwd (store and accumulate) at 2048@10x10 -> 5x5, batch 160 (a partial last pass),
-    with the windows of WINDOWS planted: the output as torch's max_pool2d, the gradient routed to torch's index"""
+    with the windows of WINDOWS planted: the output as torch's max_pool2d, the gradient routed to torch's index
+    (elementwise_checks.pool_ref)"""
     from mcb200 import ops
-    c = ES.POOL[1]
+    c = EC.POOL[1]
     n, h, w, ch = c["n"], c["h"], c["w"], c["c"]
-    g = ES.gen("nonfinite pool")
-    x = ES.randn(g, n, h, w, ch).to(BF)
+    g = EC.gen("nonfinite pool")
+    x = EC.randn(g, n, h, w, ch).to(BF)
     total = n * (h // 2) * (w // 2) * ch // 8
-    plant_windows(x, stride_places(total, 256))
-    dy = ES.randn(g, n, h // 2, w // 2, ch).to(BF)
-    ref_y, routed = torch_pool(x, dy)
-    assert_nonfinite_like(ops.maxpool2_fwd(x), ref_y, exact_bar("maxpool2_fwd"), "maxpool2_fwd")
+    plant_windows(x, EC.stride_places(total, 256))
+    dy = EC.randn(g, n, h // 2, w // 2, ch).to(BF)
+    ref_y, routed = EC.pool_ref(x, dy)
+    assert_nonfinite_like(ops.maxpool2_fwd(x), ref_y, "maxpool2_fwd", 0.0, rel=0.0)
     dx = torch.empty_like(x)
     ops.maxpool2_bwd(x, dy, dx, False)
-    assert_nonfinite_like(dx, routed, exact_bar("maxpool2_bwd store"), "maxpool2_bwd store")
-    pre = ES.randn(g, n, h, w, ch).to(BF)
+    assert_nonfinite_like(dx, routed, "maxpool2_bwd store", 0.0, rel=0.0)
+    pre = EC.randn(g, n, h, w, ch).to(BF)
     dx = pre.clone()
     ops.maxpool2_bwd(x, dy, dx, True)
-    acc = (pre.float().cpu() + routed).to(BF)
-    assert_nonfinite_like(dx, acc, exact_bar("maxpool2_bwd accumulate"), "maxpool2_bwd accumulate")
+    acc = (pre.float() + routed.float()).to(BF)
+    assert_nonfinite_like(dx, acc, "maxpool2_bwd accumulate", 0.0, rel=0.0)
 
 
 def test_maxpool_bwd_skip_relu_nonfinite(mcb, cuda):
@@ -387,23 +328,20 @@ def test_maxpool_bwd_skip_relu_nonfinite(mcb, cuda):
     batch 32: g = (y <= 0) ? 0 : bf16(g + routed dpool), routed to torch's index; db += per-channel sums of g"""
     from mcb200 import ops
     n, h, w, ch = 32, 80, 80, 64
-    g = ES.gen("nonfinite skip pool")
-    y = ES.randn(g, n, h, w, ch).clamp_min(0).to(BF)
+    g = EC.gen("nonfinite skip pool")
+    y = EC.randn(g, n, h, w, ch).clamp_min(0).to(BF)
     pooled = n * (h // 2) * (w // 2)
-    lanes = (256 - 256 % (ch // 8)) // (ch // 8)
-    grid = max(1, min(-(-pooled // (lanes * 4)), CC.sms() * 4))
+    grid, lanes = EC.reduce_grid(pooled, ch)
     second = grid * lanes + 3                               # a pooled pixel a lane reaches on its second pass
     # y is a ReLU output: the windows without -Inf
     plant_windows(y, [i * (ch // 8) for i in (5, second, pooled - 1)],
                   [p for p in WINDOWS if not any(v == -INF for v in p)])
-    dpool = ES.randn(g, n, h // 2, w // 2, ch).to(BF)
-    g0 = ES.randn(g, n, h, w, ch).to(BF)
-    _, routed = torch_pool(y, dpool)
-    t = (g0.float().cpu() + routed).to(BF).float()
-    ref = torch.ops.aten.threshold_backward(t, y.float().cpu(), 0.0)
+    dpool = EC.randn(g, n, h // 2, w // 2, ch).to(BF)
+    g0 = EC.randn(g, n, h, w, ch).to(BF)
+    ref = EC.pool_skip_ref(y, g0, dpool)
     gg, db = g0.clone(), torch.zeros(ch, device=cuda)
     ops.maxpool2_bwd_skip_relu(y, dpool, gg, db)
-    assert_nonfinite_like(gg, ref, exact_bar("maxpool2_bwd_skip_relu g"), "maxpool2_bwd_skip_relu g")
+    assert_nonfinite_like(gg, ref, "maxpool2_bwd_skip_relu g", 0.0, rel=0.0)
     stored = gg.double().cpu().view(-1, ch)
     CC.assert_bound(db, stored.sum(0), stored.abs().sum(0), "maxpool2_bwd_skip_relu db", rel=0.0)
 
@@ -416,10 +354,10 @@ FINAL = (8, 320, 320, 32, 2)     # n, h, w, C, K: 819200 pixels, three passes of
 def test_final_conv_fwd_nonfinite(mcb, cuda, where):
     from mcb200 import ops
     n, h, w, ch, k = FINAL
-    g = ES.gen("nonfinite final fwd")
-    x = ES.randn(g, n, h, w, ch).clamp_min(0).to(BF)
-    wt, b = ES.randn(g, k, ch) * 0.2, ES.randn(g, k)
-    places = stride_places(n * h * w, 256)
+    g = EC.gen("nonfinite final fwd")
+    x = EC.randn(g, n, h, w, ch).clamp_min(0).to(BF)
+    wt, b = EC.randn(g, k, ch) * 0.2, EC.randn(g, k)
+    places = EC.stride_places(n * h * w, 256)
     if where == "x":
         plant(x, [p * ch + cc for p, cc in zip(places, (0, 9, 17, 31))], (NAN, INF, NAN, INF))
     elif where == "w":
@@ -428,36 +366,28 @@ def test_final_conv_fwd_nonfinite(mcb, cuda, where):
         b[0], b[1] = -INF, NAN
     logits = torch.empty(n, k, h, w, device=cuda)
     ops.final_conv_fwd(x, wt.reshape(-1), b, logits)
-    xs, w64, b64 = x.double().cpu(), wt.double().cpu(), b.double().cpu().view(1, k, 1, 1)
-    ref = torch.einsum("nhwc,kc->nkhw", xs, w64) + b64
-    la = torch.einsum("nhwc,kc->nkhw", xs.abs(), w64.abs()) + b64.abs()
-    assert_nonfinite_like(logits, ref, bound_bar(la, "final_conv_fwd", rel=0.0), "final_conv_fwd (%s)" % where)
+    ref, la = EC.classifier_fwd_ref(x.cpu(), wt.cpu(), b.cpu())
+    assert_nonfinite_like(logits, ref, "final_conv_fwd (%s)" % where, la, rel=0.0)
 
 
 def test_final_conv_bwd_nonfinite(mcb, cuda):
     """dx = (x > 0) W^T dlogits, dW += sum dlogits x^T, db += sum dlogits with NaN / +-Inf in dlogits"""
     from mcb200 import ops
     n, h, w, ch, k = FINAL
-    g = ES.gen("nonfinite final bwd")
-    x = ES.randn(g, n, h, w, ch).clamp_min(0).to(BF)
-    wt = ES.randn(g, k, ch) * 0.2
-    dl = ES.randn(g, n, k, h, w)
-    for p, kk, v in zip(stride_places(n * h * w, 128, 4), (0, 1, 1, 0), (NAN, INF, -INF, NAN)):
+    g = EC.gen("nonfinite final bwd")
+    x = EC.randn(g, n, h, w, ch).clamp_min(0).to(BF)
+    wt = EC.randn(g, k, ch) * 0.2
+    dl = EC.randn(g, n, k, h, w)
+    for p, kk, v in zip(EC.stride_places(n * h * w, 128, 4), (0, 1, 1, 0), (NAN, INF, -INF, NAN)):
         dl[p // (h * w), kk, p // w % h, p % w] = v
-    pre_w, pre_b = ES.randn(g, k * ch), ES.randn(g, k)
+    pre_w, pre_b = EC.randn(g, k * ch), EC.randn(g, k)
     dx, dw, db = torch.empty_like(x), pre_w.clone(), pre_b.clone()
     ops.final_conv_bwd(x, wt.reshape(-1), dl, dx, dw, db)
-    xs, ds, w64 = x.double().cpu(), dl.double().cpu(), wt.double().cpu()
-    gx = torch.where(xs > 0, torch.einsum("nkhw,kc->nhwc", ds, w64), torch.zeros(()).double())
-    ga = torch.einsum("nkhw,kc->nhwc", ds.abs(), w64.abs())
-    assert_nonfinite_like(dx, gx, tol_bar(2.0 ** -8 * gx.abs().nan_to_num(0, 0, 0) + 2.0 ** -20 * ga.nan_to_num(
-        0, 0, 0), "final_conv_bwd dx"), "final_conv_bwd dx")
-    ref_w = pre_w.double().cpu() + torch.einsum("nkhw,nhwc->kc", ds, xs).reshape(-1)
-    aw = pre_w.double().cpu().abs() + torch.einsum("nkhw,nhwc->kc", ds.abs(), xs.abs()).reshape(-1)
-    ref_b = pre_b.double().cpu() + ds.sum((0, 2, 3))
-    ab = pre_b.double().cpu().abs() + ds.abs().sum((0, 2, 3))
-    assert_nonfinite_like(dw, ref_w, bound_bar(aw, "final_conv_bwd dW", rel=0.0), "final_conv_bwd dW")
-    assert_nonfinite_like(db, ref_b, bound_bar(ab, "final_conv_bwd db", rel=0.0), "final_conv_bwd db")
+    gx, ga, sw, aw, sb, ab = EC.classifier_bwd_ref(x.cpu(), wt.cpu(), dl.cpu())
+    assert_nonfinite_like(dx, gx, "final_conv_bwd dx", 0.0, extra=2.0 ** -20 * ga)
+    pw, pb = pre_w.double().cpu(), pre_b.double().cpu()
+    assert_nonfinite_like(dw, pw + sw, "final_conv_bwd dW", pw.abs() + aw, rel=0.0)
+    assert_nonfinite_like(db, pb + sb, "final_conv_bwd db", pb.abs() + ab, rel=0.0)
 
 
 # ------------------------------------------------------------------------------------------------ softmax and loss
@@ -469,14 +399,14 @@ def test_loss_nonfinite_logit(mcb, cuda, kind, act):
     last pixel's other class: the loss, the four sums and d(loss)/d(logits) against autograd of the reference's loss
     in float64 on the CPU"""
     from mcb200 import ops
-    logits, t = ES.loss_case()
+    logits, t = EC.loss_case()
     z = logits.clone()
     v = {"nan": NAN, "+inf": INF, "-inf": -INF}[kind]
     n, _, s, _ = z.shape
-    p = stride_places(n * s * s, 256)[2]
+    p = EC.stride_places(n * s * s, 256)[2]
     z[p // (s * s), 1, p // s % s, p % s] = v
     z[n - 1, 0, s - 1, s - 1] = v
-    cfg = dict(size_c=ES.SIZE_C, dice_activation=act)
+    cfg = dict(size_c=EC.SIZE_C, dice_activation=act)
     sums = torch.zeros(4, dtype=F64, device=cuda)
     ops.loss_partials(z, t, sums, mode=0, **cfg)
     dlog, loss = torch.empty_like(z), torch.zeros((), device=cuda)
@@ -484,47 +414,47 @@ def test_loss_nonfinite_logit(mcb, cuda, kind, act):
     lg = z.double().cpu().requires_grad_(True)
     ref = SD.mixed_loss(lg, t.double().cpu(), imsize=(s, s), activation=act)
     ref.backward()
-    assert_nonfinite_like(loss.reshape(1), ref.detach().reshape(1), None, "loss (%s)" % act)
-    assert_nonfinite_like(dlog, lg.grad, None, "dlogits (%s)" % act)
+    assert_nonfinite_like(loss.reshape(1), ref.detach().reshape(1), "loss (%s)" % act)
+    assert_nonfinite_like(dlog, lg.grad, "dlogits (%s)" % act)
     if act == "softmax":
-        assert_nonfinite_like(ops.softmax2(z), torch.softmax(z.double().cpu(), 1), None, "softmax2")
+        assert_nonfinite_like(ops.softmax2(z), torch.softmax(z.double().cpu(), 1), "softmax2")
 
 
 # ------------------------------------------------------------------------------------------------------------- Adam
 @pytest.mark.parametrize("entry", ["adam_step", "adam_step_dyn"])
 def test_adam_nonfinite_gradient(mcb, cuda, entry):
     """one step with NaN and +-Inf gradients: p, m and v against torch.optim.Adam in float64 (L2 decay, the gradient
-    scale applied first); the finite elements within test_elementwise_scale_gpu.check_adam's bounds; the bf16 copy of p
+    scale applied first); the finite elements within elementwise_checks.check_adam's bounds; the bf16 copy of p
     non-finite where p is"""
     from mcb200 import ops
-    threads = ES.grid_for(1 << 30, 256) * 256
+    threads = EC.grid_for(1 << 30, 256) * 256
     n = 3 * threads + 1001
-    g = ES.gen("nonfinite adam")
-    p = ES.randn(g, n) * 0.05
-    m, v = ES.randn(g, n) * 1e-3, ES.rand(g, n) * 1e-6
-    grad = ES.randn(g, n) * 1e-2
-    places = stride_places(n, 256)
+    g = EC.gen("nonfinite adam")
+    p = EC.randn(g, n) * 0.05
+    m, v = EC.randn(g, n) * 1e-3, EC.rand(g, n) * 1e-6
+    grad = EC.randn(g, n) * 1e-2
+    places = EC.stride_places(n, 256)
     plant(grad, places + [q - 1 for q in places] + [q - 2 for q in places])
-    t, lr = 3, ES.adam_lr(3)
+    t, lr = 3, EC.adam_lr(3)
     p0, m0, v0 = p.clone(), m.clone(), v.clone()
     p16 = torch.empty(n, dtype=BF, device=cuda)
     if entry == "adam_step":
-        ops.adam_step(p, grad, m, v, p16, t, lr, ES.BETAS, ES.ADAM_EPS, ES.WD, ES.GRAD_SCALE)
+        ops.adam_step(p, grad, m, v, p16, t, lr, EC.BETAS, EC.ADAM_EPS, EC.WD, EC.GRAD_SCALE)
     else:
-        hyper = torch.tensor(ops.adam_hyper(lr, ES.BETAS, t), dtype=torch.float32, device=cuda)
-        ops.adam_step_dyn(p, grad, m, v, p16, hyper, ES.BETAS, ES.ADAM_EPS, ES.WD, ES.GRAD_SCALE)
+        hyper = torch.tensor(ops.adam_hyper(lr, EC.BETAS, t), dtype=torch.float32, device=cuda)
+        ops.adam_step_dyn(p, grad, m, v, p16, hyper, EC.BETAS, EC.ADAM_EPS, EC.WD, EC.GRAD_SCALE)
     tp = p0.double().cpu().requires_grad_(True)
-    opt = torch.optim.Adam([tp], lr=lr, betas=ES.BETAS, eps=ES.ADAM_EPS, weight_decay=ES.WD)
+    opt = torch.optim.Adam([tp], lr=lr, betas=EC.BETAS, eps=EC.ADAM_EPS, weight_decay=EC.WD)
     # the kernel's pre-step state: the step below runs at t
     opt.state[tp] = st = dict(step=torch.tensor(float(t - 1)), exp_avg=m0.double().cpu(), exp_avg_sq=v0.double().cpu())
-    tp.grad = grad.double().cpu() * C.c_float(ES.GRAD_SCALE).value
+    tp.grad = grad.double().cpu() * C.c_float(EC.GRAD_SCALE).value
     opt.step()
     keep = torch.isfinite(tp.detach()) & torch.isfinite(st["exp_avg"]) & torch.isfinite(st["exp_avg_sq"])
     for name, got, want in (("p", p, tp.detach()), ("m", m, st["exp_avg"]), ("v", v, st["exp_avg_sq"])):
-        assert_nonfinite_like(got, want, None, "%s %s" % (entry, name))
+        assert_nonfinite_like(got, want, "%s %s" % (entry, name))
     k = keep.to(cuda)
-    ES.check_adam(t, lr, p0[k], m0[k], v0[k], grad[k], p[k], m[k], v[k], entry)
-    assert_nonfinite_like(p16, p, None, entry + " bf16 copy")
+    EC.check_adam(t, lr, p0[k], m0[k], v0[k], grad[k], p[k], m[k], v[k], entry)
+    assert_nonfinite_like(p16, p, entry + " bf16 copy")
 
 
 # ------------------------------------------------------------------------------------ casts and layout kernels
@@ -543,7 +473,7 @@ def with_extremes(x, flat):
 
 
 def assert_cast_like(got, ref, what):
-    assert_nonfinite_like(got, ref, exact_bar(what), what)
+    assert_nonfinite_like(got, ref, what, 0.0, rel=0.0)
 
 
 def test_cast_and_layout_nonfinite(mcb, cuda):
@@ -551,9 +481,9 @@ def test_cast_and_layout_nonfinite(mcb, cuda):
     to +-Inf as tensor.to(torch.bfloat16) does; the largest finite value below the tie stays finite"""
     from mcb200 import ops
     n, ch, h, w = 32, 3, 320, 320
-    g = ES.gen("nonfinite cast")
-    x = ES.randn(g, n, ch, h, w)
-    with_extremes(x, stride_places(x.numel(), 256))
+    g = EC.gen("nonfinite cast")
+    x = EC.randn(g, n, ch, h, w)
+    with_extremes(x, EC.stride_places(x.numel(), 256))
     ref = x.to(BF)
     assert bool(torch.isinf(ref).sum() >= 4) and int((ref.view(torch.int16) == 0x7F7F).sum()) >= 1
     assert_cast_like(ops.cast_bf16(x.view(-1), torch.empty(x.numel(), dtype=BF, device=cuda)), ref.view(-1),
@@ -569,8 +499,8 @@ def test_im2col_nonfinite(mcb, cuda, entry):
     column that reads them (F.unfold of the same image, then the bf16 cast)"""
     from mcb200 import ops
     n, h, w = 32, 320, 300          # width 300: a partial last strip
-    g = ES.gen("nonfinite im2col", entry)
-    x = ES.randn(g, n, 3, h, w)
+    g = EC.gen("nonfinite im2col", entry)
+    x = EC.randn(g, n, 3, h, w)
     with_extremes(x, [3 * w + 7, (n // 2) * 3 * h * w + h * w + 5 * w + 100, x.numel() - 1])
     if entry == "stem_im2col":
         col = ops.stem_im2col(x)
@@ -579,7 +509,7 @@ def test_im2col_nonfinite(mcb, cuda, entry):
         col = ops.vgg_input_im2col(x)
         k, s, pad, taps, width = 3, 1, 1, 27, 32
     ho, wo = h // s, w // s
-    for sl in ES.chunks(n, 3 * h * w * k * k // (s * s)):
+    for sl in EC.chunks(n, 3 * h * w * k * k // (s * s)):
         u = F.unfold(x[sl].cpu(), k, padding=pad, stride=s)
         ref = u.view(u.shape[0], 3, k * k, ho, wo).permute(0, 3, 4, 2, 1).reshape(u.shape[0], ho, wo, taps)
         assert_cast_like(col[sl, ..., :taps], ref.to(BF), "%s [images %d:%d]" % (entry, sl.start, sl.stop))
@@ -589,10 +519,11 @@ def test_im2col_nonfinite(mcb, cuda, entry):
 # ------------------------------------------------------------------------------------------ fixed-order finishing sum
 def test_det_sum_nonfinite_rows(mcb, cuda):
     """mcb_det_sum_f32 over 70 rows: columns with one NaN, with +Inf and -Inf in different rows (Inf - Inf), with +Inf
-    only; against tests/test_detsum_gpu.py's float32 re-summation in the library's order, bit for bit where finite"""
+    only; against the float32 re-summation in the library's order (elementwise_checks.reference_sum), bit for bit
+    where finite"""
     rng = np.random.default_rng(70)
     nrows, n = 70, 1000
-    rows = DS.wide_range_rows(rng, nrows, n)
+    rows = EC.wide_range_rows(rng, nrows, n)
     rows[3, 10] = np.nan
     rows[69, 999] = np.nan
     rows[0, 20], rows[45, 20] = np.inf, -np.inf
@@ -601,9 +532,9 @@ def test_det_sum_nonfinite_rows(mcb, cuda):
     rows[33, 23] = -np.inf
     out0 = rng.standard_normal(n).astype(np.float32)
     with np.errstate(invalid="ignore", over="ignore"):
-        want = (out0 + DS.reference_sum(rows)).astype(np.float32)
-    got = DS.run(rows, n, n, 0, out0, cuda)
-    assert_nonfinite_like(torch.from_numpy(got), torch.from_numpy(want), exact_bar("det_sum"), "det_sum")
+        want = (out0 + EC.reference_sum(rows)).astype(np.float32)
+    got = EC.run_det_sum(rows, n, n, 0, out0)
+    assert_nonfinite_like(torch.from_numpy(got), torch.from_numpy(want), "det_sum", 0.0, rel=0.0)
     assert np.isnan(got[[10, 20, 21, 999]]).all() and got[22] == np.inf and got[23] == -np.inf
 
 
@@ -707,7 +638,7 @@ def test_eval_forward_nonfinite(mcb, cuda, enc, n, s):
             with torch.no_grad():
                 w.data[idx] = saved
         ref = reference_eval(enc, sdv, Xv[[0, last]])
-        assert_nonfinite_like(got[[0, last]], ref, None, "%s eval logits (%s)" % (enc, variant))
+        assert_nonfinite_like(got[[0, last]], ref, "%s eval logits (%s)" % (enc, variant))
         bad = (~torch.isfinite(got)).flatten(1).any(1)
         print("%s b%d %s: %d of %d logits of image 0 non-finite, images with a non-finite logit: %d" % (
             enc, n, variant, int((~torch.isfinite(got[0])).sum()), got[0].numel(), int(bad.sum())))
@@ -742,7 +673,7 @@ def check_poisoned_step(enc, loss, stats, params, ref):
     ref_loss, ref_stats, ref_nan = ref
     assert np.isnan(float(loss)) and np.isnan(ref_loss), (float(loss), ref_loss)
     for k in ref_stats:
-        assert_nonfinite_like(stats[k], ref_stats[k], None, "%s %s" % (enc, k))
+        assert_nonfinite_like(stats[k], ref_stats[k], "%s %s" % (enc, k))
     nan_stats = [k for k in ref_stats if bool(torch.isnan(ref_stats[k]).any())]
     assert nan_stats, "the poisoned conv's BatchNorm must get NaN running statistics"
     got_nan = nan_params(params)

@@ -7,14 +7,16 @@ H100 path:
   * the max-pool backward of a stage output that also feeds a decoder concat (mcb_maxpool2_bwd_skip_relu).
 
 References and bars: oracle/conv_checks.py (float64 from the bf16-rounded operands, on the device for the input conv
-and the pool; bf16 outputs within 2^-8 |ref| + 2^-16 A, fp32 sums and weight gradients within 2^-16 A).  Integer-
-valued variants must match bit for bit.  Every case asserts its launch regime from the device's SM count."""
+and the pool; bf16 outputs within 2^-8 |ref| + 2^-16 A, fp32 sums and weight gradients within 2^-16 A); the pool's
+routing and launch model: oracle/elementwise_checks.py.  Integer-valued variants must match bit for bit.  Every case
+asserts its launch regime from the device's SM count."""
 import pytest
 import torch
 import torch.nn.functional as F
 
 from oracle.conv_checks import (assert_bound, assert_exact, assert_same, assert_tiles_per_cta, bf16r, check_sums, dev,
-                                dgrad_ref, fwd_ref, nchw, nhwc, pack, run_fwd, sms, tile_count, wgrad_ref)
+                                dgrad_ref, fwd_ref, nchw, pack, run_fwd, tile_count, wgrad_ref)
+from oracle.elementwise_checks import pool_skip_ref, reduce_grid
 
 pytestmark = pytest.mark.gpu
 
@@ -170,48 +172,29 @@ def test_concat_32_64_persistent(mcb, cuda):
 
 
 # ---------------------------------------------------------------------------------------------------- pool + skip
-def _pool_skip_ref(y, gskip, dpool):
-    """float64 NCHW: g = (gskip + dpool routed to the first maximum of each window) * (y > 0)"""
-    n, c, h, w = y.shape
-    win = y.view(n, c, h // 2, 2, w // 2, 2).permute(0, 1, 2, 4, 3, 5).reshape(n, c, h // 2, w // 2, 4)
-    first = F.one_hot(win.argmax(-1), 4).double()          # argmax returns the first maximal index
-    routed = (first * dpool.unsqueeze(-1)).view(n, c, h // 2, w // 2, 2, 2).permute(0, 1, 2, 4, 3, 5).reshape(
-        n, c, h, w)
-    return (gskip + routed) * (y > 0).double()
-
-
-def _pool_regime(n, h, w, c):
-    """windows per thread of the capped grid (elementwise.cu reduce_cfg / mcb_maxpool2_bwd_skip_relu)"""
-    c8 = c // 8
-    threads = 256 - 256 % c8
-    lanes = threads // c8
-    pooled = n * (h // 2) * (w // 2)
-    grid = max(1, min((pooled + lanes * 4 - 1) // (lanes * 4), sms() * 4))
-    return pooled / (grid * lanes)
-
-
 POOL_SHAPES = [(8, 320, 320, 64), (4, 160, 160, 128), (2, 40, 40, 256), (2, 20, 20, 512), (3, 6, 10, 64)]
 
 
 @pytest.mark.parametrize("n,h,w,c", POOL_SHAPES)
 def test_pool_skip_relu_integer_exact(mcb, cuda, n, h, w, c):
     from mcb200 import ops
-    per = _pool_regime(n, h, w, c)
+    pooled = n * (h // 2) * (w // 2)
+    grid, lanes = reduce_grid(pooled, c)
     if n * h * w * c >= 8 * 160 * 160 * 64:
-        assert per > 2                                   # every thread loops over several windows
+        assert pooled / (grid * lanes) > 2               # every thread loops over several windows
     g = torch.Generator(device=cuda).manual_seed(n + h + c)
     # ReLU outputs in {0, 1, 2}: zeros (masked) and ties (first maximum) in most windows
     y = torch.randint(-2, 3, (n, c, h, w), generator=g, device=cuda).clamp_min(0).double()
     gskip = torch.randint(-4, 5, (n, c, h, w), generator=g, device=cuda).double()
     dpool = torch.randint(-4, 5, (n, c, h // 2, w // 2), generator=g, device=cuda).double()
-    ref = _pool_skip_ref(y, gskip, dpool)
+    ref = nchw(pool_skip_ref(dev(y), dev(gskip), dev(dpool)))
     gd = dev(gskip)
     base = torch.randint(-8, 9, (c,), generator=g, device=cuda).float()
     db = base.clone()
     ops.maxpool2_bwd_skip_relu(dev(y), dev(dpool), gd, db)
     assert_exact(nchw(gd), ref, "pool skip")
     assert bool((nchw(gd)[y == 0] == 0).all())
-    assert torch.equal(db.double(), base.double() + ref.sum(dim=(0, 2, 3)))
+    assert torch.equal(db.double(), base.double() + ref.sum(dim=(0, 2, 3), dtype=torch.float64))
     db2 = base.clone()
     gd2 = dev(gskip)
     ops.maxpool2_bwd_skip_relu(dev(y), dev(dpool), gd2, db2)
@@ -226,12 +209,10 @@ def test_pool_skip_relu_real(mcb, cuda, n, h, w, c):
     y = bf16r(torch.relu(torch.randn(n, c, h, w, generator=g, device=cuda))).double()
     gskip = bf16r(torch.randn(n, c, h, w, generator=g, device=cuda)).double()
     dpool = bf16r(torch.randn(n, c, h // 2, w // 2, generator=g, device=cuda)).double()
-    ref = _pool_skip_ref(y, gskip, dpool)
     gd = dev(gskip)
     db = torch.zeros(c, dtype=torch.float32, device=cuda)
     ops.maxpool2_bwd_skip_relu(dev(y), dev(dpool), gd, db)
-    expect = nhwc(ref.float()).to(torch.bfloat16)        # fp32 sum of two bf16 values, one rounding
-    assert torch.equal(gd, expect)
+    assert torch.equal(gd, pool_skip_ref(dev(y), dev(gskip), dev(dpool)))   # the single rounding of the fp32 sum
     check_sums(db, nchw(gd), "pool skip bias gradient", False)
     db2 = torch.zeros_like(db)
     gd2 = dev(gskip)
