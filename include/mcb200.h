@@ -481,6 +481,29 @@ int mcb_coco_match(const double* iou, const long long* iou_off, const int* nd, c
                    uint8_t* gt_ignore, uint8_t* gt_taken, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Second-level scoring model (src/models.py:212-282, csrc/forest.cu; the importers are mcb200.forest)
+ * ---------------------------------------------------------------------------------------------------------------- */
+#define MCB_FOREST_SKLEARN 0      /* RandomForestRegressor.predict */
+#define MCB_FOREST_LIGHTGBM 1     /* Booster.predict of an L2 regression model */
+#define MCB_FOREST_DEFAULT_LEFT 2 /* flag bit: a missing value goes left (LightGBM's kDefaultLeftMask) */
+#define MCB_FOREST_MISSING_ZERO 1 /* (flags >> 2) & 3, LightGBM's MissingType */
+#define MCB_FOREST_MISSING_NAN 2
+/* ScoringRandomForest.transform / ScoringLightGBM.transform (src/models.py:232-243, 267-278): out fp64 [rows] =
+ * (0.0 + leaf of tree 0 + leaf of tree 1 + ... in tree order) [/ n_trees when average], for the row-major fp64 feature
+ * matrix x [rows][n_features].  One node format for both libraries: node n has feature[n] (int32), threshold[n]
+ * (fp64), left[n] / right[n] (int32: a node index, or ~k for leaf_value[k]) and flags[n] (uint8, LightGBM's
+ * decision_type layout without the categorical bit); tree_root int32 [n_trees] is a node index or ~k for a one-leaf
+ * tree.  The forest must be acyclic (mcb200.forest validates it).  semantics MCB_FOREST_SKLEARN: x is cast to float32,
+ * NaN follows DEFAULT_LEFT, else x <= threshold.  MCB_FOREST_LIGHTGBM: |x| <= (double)1e-35f becomes 0.0, NaN under a
+ * missing type other than NaN becomes 0.0, a zero under MISSING_ZERO or a NaN under MISSING_NAN follows DEFAULT_LEFT,
+ * else x <= threshold.  work fp64 [chunk_trees * rows] is caller-owned: the trees are traversed chunk by chunk, one
+ * thread per (tree, row), and each row's running sum is carried across chunks in out. */
+int mcb_forest_predict(const double* x, int rows, int n_features, const int* tree_root, int n_trees, const int* feature,
+                       const double* threshold, const int* left, const int* right, const uint8_t* flags,
+                       const double* leaf_value, int semantics, int average, double* work, int chunk_trees, double* out,
+                       void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Target preparation from COCO polygons (src/preparation.py:18-198, csrc/polygon.cu)
  * ---------------------------------------------------------------------------------------------------------------- */
 /* pycocotools maskApi.c rleFrPoly + rleDecode (cocomask.frPyObjects(polys, h, w) then decode), bit-exact.  The host

@@ -238,6 +238,9 @@ for _n, _a in _SIGS8.items():
     getattr(lib, _n).argtypes = _a
     getattr(lib, _n).restype = ci
 
+lib.mcb_forest_predict.argtypes = [vp, ci, ci, vp, ci, vp, vp, vp, vp, vp, vp, ci, ci, vp, ci, vp, vp]
+lib.mcb_forest_predict.restype = ci
+
 lib.mcb_sync_step_bump.argtypes = [vp, vp]
 lib.mcb_sync_step_bump.restype = ci
 lib.mcb_sync_exchange.argtypes = [vp, vp, ci, ci, cl, cl, ci, vp, vp, vp, vp, ci, cf, vp]

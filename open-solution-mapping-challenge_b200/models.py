@@ -604,3 +604,133 @@ class FusedTrainStep:
     def count_launches(self):
         """kernel launches of one step (our kernels + memsets issued by the plan)"""
         return self.plan.launches_fwd + self.plan.launches_bwd + (6 if self.adam_in_graph else 4)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# second-level scoring model (src/models.py:212-282): host training, device prediction
+# ---------------------------------------------------------------------------------------------------------------------
+def _convert_features_to_df(features):
+    """src/models.py:457-462: every layer but the first (background) of every image, in one frame"""
+    import pandas as pd
+    df_features = []
+    for image_features in features:
+        for layer_features in image_features[1:]:
+            df_features.append(layer_features)
+    return pd.concat(df_features)
+
+
+class _DeviceForestScoring:
+    """transform / save / load shared by the two scoring models; subclasses say how the device forest is imported"""
+
+    _forest = None
+
+    def fit_transform(self, *args, **kwargs):
+        self.fit(*args, **kwargs)
+        return self.transform(*args, **kwargs)
+
+    def _device_forest(self):
+        if self._forest is None:
+            self._forest = self._import_forest()
+        return self._forest
+
+    def transform(self, features, **kwargs):
+        """{'scores': [[list of np.float64 per layer] per image]} as the reference's loop of one predict per
+        (image, layer) gives them ([] for an empty layer), from one upload, one launch and one readback of the
+        `feature_names` columns of every frame of the call"""
+        counts, blocks = [], []
+        for image_features in features:
+            counts.append([len(layer_features) for layer_features in image_features])
+            blocks += [layer_features[self.feature_names].to_numpy(dtype=np.float64)
+                       for layer_features in image_features if len(layer_features) > 0]
+        x = np.concatenate(blocks) if blocks else np.zeros((0, len(self.feature_names)))
+        prediction = self._device_forest().predict(x)
+        scores, at = [], 0
+        for image_counts in counts:
+            image_scores = []
+            for k in image_counts:
+                image_scores.append(list(prediction[at:at + k]))
+                at += k
+            scores.append(image_scores)
+        return {'scores': scores}
+
+    def save(self, filepath):
+        import joblib
+        joblib.dump((self.estimator, self.feature_names), filepath)
+
+    def load(self, filepath):
+        import joblib
+        self.estimator, self.feature_names = joblib.load(filepath)
+        self._forest = None
+        return self
+
+
+class ScoringLightGBM(_DeviceForestScoring):
+    """src/models.py:212-249 over src/steps/sklearn/models.py:69-99.  `fit` trains a LightGBM booster on the host with
+    the reference's parameters, split and early stopping; `transform` predicts on the device from the booster's text
+    model (Booster.model_to_string(num_iteration=None): the trees up to the best iteration, the ones Booster.predict
+    uses), bit-exact to Booster.predict.  Training, and loading a saved booster (joblib unpickles a lightgbm.Booster),
+    need `lightgbm` importable.  Refused with NotImplementedError: categorical splits, linear trees, multiclass models
+    and objectives other than plain L2 'regression'."""
+
+    def __init__(self, model_params, training_params, train_size, target):
+        self.model_params = model_params
+        self.training_params = training_params
+        self.evaluation_function = None
+        self.train_size = train_size
+        self.target = target
+        self.feature_names = []
+        self.estimator = None
+
+    def fit(self, features, **kwargs):
+        import lightgbm as lgb
+        from sklearn.model_selection import train_test_split
+        df_features = _convert_features_to_df(features)
+        train_data, val_data = train_test_split(df_features, train_size=self.train_size)
+        self.feature_names = list(df_features.columns.drop(self.target))
+        train = lgb.Dataset(train_data[self.feature_names], label=train_data[self.target],
+                            feature_name=self.feature_names, categorical_feature=[])
+        valid = lgb.Dataset(val_data[self.feature_names], label=val_data[self.target],
+                            feature_name=self.feature_names, categorical_feature=[])
+        evaluation_results = {}
+        # the reference's lgb.train keywords evals_result / early_stopping_rounds / verbose_eval, as the callbacks
+        # current LightGBM takes
+        self.estimator = lgb.train(self.model_params, train, valid_sets=[train, valid], valid_names=['train', 'valid'],
+                                   num_boost_round=self.training_params['number_boosting_rounds'],
+                                   feval=self.evaluation_function,
+                                   callbacks=[lgb.record_evaluation(evaluation_results),
+                                              lgb.early_stopping(self.training_params['early_stopping_rounds']),
+                                              lgb.log_evaluation(10)])
+        self._forest = None
+        return self
+
+    def _import_forest(self):
+        from .forest import from_lightgbm_string
+        if self.estimator is None:
+            raise RuntimeError("ScoringLightGBM: no booster; fit or load one first")
+        return from_lightgbm_string(self.estimator.model_to_string(num_iteration=None))
+
+
+class ScoringRandomForest(_DeviceForestScoring):
+    """src/models.py:252-284 over src/steps/sklearn/models.py:30-40.  `fit` trains sklearn's RandomForestRegressor on
+    the host; `transform` predicts on the device, bit-exact to RandomForestRegressor.predict at n_jobs=1 (with more
+    jobs sklearn adds the trees in completion order, so its own result varies in the last bits)."""
+
+    def __init__(self, train_size, target, model_params):
+        from sklearn.ensemble import RandomForestRegressor
+        self.train_size = train_size
+        self.target = target
+        self.feature_names = []
+        self.estimator = RandomForestRegressor(**model_params)
+
+    def fit(self, features, **kwargs):
+        from sklearn.model_selection import train_test_split
+        df_features = _convert_features_to_df(features)
+        train_data, val_data = train_test_split(df_features, train_size=self.train_size)
+        self.feature_names = list(df_features.columns.drop(self.target))
+        self.estimator.fit(train_data[self.feature_names], train_data[self.target])
+        self._forest = None
+        return self
+
+    def _import_forest(self):
+        from .forest import from_sklearn
+        return from_sklearn(self.estimator)
