@@ -262,12 +262,27 @@ def build_score(image, probabilities):
 
 def dense_crf_batch(imgs, probs, compat_gaussian=3, sxy_gaussian=1, compat_bilateral=10, sxy_bilateral=1, srgb=50,
                     iterations=5):
-    """imgs (N,3,H,W) float32 ImageNet-normalised, probs (N,2,H,W) float32, both cuda -> (N,2,H,W) float32"""
-    assert imgs.is_cuda and probs.is_cuda and imgs.dtype == torch.float32 and probs.dtype == torch.float32
-    imgs, probs = imgs.contiguous(), probs.contiguous()
+    """imgs (N,3,H,W) float32 ImageNet-normalised, probs (N,2,H,W) float32, both cuda -> (N,2,H,W) float32.
+    Mismatched shapes, dtypes or devices raise ValueError before anything is launched: the kernels index both buffers
+    with probs' shape."""
+    if not (isinstance(imgs, torch.Tensor) and isinstance(probs, torch.Tensor)):
+        raise ValueError("dense_crf_batch: imgs and probs must be tensors")
+    if imgs.dtype != torch.float32 or probs.dtype != torch.float32:
+        raise ValueError("dense_crf_batch: imgs and probs must be float32, got %s and %s" % (imgs.dtype, probs.dtype))
+    if not (imgs.is_cuda and imgs.device == probs.device):
+        raise ValueError("dense_crf_batch: imgs and probs must be on one CUDA device, got %s and %s"
+                         % (imgs.device, probs.device))
+    if probs.dim() != 4 or imgs.dim() != 4:
+        raise ValueError("dense_crf_batch: imgs (N,3,H,W) and probs (N,2,H,W), got %s and %s"
+                         % (tuple(imgs.shape), tuple(probs.shape)))
     n, c, h, w = probs.shape
     if c != 2:
         raise NotImplementedError("dense_crf: 2 labels (the reference builds DenseCRF2D(width, height, 2))")
+    if tuple(imgs.shape) != (n, 3, h, w):
+        raise ValueError("dense_crf_batch: imgs %s does not match probs %s" % (tuple(imgs.shape), tuple(probs.shape)))
+    imgs, probs = imgs.contiguous(), probs.contiguous()
+    if probs.numel() == 0:
+        return torch.empty_like(probs)
     rgb = torch.empty((n, h, w, 3), dtype=torch.uint8, device=probs.device)
     L.fcall("mcb_crf_rgb_from_normalized", imgs.data_ptr(), rgb.data_ptr(), n, h, w)
     out = torch.empty_like(probs)
@@ -289,14 +304,33 @@ def dense_crf(img, output_probs, compat_gaussian=3, sxy_gaussian=1, compat_bilat
 
 def watershed_batch(prob, markers, mask, levels=256):
     """prob (P,H,W) float32|float64, markers (P,H,W) int32, mask (P,H,W) uint8|bool, cuda -> int32 labels.
-    Not a reference function; semantics = oracle/post_oracle.py::minimax_watershed (parity unpinned)."""
-    assert prob.is_cuda and prob.dtype in (torch.float32, torch.float64)
+    Not a reference function; semantics = oracle/post_oracle.py::minimax_watershed (parity unpinned).
+    Mismatched shapes, dtypes or devices raise ValueError before anything is launched: the kernel indexes all three
+    buffers with prob's shape."""
+    if not all(isinstance(t, torch.Tensor) for t in (prob, markers, mask)):
+        raise ValueError("watershed_batch: prob, markers and mask must be tensors")
+    if prob.dtype not in (torch.float32, torch.float64):
+        raise ValueError("watershed_batch: prob must be float32 or float64, got %s" % prob.dtype)
+    if markers.dtype not in (torch.int32, torch.int64, torch.int16, torch.int8, torch.uint8):
+        raise ValueError("watershed_batch: markers must be an integer tensor, got %s" % markers.dtype)
+    if mask.dtype not in (torch.bool, torch.uint8):
+        raise ValueError("watershed_batch: mask must be bool or uint8, got %s" % mask.dtype)
+    if not (prob.is_cuda and markers.device == prob.device and mask.device == prob.device):
+        raise ValueError("watershed_batch: prob, markers and mask must be on one CUDA device, got %s, %s and %s"
+                         % (prob.device, markers.device, mask.device))
+    if prob.dim() != 3 or markers.shape != prob.shape or mask.shape != prob.shape:
+        raise ValueError("watershed_batch: prob, markers and mask must all be (P,H,W), got %s, %s and %s"
+                         % (tuple(prob.shape), tuple(markers.shape), tuple(mask.shape)))
+    if not 2 <= int(levels) <= 65536:
+        raise ValueError("watershed_batch: levels %d outside [2, 65536]" % int(levels))
     prob, markers = prob.contiguous(), markers.contiguous().to(torch.int32)
     mask = mask.contiguous()
     if mask.dtype == torch.bool:
         mask = mask.view(torch.uint8)
     p, h, w = prob.shape
     out = torch.empty((p, h, w), dtype=torch.int32, device=prob.device)
+    if out.numel() == 0:
+        return out
     ws = torch.empty(3 * p * h * w, dtype=torch.int32, device=prob.device)
     L.fcall("mcb_watershed", prob.data_ptr(), int(prob.dtype == torch.float64), markers.data_ptr(), mask.data_ptr(),
             out.data_ptr(), ws.data_ptr(), p, h, w, int(levels))

@@ -248,6 +248,8 @@ def dense_crf(img, output_probs, compat_gaussian=3, sxy_gaussian=1, compat_bilat
         out = np.zeros_like(a)
         ys0, ys1 = max(0, -dy), min(H, H - dy)
         xs0, xs1 = max(0, -dx), min(W, W - dx)
+        if ys0 >= ys1 or xs0 >= xs1:   # a shift past the image's edge (images smaller than the window)
+            return out
         out[..., ys0:ys1, xs0:xs1] = a[..., ys0 + dy:ys1 + dy, xs0 + dx:xs1 + dx]
         return out
 
@@ -287,10 +289,20 @@ def dense_crf(img, output_probs, compat_gaussian=3, sxy_gaussian=1, compat_bilat
 # --------------------------------------------------------------------------------------------------------------------
 # watershed (PARITY UNPINNED: not a reference function; this restatement DEFINES the semantics)
 # --------------------------------------------------------------------------------------------------------------------
+def relief_levels(prob, levels=256):
+    """the quantised relief of minimax_watershed: floor((1 - prob) * (levels - 1)) in float64, clipped to
+    [0, levels - 1] BEFORE the cast to int64 (so no |prob|, however large, can overflow the cast).  Non-finite values:
+    +Inf gives 0 and -Inf gives levels - 1 by the clip; NaN gives 0, as if prob were 1 (lowest ground)."""
+    v = np.floor((1.0 - np.asarray(prob).astype(np.float64)) * (levels - 1))
+    v = np.where(np.isnan(v), 0.0, np.clip(v, 0.0, float(levels - 1)))
+    return v.astype(np.int64)
+
+
 def minimax_watershed(prob, markers, mask, levels=256):
     """Marker-based watershed on the relief -prob (4-connectivity), defined order-independently in three stages so
     that any relaxation schedule reaches the same fixed point:
-      level(p) = floor((1 - prob(p)) * (levels - 1))   (quantised relief; high probability = low ground)
+      level(p) = floor((1 - prob(p)) * (levels - 1))   (quantised relief; high probability = low ground), clipped to
+                 [0, levels - 1] in float64; NaN is level 0 (relief_levels)
       1. cost(p)  = min over paths from any marker pixel to p inside `mask` of the MAX level on the path
                     (marker pixels have cost 0);
       2. dist(p)  = fewest steps from a marker along "tight" moves q->p, i.e. cost(p) == max(cost(q), level(p));
@@ -298,8 +310,7 @@ def minimax_watershed(prob, markers, mask, levels=256):
     Pixels outside `mask` or unreachable get 0.  prob: (H, W) float; markers: (H, W) int32 (0 = none);
     mask: (H, W) bool.  Returns int32 (H, W)."""
     H, W = prob.shape
-    lev = np.floor((1.0 - prob.astype(np.float64)) * (levels - 1)).astype(np.int64)
-    lev = np.clip(lev, 0, levels - 1)
+    lev = relief_levels(prob, levels)
     INF = np.int64(1 << 40)
     mask = mask.astype(bool) | (markers > 0)
     is_m = markers > 0
